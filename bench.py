@@ -1,17 +1,17 @@
 #!/usr/bin/env python
 """bench.py — MAGMA hot-path benchmark (BASELINE.json metric: image-caption samples/sec, fwd+bwd).
 
-  python bench.py --gpus N --steps K --warmup W            # B200-native arm (this repo's kernels)
+  python bench.py --gpus N --steps K --warmup W            # this repo's kernels (H100, sm_90a)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on host cores
 
 A "step" is one `train_step`: Magma.forward (CLIP ViT-L/14 -> ImagePrefix -> GPT-J-6B + MLP adapters -> LM head ->
 shifted CE) + backward (LM and encoder frozen: dgrad everywhere, wgrad for adapters/prefix) + gradient all-reduce
 (N > 1) + fused AdamW on the trainable set, at BASELINE.json config 2: batch 8 per GPU, 224x224, seq_len 128, bf16,
-random-init weights of the real architecture, synthetic data (SURVEY.md §8d).
+random-init weights of the real architecture, synthetic data.
 
 Prints ONE JSON line (rank 0). `value` = samples/s with inputs resident in HBM; `e2e` = the same through the public
 `train_step(config, loader, engine)` call with pinned HOST batches (H2D copy + loss D2H read inside the timed
-region). `roofline` is for the dominant kernel (the tcgen05 GEMM core): algorithmic FLOPs of its launches / the sum
+region). `roofline` is for the dominant kernel (the wgmma GEMM core): algorithmic FLOPs of its launches / the sum
 of their CUDA-event durations, measured in a second pass of the same steps with per-launch events enabled.
 """
 import argparse
@@ -28,7 +28,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 B_PER_GPU, S, RES = 8, 128, 224
-# algorithmic FLOPs / sample, fwd+bwd, LM + encoder frozen (BASELINE.md §4, SURVEY.md §8d)
+# algorithmic FLOPs / sample, fwd+bwd, LM + encoder frozen
 D, R_AD, V, NL = 4096, 1024, 50258, 28
 LM_FWD = NL * (24 * D * D + 4 * D * R_AD) * S + 2 * D * V * S + NL * 4 * S * S * D
 VIT_FWD = 24 * (24 * 1024 * 1024 * 257 + 4 * 257 * 257 * 1024) + 2 * 588 * 1024 * 256
@@ -40,7 +40,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", d.get("bf16_tflops")), d.get("hbm_gbs"), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense BF16, HBM3; 700 W card)"
 
 
 class ClockSampler:
@@ -254,7 +254,7 @@ def run_reference(args):
     return 0
 
 
-# BASELINE.json config 4 asks for an NFNet-F6 encoder, which the reference does not have (SURVEY.md fact 2: its conv
+# BASELINE.json config 4 asks for an NFNet-F6 encoder, which the reference does not have (its conv
 # encoders are timm nf_resnet50 and the CLIP ResNets) and this repo has not built; the conv-trunk hot path that IS built is
 # the encoder MAGMA_v1.yml actually ships, CLIP RN50x16 (`clip_resnet_large`) at its native 384 px. Its prefix is 144 tokens
 # (one per 12 x 12 position), which must fit inside seq_len (fact 3): 144 + 128 caption positions = 272.
@@ -269,14 +269,31 @@ def workload_config(n, note="", conv=False):
                             "(= 144 prefix + 128 caption positions), fwd+bwd+AdamW, LM and image encoder frozen (eval-mode "
                             "BatchNorm folded), random-init weights",
                 "global_batch": CONV["batch"] * n, "seq_len": CONV["seq"], "image": CONV["res"], "parallelism": f"dp{n}",
-                "l2": "working set per step (12.2 GB of bf16 weights streamed) exceeds the 126 MB L2; no explicit flush",
+                "l2": "working set per step (12.2 GB of bf16 weights streamed) exceeds the 50 MB L2; no explicit flush",
                 "note": note}
     return {"workload": "BASELINE.json config 2: CLIP ViT-L/14 (clip_vit_large, pooled -> image_seq_len 2) + GPT-J-6B "
                         "+ MLP adapters (normal, f=4), batch 8 per GPU, 224x224 images, seq_len 128, fwd+bwd+AdamW, "
                         "LM and image encoder frozen, random-init weights",
             "global_batch": B_PER_GPU * n, "seq_len": S, "image": RES, "parallelism": f"dp{n}",
-            "l2": "working set per step (12.2 GB of bf16 weights streamed) exceeds the 126 MB L2; no explicit flush",
+            "l2": "working set per step (12.2 GB of bf16 weights streamed) exceeds the 50 MB L2; no explicit flush",
             "note": note}
+
+
+def dump_outputs(out_dir, out):
+    """What the caller of the timed step receives from its last step: the loss and a fixed, seeded sample of the logits
+    (the full [B, S, vocab] tensor is ~200 MB in fp32), as float32 .npy files."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), out.loss.detach().float().reshape(1).cpu().numpy())
+    if out.logits is not None:
+        flat = out.logits.detach().reshape(-1)
+        n = min(flat.numel(), 1 << 22)  # 16 MB of fp32
+        idx = torch.randint(0, flat.numel(), (n,), generator=torch.Generator().manual_seed(0))
+        np.save(os.path.join(out_dir, "logits_sample.npy"), flat[idx.to(flat.device)].float().cpu().numpy())
+        last = out.logits.detach()[0, -1].float().cpu().numpy()  # every vocabulary entry of one position
+        np.save(os.path.join(out_dir, "logits_b0_last_position.npy"), last)
 
 
 def run_b200(args):
@@ -301,6 +318,7 @@ def run_b200(args):
                           adapter_config={"mlp": {"adapter_type": "normal", "downsample_factor": 4}}, image_seq_len=2,
                           image_embed_dropout_prob=0.1, use_image_embed_layernorm=True, image_size=Rw, seq_len=Sw,
                           gradient_accumulation_steps=1, freeze_img_encoder=True, lr=8e-4, lr_decay_iters=300000)
+    torch.manual_seed(0)  # adapters / image prefix draw their initial weights from torch's generator: same every run
     model = Magma(mc, device=dev, init_seed=0)
     model.train()
     engine = B200Engine(model, mc)
@@ -313,7 +331,7 @@ def run_b200(args):
         out = engine(images, captions)
         engine.backward(out.loss)
         engine.step()
-        return out.loss
+        return out
 
     def barrier():
         if world > 1:
@@ -330,7 +348,7 @@ def run_b200(args):
     # ---- device-resident timing (value) ----
     sampler = ClockSampler(local_rank) if rank == 0 else None  # running before the warm-up (see its docstring)
     for i in range(max(args.warmup, 3)):
-        loss = device_step(i)
+        device_step(i)
     barrier()
     if sampler:
         sampler.mark()
@@ -338,9 +356,12 @@ def run_b200(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(args.steps):
-        loss = device_step(i)
+        out = device_step(i)
     e1.record()
     barrier()
+    loss = out.loss
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     ms_mine = e0.elapsed_time(e1)
     ms_total = max_over_ranks(ms_mine)
     rank_ms = None
@@ -404,7 +425,7 @@ def run_b200(args):
         L.mb200_prof_enable(0)
         prof_step_ms = t_ev0.elapsed_time(t_ev1) / n_prof
         ach = fl.value / (ms.value / 1e3) / 1e12 if ms.value > 0 else 0.0
-        roof = {"kernel": "gemm_tcgen05_kernel / gemm2_tcgen05_kernel (all GEMM launches of the step)", "bound": "tensor",
+        roof = {"kernel": "gemm_wgmma_kernel (all GEMM launches of the step)", "bound": "tensor",
                 "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf, "traffic": None,
                 "peak_source": peak_src, "launches_per_step": n.value / n_prof,
                 "avg_launch_us": ms.value * 1e3 / max(n.value, 1),
@@ -418,29 +439,10 @@ def run_b200(args):
                 # FLOPs (every conv is a GEMM here) over the timed step
                 "step_algorithmic_tflops": (fl.value / n_prof if conv else FLOPS_PER_SAMPLE * Bw) / (ms_step / 1e3) / 1e12,
                 "step_frac_of_peak": (fl.value / n_prof if conv else FLOPS_PER_SAMPLE * Bw) / (ms_step / 1e3) / 1e12 / peak_tf}
-        tr = os.path.join(ROOT, "profiles", "gemm_dram_traffic.json")
-        if os.path.exists(tr) and not conv:  # the capture is of the config-2 step; the conv workload has other shapes
-            try:
-                tj = json.load(open(tr))
-                roof["traffic"] = tj.get("bytes_per_launch")
-                roof["traffic_source"] = (f"{tj.get('source')}: ncu dram__bytes_read.sum + dram__bytes_write.sum over "
-                                          f"{tj.get('gemm_launches')} GEMM launches of one step ({tj.get('note', '')}); "
-                                          f"algorithmic bytes per launch in this run: {by.value / max(n.value, 1):.0f}")
-            except Exception:
-                pass
-        tc = os.path.join(ROOT, "profiles", "gemm_tc_util.json")
-        if roof is not None and os.path.exists(tc) and not conv:
-            try:  # BASELINE.json's second figure ("GPT-J block TC util %"): an ncu capture, not measurable inside a timed run
-                tj = json.load(open(tc))
-                roof["tc_util_ncu"] = {"gptj_block_tensor_pipe_pct_of_active_cycles": tj["gptj_block_tensor_pipe_pct_of_active_cycles"],
-                                       "gptj_block_tensor_pipe_pct_of_elapsed_cycles": tj["gptj_block_tensor_pipe_pct_of_elapsed_cycles"],
-                                       "source": tj["source"]}
-            except Exception:
-                pass
     if world > 1:
         dist.barrier()
 
-    # ---- gradient exchange in isolation (N > 1): bytes, time and bus bandwidth of the arena all-reduce (SURVEY.md §8e);
+    # ---- gradient exchange in isolation (N > 1): bytes, time and bus bandwidth of the arena all-reduce;
     # measured AFTER the timed regions, never part of `value`. Any failure here leaves the field null.
     allreduce = None
     if world > 1:
@@ -519,7 +521,7 @@ def run_decode(args):
     tokens, 256 greedy autoregressive steps over a static KV cache. A "step" of this workload is ONE full generation
     (prefill + 256 decode steps); `value` = generated tokens/s with the prompt embeddings resident in HBM, `e2e` = the
     same through the public API from HOST inputs (pinned fp32 images + int64 prompt ids -> preprocess/embed -> generate ->
-    token ids back on the host). Replicas only for N > 1 (SURVEY.md section 8e: inference has no collective). Roofline:
+    token ids back on the host). Replicas only for N > 1 (inference has no collective). Roofline:
     HBM — algorithmic bytes of a decode step (bf16 weights 12.16 GB + the KV rows read) / its device time."""
     import torch
     import torch.distributed as dist
@@ -616,7 +618,7 @@ def run_decode(args):
                                        "(ViT-L/14 pooled -> 2 tokens) + 6 prompt tokens, 256 greedy steps, static KV cache, "
                                        "GPT-J-6B + MLP adapters f=4, random-init weights; one step = one full generation",
                            "global_batch": B * world, "prompt_len": s0, "new_tokens": n_new, "parallelism": f"replicas{world}",
-                           "l2": "12.2 GB of weights streamed per decode step exceed the 126 MB L2; no explicit flush"},
+                           "l2": "12.2 GB of weights streamed per decode step exceed the 50 MB L2; no explicit flush"},
                 "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roof, "cpu_baseline": None,
                 "tokens_head": out[0, s0:s0 + 8].tolist()}
         print(json.dumps(line), flush=True)
@@ -631,6 +633,9 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs (loss, seeded logits sample) as "
+                         "float32 .npy files into DIR")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-eager", action="store_true")
@@ -642,6 +647,8 @@ def main():
     if args.impl == "reference":
         return run_reference(args)
     if args.workload == "decode":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the outputs of the train / conv step; the decode workload has none")
         return run_decode(args)
     return run_b200(args)
 

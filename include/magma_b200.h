@@ -1,16 +1,16 @@
 /*
  * magma_b200 — C ABI of libmagma_b200.so
  *
- * B200-native (sm_100a) re-backing of the MAGMA forward/backward hot path. The reference
+ * Hopper-native (sm_90a) re-backing of the MAGMA forward/backward hot path. The reference
  * (Aleph-Alpha/magma) has no FFI layer of its own: its seams are Python factories and nn.Module
- * duck types (SURVEY.md §8b). Each entry point below names the reference call site whose arithmetic
+ * duck types. Each entry point below names the reference call site whose arithmetic
  * it replaces. All pointers are raw DEVICE pointers into caller-owned (PyTorch-owned) storage; the
  * library never allocates or frees tensor memory. All work is enqueued on the passed CUDA stream
  * (`void* stream` is a cudaStream_t); no entry point synchronises the device unless stated.
  *
  * Return value: 0 on success, negative MB200_E_* on failure; mb200_last_error() returns a
  * thread-local message. Nothing throws across this boundary. There is no CPU fallback: every
- * compute entry point refuses to run (MB200_E_ARCH) unless the current device is sm_100.
+ * compute entry point refuses to run (MB200_E_ARCH) unless the current device is sm_90.
  */
 #ifndef MAGMA_B200_H_
 #define MAGMA_B200_H_
@@ -54,7 +54,7 @@ enum {
 
 int mb200_version(void);
 const char* mb200_last_error(void);
-/* 0 when the current CUDA device is sm_100 (B200), MB200_E_ARCH otherwise. */
+/* 0 when the current CUDA device is sm_90 (H100), MB200_E_ARCH otherwise. */
 int mb200_check_device(void);
 /* Limit the persistent GEMM grids to n_sms SMs (0 = all, the default; also env MB200_GEMM_SMS). Data-parallel training
  * may leave a few SMs free for NCCL's CTAs so the gradient all-reduce overlaps the backward GEMMs. Returns the limit in
@@ -63,7 +63,7 @@ int mb200_set_gemm_sm_limit(int n_sms);
 /* Cap the grids of the optimizer kernels (mb200_sumsq, mb200_adamw_step) at n_blocks blocks of 256 threads (0 = the
  * default, 16 blocks per SM). With 2 blocks per SM they fit in the registers a persistent GEMM CTA leaves free, so an
  * optimizer step issued on a side stream runs BESIDE the next step's frozen-encoder GEMMs instead of owning every SM
- * until it is done (B200Engine, DESIGN.md section 3.10). Returns the cap in effect. */
+ * until it is done (B200Engine). Returns the cap in effect. */
 int mb200_set_optimizer_grid(int n_blocks);
 /* number of kernels this library has launched since load (bench.py reports the delta as gpu_launches). */
 long long mb200_launch_count(void);
@@ -73,7 +73,7 @@ int mb200_prof_enable(int on);
 int mb200_prof_read(double* gemm_ms, double* gemm_flops, double* gemm_bytes, long long* gemm_launches);
 
 /* -------------------------------------------------------------------------------------------
- * GEMM core (tcgen05.mma + TMEM accumulators + TMA operand staging, persistent, warp-specialised)
+ * GEMM core (wgmma.mma_async + register accumulators + TMA operand staging, persistent, warp-specialised)
  *
  *   C[b][M,N] = epilogue( alpha * A[b][M,K] * B[b][N,K]^T )
  *

@@ -1,4 +1,4 @@
-"""magma_b200 — B200-native (sm_100a) re-backing of the MAGMA forward/backward hot path.
+"""magma_b200 — Hopper-native (sm_90a) re-backing of the MAGMA forward/backward hot path.
 
 The top-level names mirror `magma/__init__.py` of the reference (`from magma import Magma` -> `from magma_b200 import
 Magma`); they resolve lazily so that `import magma_b200` (e.g. by the build script) does not pull in torch."""

@@ -1,6 +1,6 @@
 """ctypes loader for libmagma_b200.so (the C ABI declared in include/magma_b200.h).
 
-There is deliberately no fallback: if the shared library is missing or the device is not sm_100 every
+There is deliberately no fallback: if the shared library is missing or the device is not sm_90 every
 compute entry point raises. PyTorch is used only for device memory and streams.
 """
 import ctypes

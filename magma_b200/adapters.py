@@ -1,5 +1,5 @@
 """Adapter modules — drop-in for magma/adapters.py (same class names, constructor signatures and state-dict
-keys `adapter.{0,2}.{weight,bias}`), re-backed by the tcgen05 GEMM core.
+keys `adapter.{0,2}.{weight,bias}`), re-backed by the wgmma GEMM core.
 
 Inside the LM the adapters are executed by the C++ GPT-J runtime (csrc/gptj_sched.cu), which discovers them through the
 same `block.mlp` / `block.attn` rewiring the reference performs (magma/magma.py:128-169). `forward` below is the

@@ -1,8 +1,8 @@
-"""Build libmagma_b200.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Build libmagma_b200.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc.
 
 `python -m magma_b200.build` or `magma_b200.build.build()`. nvcc cross-compiles without a GPU, so this
 is also the CPU-side "does it build" check run by `__graft_entry__.build()`. The built library lands in
-`magma_b200/lib/` (git-ignored, but shipped to the GPU box by gpurun).
+`magma_b200/lib/` (git-ignored build products).
 """
 import os
 import subprocess
@@ -16,7 +16,7 @@ OBJDIR = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(LIBDIR, "libmagma_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -45,7 +45,7 @@ def _compile_one(src, verbose):
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu under csrc/ for sm_100a and link libmagma_b200.so. Returns the library path."""
+    """Compile every .cu under csrc/ for sm_90a and link libmagma_b200.so. Returns the library path."""
     os.makedirs(OBJDIR, exist_ok=True)
     srcs = _sources()
     hdr_m = _headers_mtime()

@@ -1,4 +1,4 @@
-"""Checkpoint key adapter (SURVEY.md §8f rank 2) for `Magma.from_checkpoint` (magma/magma.py:278-301).
+"""Checkpoint key adapter for `Magma.from_checkpoint` (magma/magma.py:278-301).
 
 The published MAGMA checkpoint (`mp_rank_00_model_states.pt["module"]`, README.md:74) was written by the reference
 with the finetuneanon/transformers GPT-Neo(jax, rotary) fork as the LM, whose parameter names differ from the HF GPT-J

@@ -2,19 +2,21 @@
 // (S <= 128 — BASELINE.json config 2 has S = 128), head_dim a multiple of 64 up to 256.
 //
 // Replaces, per layer, the 3 (forward) / 6 (backward) launches of the GEMM-based path of the schedules — QK^T GEMM,
-// softmax kernel, PV GEMM; dP, dV, softmax-bwd, dQ, dK GEMMs — which spend most of their ~12-18 us each on fixed
-// launch / prologue / epilogue cost for 0.5 % of the step's FLOPs. Numerics are those of the reference
+// softmax kernel, PV GEMM; dP, dV, softmax-bwd, dQ, dK GEMMs — which spend most of their time on fixed launch /
+// prologue / epilogue cost for 0.5 % of the step's FLOPs. Numerics are those of the reference
 // (GPTJAttention._attn, hf:gptj/modeling_gptj.py:136-149): fp32 scores from bf16 q,k, / sqrt(hd), causal mask,
 // fp32 softmax, probabilities rounded to bf16 before P*V; the backward uses the saved bf16 P.
 //
-// Forward, 128 threads (thread t <-> query row t <-> TMEM lane t):
+// 256 threads = two warpgroups; warpgroup w owns rows [64 w, 64 w + 64) of every 128-row product and holds them as a
+// wgmma accumulator fragment (wgmma.cuh): a row is spread over the 4 threads of a quad, so row reductions (softmax
+// maximum and sum, rowsum(dP * P)) are two quad shuffles.
+// Forward:
 //   TMA: Q, K ([S, hd] K-major, hd/64 boxes of 128x64) and V -> smem (SWIZZLE_128B)
-//   S = Q K^T      tcgen05.mma 128x128xhd  -> TMEM cols [0,128)
-//   softmax in registers (one row per thread, no shuffles); P -> bf16 -> smem (UMMA K-major layout) and -> global
-//   O = P V        tcgen05.mma 128xhdx128 (V as MN-major B operand: same bytes as its K-major tile)  -> TMEM [256,256+hd)
-//   O -> bf16 -> global [B,S,H,hd]
-// Backward, 128 threads:
-//   dP = dO V^T ; dV = P^T dO (P, dO as MN-major operands: same smem bytes) ; dS = P*(dP - rowsum(dP*P))/sqrt(hd)
+//   S = Q K^T      wgmma 64x128xhd per warpgroup
+//   softmax in registers; P -> bf16 -> smem (K-major operand layout) and -> global
+//   O = P V        wgmma 64xhdx128 (V as MN-major B operand: same bytes as its K-major tile) -> bf16 -> global
+// Backward:
+//   dP = dO V^T ; dS = P*(dP - rowsum(dP*P))/sqrt(hd) ; dV = P^T dO (P, dO as MN-major operands: same smem bytes)
 //   dQ = dS K ; dK = dS^T Q, both with the inverse rotary rotation applied on the way out (they are gradients of the
 //   rotated q,k), written straight into the fused dqkv buffer.
 #include <stdlib.h>
@@ -23,7 +25,7 @@
 
 namespace mb200 {
 
-static constexpr int kAttThreads = 128;
+static constexpr int kAttThreads = 256;
 static constexpr int kTile = 128 * 64 * 2;  // one 128-row x 64-col bf16 box = 16 KB
 
 struct AttnParams {
@@ -41,31 +43,38 @@ struct AttnParams {
 };
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// the 128 threads of warpgroup `wg` meet (named barriers 1 and 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
-// write 8 consecutive bf16 (one 16-byte chunk j of k-block kb) of row r into a K-major SWIZZLE_128B operand tile
-__device__ __forceinline__ void st_operand_chunk(uint32_t tile_base, int r, int kb, int j, uint4 v) {
-  const uint32_t a = tile_base + (uint32_t)(kb * kTile + r * 128 + ((j ^ (r & 7)) << 4));
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+// byte offset of element (r, c) in a K-major SWIZZLE_128B operand tile made of 16 KB [128 rows x 64 cols] k-blocks
+__device__ __forceinline__ uint32_t operand_off(int r, int c) {
+  return (uint32_t)((c >> 6) * kTile + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2);
+}
+__device__ __forceinline__ void st_pair(uint32_t saddr, float a, float b) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(f32x2_to_bf16(a, b)) : "memory");
+}
+__device__ __forceinline__ float2 ld_pair(uint32_t saddr) {
+  uint32_t u;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(saddr));
+  return bf16x2_to_f32(u);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-__device__ __forceinline__ uint4 pack8f(const float* f) {
-  uint4 u;
-  __nv_bfloat162 h0 = __floats2bfloat162_rn(f[0], f[1]), h1 = __floats2bfloat162_rn(f[2], f[3]);
-  __nv_bfloat162 h2 = __floats2bfloat162_rn(f[4], f[5]), h3 = __floats2bfloat162_rn(f[6], f[7]);
-  u.x = *reinterpret_cast<uint32_t*>(&h0);
-  u.y = *reinterpret_cast<uint32_t*>(&h1);
-  u.z = *reinterpret_cast<uint32_t*>(&h2);
-  u.w = *reinterpret_cast<uint32_t*>(&h3);
-  return u;
-}
-
-// issue the k-steps of one 128 x N x (nkb*64) product. A/B tiles are sequences of 16 KB k-blocks (K-major) or of
-// 16 KB 64-wide MN chunks holding 128 k-rows each (MN-major).
-template <bool A_MN, bool B_MN>
-__device__ __forceinline__ void issue_mma(uint32_t d_tmem, uint32_t a_base, uint32_t b_base, int nkb, int N,
-                                          uint32_t acc0 = 0u) {  // acc0 != 0: accumulate onto what D already holds
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+// D[64 rows of warpgroup wg] = A * B over nkb k-blocks of 64. A / B tiles are sequences of 16 KB k-blocks (K-major) or of
+// 16 KB 64-wide MN chunks holding 128 k-rows each (MN-major). The warpgroup's rows of A are rows 64 wg.. of each k-block
+// (K-major) or MN chunk wg (MN-major). Returns with the products complete.
+template <int N, bool A_MN, bool B_MN>
+__device__ __forceinline__ void wg_mma(float (&d)[N / 2], int wg, uint32_t a_base, uint32_t b_base, int nkb,
+                                       uint32_t acc0 = 0u) {
+  a_base += A_MN ? (uint32_t)(wg * kTile) : (uint32_t)(wg * 64 * 128);
+  wgmma_fence();
   for (int kb = 0; kb < nkb; ++kb) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -75,7 +84,46 @@ __device__ __forceinline__ void issue_mma(uint32_t d_tmem, uint32_t a_base, uint
       const uint32_t bo = B_MN ? (uint32_t)((kb * 4 + k) * 2048) : (uint32_t)(kb * kTile + k * 32);
       const uint64_t da = make_smem_desc(a_base + ao, A_MN ? (uint32_t)kTile : 0u, 1024);
       const uint64_t db = make_smem_desc(b_base + bo, B_MN ? (uint32_t)kTile : 0u, 1024);
-      umma_bf16(d_tmem, da, db, idesc, ((kb | k) != 0 ? 1u : 0u) | acc0);
+      wgmma_bf16<N, A_MN ? 1 : 0, B_MN ? 1 : 0>(d, da, db, ((kb | k) != 0 ? 1u : 0u) | acc0);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+}
+
+// fragment coordinates of this thread: rows r0 and r0 + 8 of the warpgroup's 64, columns 8 j + c0 + {0, 1}
+struct Frag {
+  int wg, r0, c0, quad0;
+  __device__ __forceinline__ Frag() {
+    const int t = threadIdx.x;
+    wg = t >> 7;
+    r0 = wg * 64 + ((t & 127) >> 5) * 16 + ((t & 31) >> 2);
+    c0 = 2 * (t & 3);
+    quad0 = (t & 3) == 0;
+  }
+};
+
+// store a 64 x HD fragment as bf16 rows dst + row * ld (rows >= nrows skipped), with the inverse rotary rotation of the
+// first `rot` columns when tab != nullptr (row r uses position r)
+template <int HD>
+__device__ __forceinline__ void store_rows(const Frag& f, const float (&d)[HD / 2], bf16* dst, long long ld, int nrows,
+                                           const float2* tab, int rot) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = f.r0 + 8 * h;
+    if (r >= nrows) continue;
+    bf16* row = dst + (long long)r * ld;
+#pragma unroll
+    for (int j = 0; j < HD / 8; ++j) {
+      const int c = 8 * j + f.c0;
+      float a0 = d[4 * j + 2 * h], a1 = d[4 * j + 2 * h + 1];
+      if (tab != nullptr && c < rot) {
+        const float2 cs = __ldg(tab + (long long)r * (rot >> 1) + (c >> 1));
+        const float b0 = a0 * cs.x + a1 * cs.y;  // transpose of [[c, -s], [s, c]]
+        a1 = a1 * cs.x - a0 * cs.y;
+        a0 = b0;
+      }
+      *reinterpret_cast<uint32_t*>(row + c) = f32x2_to_bf16(a0, a1);
     }
   }
 }
@@ -83,12 +131,13 @@ __device__ __forceinline__ void issue_mma(uint32_t d_tmem, uint32_t a_base, uint
 // ---------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------
+template <int HD>
 __global__ void __launch_bounds__(kAttThreads, 1)
 attn_fwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nhb = p.hd >> 6;  // 64-wide head-dim blocks
+  constexpr int nhb = HD / 64;  // 64-wide head-dim blocks
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + nhb * kTile;
   uint8_t* sV = sK + nhb * kTile;
@@ -96,27 +145,20 @@ attn_fwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kTile);
   uint64_t* bar_qk = bars + 0;
   uint64_t* bar_v = bars + 1;
-  uint64_t* bar_s = bars + 2;
-  uint64_t* bar_o = bars + 3;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 4);
 
-  const int t = threadIdx.x, warp = t >> 5;
+  const int t = threadIdx.x;
   const int h = blockIdx.x % p.H, b = blockIdx.x / p.H;
+  const Frag f;
 
   pdl_trigger();
   if (t == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-    for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
+    for (int i = 0; i < 2; ++i) mbar_init(&bars[i], 1);
     mbar_fence_init();
   }
-  __syncwarp();
-  if (warp == 0) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
   pdl_wait();
 
   if (t == 0) {
@@ -127,122 +169,64 @@ attn_fwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     }
     mbar_expect_tx(bar_v, nhb * kTile);
     for (int kb = 0; kb < nhb; ++kb) tma_load_4d(sV + kb * kTile, &tmV, bar_v, kb * 64, 0, h, b);
-    mbar_wait(bar_qk, 0);
-    tc_fence_after();
-    issue_mma<false, false>(tmem, smem_u32(sQ), smem_u32(sK), nhb, 128);  // S = Q K^T
-    umma_commit(bar_s);
   }
-  // ---- softmax: thread t owns query row t ----
-  mbar_wait(bar_s, 0);
-  tc_fence_after();
-  float s[128];
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    uint32_t rr[32];
-    tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(c * 32), rr);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) s[c * 32 + j] = __uint_as_float(rr[j]) * p.scale;
-  }
-  const int lim = min(p.S, t + 1);  // causal: keys 0..t
-  float m = -INFINITY;
-#pragma unroll
-  for (int j = 0; j < 128; ++j)
-    if (j < lim) m = fmaxf(m, s[j]);
-  float sum = 0.f;
-#pragma unroll
-  for (int j = 0; j < 128; ++j) {
-    s[j] = j < lim ? __expf(s[j] - m) : 0.f;
-    sum += s[j];
-  }
-  const float inv = t < p.S ? 1.f / sum : 0.f;
-  bf16* prow = p.P + (((long long)b * p.H + h) * p.S + t) * p.ldP;
+  mbar_wait(bar_qk, 0);
+  float s[64];
+  wg_mma<128, false, false>(s, f.wg, smem_u32(sQ), smem_u32(sK), nhb);  // S = Q K^T
   const uint32_t sP_s = smem_u32(sP);
 #pragma unroll
-  for (int kb = 0; kb < 2; ++kb) {
+  for (int hh = 0; hh < 2; ++hh) {
+    const int q = f.r0 + 8 * hh;
+    const int lim = min(p.S, q + 1);  // causal: keys 0..q
+    float m = -INFINITY;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float f[8];
+    for (int j = 0; j < 16; ++j)
 #pragma unroll
-      for (int e = 0; e < 8; ++e) f[e] = s[kb * 64 + j * 8 + e] * inv;
-      const uint4 u = pack8f(f);
-      st_operand_chunk(sP_s, t, kb, j, u);
-      const int col = kb * 64 + j * 8;
-      if (t < p.S && col < p.ldP) *reinterpret_cast<uint4*>(prow + col) = u;  // saved for backward (ldP % 8 == 0)
+      for (int e = 0; e < 2; ++e) {
+        float& v = s[4 * j + 2 * hh + e];
+        v *= p.scale;
+        if (8 * j + f.c0 + e < lim) m = fmaxf(m, v);
+      }
+    m = quad_max(m);
+    float sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float& v = s[4 * j + 2 * hh + e];
+        v = 8 * j + f.c0 + e < lim ? __expf(v - m) : 0.f;
+        sum += v;
+      }
+    sum = quad_sum(sum);
+    const float inv = q < p.S ? 1.f / sum : 0.f;
+    bf16* prow = p.P + (((long long)b * p.H + h) * p.S + q) * p.ldP;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = 8 * j + f.c0;
+      const float a0 = s[4 * j + 2 * hh] * inv, a1 = s[4 * j + 2 * hh + 1] * inv;
+      st_pair(sP_s + operand_off(q, c), a0, a1);
+      if (q < p.S && c < p.ldP) *reinterpret_cast<uint32_t*>(prow + c) = f32x2_to_bf16(a0, a1);  // saved for backward
     }
   }
   fence_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  tc_fence_before();
-  __syncthreads();
-  if (t == 0) {
-    tc_fence_after();
-    mbar_wait(bar_v, 0);
-    issue_mma<false, true>(tmem + 256, sP_s, smem_u32(sV), 2, p.hd);  // O = P V   (K = 128 keys)
-    umma_commit(bar_o);
-  }
-  mbar_wait(bar_o, 0);
-  tc_fence_after();
-  bf16* orow = p.O + ((long long)b * p.S + t) * p.ldo + (long long)h * p.hd;
-  for (int c = 0; c < p.hd / 32; ++c) {
-    uint32_t rr[32];
-    tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(256 + c * 32), rr);
-    tmem_ld_wait();
-    if (t < p.S) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(rr[j + e]);
-        *reinterpret_cast<uint4*>(orow + c * 32 + j) = pack8f(f);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem);
-  }
+  wg_sync(f.wg);       // this warpgroup's rows of P are complete
+  mbar_wait(bar_v, 0);
+  float o[HD / 2];
+  wg_mma<HD, false, true>(o, f.wg, sP_s, smem_u32(sV), 2);  // O = P V   (K = 128 keys)
+  store_rows<HD>(f, o, p.O + (long long)b * p.S * p.ldo + (long long)h * HD, p.ldo, p.S, nullptr, 0);
 }
 
 // ---------------------------------------------------------------------------------------------
 // backward
 // ---------------------------------------------------------------------------------------------
-// store one gradient row (thread's TMEM lane) of width hd into dst, optionally applying the inverse rotary rotation
-__device__ __forceinline__ void store_grad_row(uint32_t taddr, bf16* dst, int hd, bool valid, const float2* tab_row,
-                                               int rot) {
-  for (int c = 0; c < hd / 32; ++c) {
-    uint32_t rr[32];
-    tmem_ld_32x32(taddr + (uint32_t)(c * 32), rr);
-    tmem_ld_wait();
-    if (valid) {
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(rr[j]);
-      if (tab_row != nullptr && c * 32 < rot) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          if (c * 32 + j < rot) {
-            const float2 cs = __ldg(tab_row + ((c * 32 + j) >> 1));
-            const float a0 = f[j], a1 = f[j + 1];
-            f[j] = a0 * cs.x + a1 * cs.y;      // transpose of [[c, -s], [s, c]]
-            f[j + 1] = a1 * cs.x - a0 * cs.y;
-          }
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) *reinterpret_cast<uint4*>(dst + c * 32 + j) = pack8f(f + j);
-    }
-  }
-}
-
+template <int HD>
 __global__ void __launch_bounds__(kAttThreads, 1)
 attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
                      const __grid_constant__ CUtensorMap tmP, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nhb = p.hd >> 6;
+  constexpr int nhb = HD / 64;
   uint8_t* R1 = smem;                 // dO, later Q
   uint8_t* R2 = R1 + nhb * kTile;     // V, later K
   uint8_t* R3 = R2 + nhb * kTile;     // P   (2 k-blocks)
@@ -250,16 +234,12 @@ attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   uint64_t* bars = reinterpret_cast<uint64_t*>(R4 + 2 * kTile);
   uint64_t* bar_a = bars + 0;   // dO + V landed
   uint64_t* bar_p = bars + 1;   // P landed
-  uint64_t* bar_1 = bars + 2;   // dP done
-  uint64_t* bar_2 = bars + 3;   // dV done (and dP)
-  uint64_t* bar_k = bars + 4;   // K landed
-  uint64_t* bar_q = bars + 5;   // Q landed
-  uint64_t* bar_3 = bars + 6;   // dQ done
-  uint64_t* bar_4 = bars + 7;   // dK done
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* bar_k = bars + 2;   // K landed
+  uint64_t* bar_q = bars + 3;   // Q landed
 
-  const int t = threadIdx.x, warp = t >> 5;
+  const int t = threadIdx.x;
   const int h = blockIdx.x % p.H, b = blockIdx.x / p.H;
+  const Frag f;
 
   pdl_trigger();
   if (t == 0) {
@@ -268,16 +248,10 @@ attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmdO);
     tma_prefetch_desc(&tmP);
-    for (int i = 0; i < 8; ++i) mbar_init(&bars[i], 1);
+    for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
     mbar_fence_init();
   }
-  __syncwarp();
-  if (warp == 0) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-  const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
   pdl_wait();
 
   if (t == 0) {
@@ -288,98 +262,58 @@ attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     }
     mbar_expect_tx(bar_p, 2 * kTile);
     for (int kb = 0; kb < 2; ++kb) tma_load_4d(R3 + kb * kTile, &tmP, bar_p, kb * 64, 0, h, b);
-    mbar_wait(bar_a, 0);
-    tc_fence_after();
-    issue_mma<false, false>(tmem, smem_u32(R1), smem_u32(R2), nhb, 128);  // dP[q,k] = dO V^T
-    umma_commit(bar_1);
-    mbar_wait(bar_p, 0);
-    tc_fence_after();
-    issue_mma<true, true>(tmem + 256, smem_u32(R3), smem_u32(R1), 2, p.hd);  // dV[k,:] = P^T dO  (K = queries)
-    umma_commit(bar_2);
   }
-  // ---- dS: thread t owns query row t ----
-  mbar_wait(bar_1, 0);
-  tc_fence_after();
+  const uint32_t R3_s = smem_u32(R3), R4_s = smem_u32(R4);
   {
-    const bf16* prow = p.P + (((long long)b * p.H + h) * p.S + t) * p.ldP;
-    const uint32_t dS_s = smem_u32(R4);
-    float acc = 0.f;
-    // two passes over the row in 32-column chunks (TMEM re-reads are cheap; keeps the row out of registers):
-    // pass 0 accumulates sum_j dP*P, pass 1 forms dS = P * (dP - sum) / sqrt(hd) and writes the operand tile
-#pragma unroll 1
-    for (int pass = 0; pass < 2; ++pass) {
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t rr[32];
-        tmem_ld_32x32(lane_addr + (uint32_t)(c * 32), rr);
-        tmem_ld_wait();
-        float pr[32];
+    mbar_wait(bar_a, 0);
+    float dp[64];
+    wg_mma<128, false, false>(dp, f.wg, smem_u32(R1), smem_u32(R2), nhb);  // dP[q,k] = dO V^T
+    // ---- dS = P * (dP - rowsum(dP * P)) / sqrt(hd); P as loaded by TMA (zeros beyond S) ----
+    mbar_wait(bar_p, 0);
 #pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          const int col = c * 32 + j;
-          uint4 u = make_uint4(0, 0, 0, 0);
-          if (t < p.S && col < p.ldP) u = *reinterpret_cast<const uint4*>(prow + col);
-          const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&u);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q = f.r0 + 8 * hh;
+      float acc = 0.f;
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 f = __bfloat1622float2(hh[e]);
-            pr[j + 2 * e] = (col + 2 * e < p.S) ? f.x : 0.f;
-            pr[j + 2 * e + 1] = (col + 2 * e + 1 < p.S) ? f.y : 0.f;
-          }
-        }
-        if (pass == 0) {
+      for (int j = 0; j < 16; ++j) {
+        const float2 pr = ld_pair(R3_s + operand_off(q, 8 * j + f.c0));
+        acc += dp[4 * j + 2 * hh] * pr.x + dp[4 * j + 2 * hh + 1] * pr.y;
+      }
+      acc = quad_sum(acc);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) acc += __uint_as_float(rr[j]) * pr[j];
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = pr[j + e] * (__uint_as_float(rr[j + e]) - acc) * p.scale;
-            const int col = c * 32 + j;
-            st_operand_chunk(dS_s, t, col >> 6, (col & 63) >> 3, pack8f(f));
-          }
-        }
+      for (int j = 0; j < 16; ++j) {
+        const uint32_t off = operand_off(q, 8 * j + f.c0);
+        const float2 pr = ld_pair(R3_s + off);
+        st_pair(R4_s + off, pr.x * (dp[4 * j + 2 * hh] - acc) * p.scale, pr.y * (dp[4 * j + 2 * hh + 1] - acc) * p.scale);
       }
     }
   }
+  const long long HDall = (long long)p.H * HD;
+  bf16* gbase = p.dqkv + (long long)b * p.S * p.ld_dqkv + (long long)h * HD;
+  {
+    float dv[HD / 2];
+    wg_mma<HD, true, true>(dv, f.wg, R3_s, smem_u32(R1), 2);  // dV[k,:] = P^T dO  (K = queries)
+    store_rows<HD>(f, dv, gbase + 2 * HDall, p.ld_dqkv, p.S, nullptr, 0);
+  }
   fence_async_smem();
-  // ---- dV rows (thread t <-> key row t) ----
-  mbar_wait(bar_2, 0);
-  tc_fence_after();
+  __syncthreads();  // dS complete in smem (all rows); dO and V no longer read by either warpgroup
   if (t == 0) {
-    // dO and V are no longer read by the tensor core: stream K over V and Q over dO while dV drains
     mbar_expect_tx(bar_k, nhb * kTile);
     for (int kb = 0; kb < nhb; ++kb) tma_load_4d(R2 + kb * kTile, &tmK, bar_k, kb * 64, 0, h, b);
     mbar_expect_tx(bar_q, nhb * kTile);
     for (int kb = 0; kb < nhb; ++kb) tma_load_4d(R1 + kb * kTile, &tmQ, bar_q, kb * 64, 0, h, b);
   }
-  const long long grow = ((long long)b * p.S + t) * p.ld_dqkv + (long long)h * p.hd;
-  const long long HD = (long long)p.H * p.hd;
-  store_grad_row(lane_addr + 256, p.dqkv + grow + 2 * HD, p.hd, t < p.S, nullptr, 0);
-  tc_fence_before();
-  __syncthreads();  // dS complete in smem (all rows), dP and dV TMEM regions drained by every thread
-  if (t == 0) {
-    tc_fence_after();
+  {
     mbar_wait(bar_k, 0);
-    issue_mma<false, true>(tmem, smem_u32(R4), smem_u32(R2), 2, p.hd);  // dQ[q,:] = dS K      (K = keys)
-    umma_commit(bar_3);
-    mbar_wait(bar_q, 0);
-    issue_mma<true, true>(tmem + 256, smem_u32(R4), smem_u32(R1), 2, p.hd);  // dK[k,:] = dS^T Q  (K = queries)
-    umma_commit(bar_4);
+    float dq[HD / 2];
+    wg_mma<HD, false, true>(dq, f.wg, R4_s, smem_u32(R2), 2);  // dQ[q,:] = dS K      (K = keys)
+    store_rows<HD>(f, dq, gbase, p.ld_dqkv, p.S, p.rope_tab, p.rot);
   }
-  const float2* tab_row = p.rope_tab ? p.rope_tab + (long long)t * (p.rot >> 1) : nullptr;
-  mbar_wait(bar_3, 0);
-  tc_fence_after();
-  store_grad_row(lane_addr, p.dqkv + grow, p.hd, t < p.S, tab_row, p.rot);
-  mbar_wait(bar_4, 0);
-  tc_fence_after();
-  store_grad_row(lane_addr + 256, p.dqkv + grow + HD, p.hd, t < p.S, tab_row, p.rot);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem);
+  {
+    mbar_wait(bar_q, 0);
+    float dk[HD / 2];
+    wg_mma<HD, true, true>(dk, f.wg, R4_s, smem_u32(R1), 2);  // dK[k,:] = dS^T Q  (K = queries)
+    store_rows<HD>(f, dk, gbase + HDall, p.ld_dqkv, p.S, p.rope_tab, p.rot);
   }
 }
 
@@ -390,12 +324,12 @@ attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 // softmax over the WHOLE key row in fp32, probabilities rounded to bf16 before P*V — hf:gptj/modeling_gptj.py:136-149,
 // hf:clip/modeling_clip.py:282-330), obtained with two sweeps over the key tiles instead of an online rescale:
 //   sweep 1: S_j = Q K_j^T per 128-key tile, running row maximum m and sum l = sum exp(s - m)          (no V, no O)
-//   sweep 2: S_j again, p = bf16(exp(s - m) / l) exactly as the materialised path rounds it, O += P_j V_j in TMEM
-// so O never needs rescaling (no TMEM read-modify-write of a 128 x hd fp32 tile) and P — when the caller wants it for
-// the backward pass — is bit-identical to what softmax_fwd_kernel would have written. QK^T is computed twice: +50 % of
-// the attention FLOPs, which are < 1 % of the step (S = 128 .. 2048), in exchange for no [B,H,S,S] fp32 score buffer.
-// K / V tiles are double-buffered (TMA of tile j+1 under the softmax of tile j) when head_dim <= 128; at head_dim 256
-// one buffer each fits next to Q and P (224 KB) and the next tile is prefetched into L2 instead.
+//   sweep 2: S_j again, p = bf16(exp(s - m) / l) exactly as the materialised path rounds it, O += P_j V_j in registers
+// so O never needs rescaling and P — when the caller wants it for the backward pass — is bit-identical to what
+// softmax_fwd_kernel would have written. QK^T is computed twice: +50 % of the attention FLOPs, which are < 1 % of the
+// step, in exchange for no [B,H,S,S] fp32 score buffer. K / V tiles are double-buffered (TMA of tile j+1 under the
+// softmax of tile j) when head_dim <= 128; at head_dim 256 one buffer each fits next to Q and P (224 KB) and the next
+// tile is prefetched into L2 instead.
 struct FlashParams {
   int Sq, Sk, H, hd, causal, kv_off;  // key j visible to query i iff j < Sk and (!causal or j <= i + kv_off)
   float scale;
@@ -406,13 +340,13 @@ struct FlashParams {
   float2* stats;       // optional [B,H,Sq] (row max of the scaled scores, 1 / sum)
 };
 
-template <int NBUF>
+template <int HD, int NBUF>
 __global__ void __launch_bounds__(kAttThreads, 1)
 attn_fwd_flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, const FlashParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nhb = p.hd >> 6;
+  constexpr int nhb = HD / 64;
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + nhb * kTile;            // NBUF buffers
   uint8_t* sV = sK + NBUF * nhb * kTile;     // NBUF buffers
@@ -421,33 +355,20 @@ attn_fwd_flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   uint64_t* bar_q = bars + 0;
   uint64_t* bar_k = bars + 1;   // [2]
   uint64_t* bar_v = bars + 3;   // [2]
-  uint64_t* bar_s = bars + 5;
-  uint64_t* bar_o = bars + 6;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 7);
 
-  const int t = threadIdx.x, warp = t >> 5;
+  const int t = threadIdx.x;
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
-  const int qi = q0 + t;  // this thread's query row
+  const Frag f;
 
   pdl_trigger();
   if (t == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-    for (int i = 0; i < 7; ++i) mbar_init(&bars[i], 1);
+    for (int i = 0; i < 5; ++i) mbar_init(&bars[i], 1);
     mbar_fence_init();
   }
-  __syncwarp();
-  if (warp == 0) {
-    if (NBUF == 2) tmem_alloc<256>(tmem_ptr);
-    else tmem_alloc<512>(tmem_ptr);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-  const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-  const uint32_t tmem_o = tmem + 128;
   pdl_wait();
 
   // key tiles this query tile looks at
@@ -456,10 +377,16 @@ attn_fwd_flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const int last_key = min(p.Sk - 1, q0 + 127 + p.kv_off);
     n_kv = last_key < 0 ? 0 : min(n_kv, (last_key >> 7) + 1);
   }
-  const int row_lim = !p.causal ? p.Sk : min(p.Sk, qi + p.kv_off + 1);  // keys [0, row_lim) are visible to this row
-  const bool row_ok = qi < p.Sq;
+  int row_lim[2];  // keys [0, row_lim) are visible to this thread's two rows
+  bool row_ok[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qi = q0 + f.r0 + 8 * hh;
+    row_lim[hh] = !p.causal ? p.Sk : min(p.Sk, qi + p.kv_off + 1);
+    row_ok[hh] = qi < p.Sq;
+  }
 
-  uint32_t ph_k[2] = {0, 0}, ph_v[2] = {0, 0}, ph_s = 0, ph_o = 0;
+  uint32_t ph_k[2] = {0, 0}, ph_v[2] = {0, 0};
   auto load_k = [&](int j, int buf) {
     mbar_expect_tx(&bar_k[buf], nhb * kTile);
     for (int kb = 0; kb < nhb; ++kb) tma_load_4d(sK + (buf * nhb + kb) * kTile, &tmK, &bar_k[buf], kb * 64, j * 128, h, b);
@@ -470,325 +397,118 @@ attn_fwd_flash_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   };
 
   // ---------------- sweep 1: row maximum and sum ----------------
-  float m = -INFINITY, l = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   if (t == 0 && n_kv > 0) {
     mbar_expect_tx(bar_q, nhb * kTile);
     for (int kb = 0; kb < nhb; ++kb) tma_load_4d(sQ + kb * kTile, &tmQ, bar_q, kb * 64, q0, h, b);
     load_k(0, 0);
-    mbar_wait(bar_q, 0);
   }
+  if (n_kv > 0) mbar_wait(bar_q, 0);
+  float s[64];
   for (int j = 0; j < n_kv; ++j) {
     const int buf = NBUF == 2 ? (j & 1) : 0;
     if (t == 0) {
-      if (NBUF == 2 && j + 1 < n_kv) load_k(j + 1, (j + 1) & 1);  // its previous user (tile j-1) has completed (bar_s)
+      if (NBUF == 2 && j + 1 < n_kv) load_k(j + 1, (j + 1) & 1);  // its previous user (tile j-1) has completed
       if (NBUF == 1 && j + 1 < n_kv)
         for (int kb = 0; kb < nhb; ++kb) tma_prefetch_4d(&tmK, kb * 64, (j + 1) * 128, h, b);
-      mbar_wait(&bar_k[buf], ph_k[buf]);
-      tc_fence_after();
-      issue_mma<false, false>(tmem, smem_u32(sQ), smem_u32(sK + buf * nhb * kTile), nhb, 128);
-      umma_commit(bar_s);
     }
+    mbar_wait(&bar_k[buf], ph_k[buf]);
     ph_k[buf] ^= 1;
-    mbar_wait(bar_s, ph_s);
-    ph_s ^= 1;
-    tc_fence_after();
-    if (NBUF == 1 && t == 0 && j + 1 < n_kv) load_k(j + 1, 0);  // the single K buffer is free once S_j is complete
+    wg_mma<128, false, false>(s, f.wg, smem_u32(sQ), smem_u32(sK + buf * nhb * kTile), nhb);
+    __syncthreads();  // both warpgroups are done with K_j
+    if (NBUF == 1 && t == 0 && j + 1 < n_kv) load_k(j + 1, 0);
     const int kbase = j * 128;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t rr[32];
-      tmem_ld_32x32(lane_addr + (uint32_t)(c * 32), rr);
-      tmem_ld_wait();
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
       float cm = -INFINITY;
 #pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        const float sv = __uint_as_float(rr[e]) * p.scale;
-        if (kbase + c * 32 + e < row_lim) cm = fmaxf(cm, sv);
-      }
-      if (cm > m) {  // rescale the running sum to the new maximum
-        l *= __expf(m - cm);
-        m = cm;
-      }
-      if (m != -INFINITY) {
+      for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          const float sv = __uint_as_float(rr[e]) * p.scale;
-          if (kbase + c * 32 + e < row_lim) l += __expf(sv - m);
-        }
+        for (int e = 0; e < 2; ++e)
+          if (kbase + 8 * jj + f.c0 + e < row_lim[hh]) cm = fmaxf(cm, s[4 * jj + 2 * hh + e] * p.scale);
+      cm = quad_max(cm);
+      if (cm > m[hh]) {  // rescale the running sum to the new maximum
+        l[hh] *= __expf(m[hh] - cm);
+        m[hh] = cm;
+      }
+      if (m[hh] != -INFINITY) {
+        float ls = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (kbase + 8 * jj + f.c0 + e < row_lim[hh]) ls += __expf(s[4 * jj + 2 * hh + e] * p.scale - m[hh]);
+        l[hh] += quad_sum(ls);
       }
     }
-    tc_fence_before();
-    __syncthreads();  // every row of S_j has been read: the next QK^T may overwrite it
-    tc_fence_after();
   }
-  const float inv = (row_ok && l > 0.f) ? 1.f / l : 0.f;
-  if (m == -INFINITY) m = 0.f;
-  if (p.stats != nullptr && row_ok) p.stats[((long long)b * p.H + h) * p.Sq + qi] = make_float2(m, inv);
+  float inv[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    inv[hh] = (row_ok[hh] && l[hh] > 0.f) ? 1.f / l[hh] : 0.f;
+    if (m[hh] == -INFINITY) m[hh] = 0.f;
+    if (p.stats != nullptr && row_ok[hh] && f.quad0)
+      p.stats[((long long)b * p.H + h) * p.Sq + q0 + f.r0 + 8 * hh] = make_float2(m[hh], inv[hh]);
+  }
 
   // ---------------- sweep 2: probabilities and O = P V ----------------
-  bf16* prow = p.P ? p.P + (((long long)b * p.H + h) * p.Sq + qi) * p.ldP : nullptr;
   const uint32_t sP_s = smem_u32(sP);
   if (t == 0 && n_kv > 0) {
-    load_k(0, 0);  // (NBUF == 1: the buffer's last reader was S_{n_kv-1}, complete; NBUF == 2: buffer 0's last load was
-    load_v(0, 0);  //  consumed in sweep 1 unless n_kv is even — either way its MMA has completed)
+    load_k(0, 0);  // buffer 0's last user completed before the last __syncthreads of sweep 1
+    load_v(0, 0);
   }
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   for (int j = 0; j < n_kv; ++j) {
     const int buf = NBUF == 2 ? (j & 1) : 0;
     if (t == 0) {
       if (NBUF == 2 && j + 1 < n_kv) {
         load_k(j + 1, (j + 1) & 1);
-        load_v(j + 1, (j + 1) & 1);   // V_{j-1} (same buffer) was consumed by the PV of tile j-1: bar_o waited below
+        load_v(j + 1, (j + 1) & 1);   // V_{j-1} (same buffer) was consumed by the PV of tile j-1 (synchronised below)
       }
       if (NBUF == 1 && j + 1 < n_kv)
         for (int kb = 0; kb < nhb; ++kb) {
           tma_prefetch_4d(&tmK, kb * 64, (j + 1) * 128, h, b);
           tma_prefetch_4d(&tmV, kb * 64, (j + 1) * 128, h, b);
         }
-      mbar_wait(&bar_k[buf], ph_k[buf]);
-      tc_fence_after();
-      issue_mma<false, false>(tmem, smem_u32(sQ), smem_u32(sK + buf * nhb * kTile), nhb, 128);
-      umma_commit(bar_s);
     }
+    mbar_wait(&bar_k[buf], ph_k[buf]);
     ph_k[buf] ^= 1;
-    mbar_wait(bar_s, ph_s);
-    ph_s ^= 1;
-    tc_fence_after();
+    wg_mma<128, false, false>(s, f.wg, smem_u32(sQ), smem_u32(sK + buf * nhb * kTile), nhb);
+    __syncthreads();  // both warpgroups are done with K_j
     if (NBUF == 1 && t == 0 && j + 1 < n_kv) load_k(j + 1, 0);
     const int kbase = j * 128;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t rr[32];
-      tmem_ld_32x32(lane_addr + (uint32_t)(c * 32), rr);
-      tmem_ld_wait();
 #pragma unroll
-      for (int g8 = 0; g8 < 4; ++g8) {
-        float f[8];
+    for (int hh = 0; hh < 2; ++hh) {
+      const int r = f.r0 + 8 * hh;
+      bf16* prow = p.P ? p.P + (((long long)b * p.H + h) * p.Sq + q0 + r) * p.ldP : nullptr;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int key = kbase + c * 32 + g8 * 8 + e;
-          f[e] = key < row_lim ? __expf(__uint_as_float(rr[g8 * 8 + e]) * p.scale - m) * inv : 0.f;
-        }
-        const uint4 u = pack8f(f);
-        const int col = c * 32 + g8 * 8;
-        st_operand_chunk(sP_s, t, col >> 6, (col & 63) >> 3, u);
-        if (prow != nullptr && row_ok && kbase + col < p.ldP) *reinterpret_cast<uint4*>(prow + kbase + col) = u;
+      for (int jj = 0; jj < 16; ++jj) {
+        const int c = 8 * jj + f.c0;
+        float a[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          a[e] = kbase + c + e < row_lim[hh] ? __expf(s[4 * jj + 2 * hh + e] * p.scale - m[hh]) * inv[hh] : 0.f;
+        st_pair(sP_s + operand_off(r, c), a[0], a[1]);
+        if (prow != nullptr && row_ok[hh] && kbase + c < p.ldP)
+          *reinterpret_cast<uint32_t*>(prow + kbase + c) = f32x2_to_bf16(a[0], a[1]);
       }
     }
     fence_async_smem();
-    tc_fence_before();
-    __syncthreads();  // P_j complete in smem; S_j fully read
-    if (t == 0) {
-      tc_fence_after();
-      mbar_wait(&bar_v[buf], ph_v[buf]);
-      tc_fence_after();
-      issue_mma<false, true>(tmem_o, sP_s, smem_u32(sV + buf * nhb * kTile), 2, p.hd, j > 0 ? 1u : 0u);  // O += P_j V_j
-      umma_commit(bar_o);
-    }
+    wg_sync(f.wg);  // this warpgroup's rows of P_j are complete
+    mbar_wait(&bar_v[buf], ph_v[buf]);
     ph_v[buf] ^= 1;
-    // P (smem) and, with one buffer, V are reused by the next tile: wait for this PV before going on
-    mbar_wait(bar_o, ph_o);
-    ph_o ^= 1;
-    tc_fence_after();
+    wg_mma<HD, false, true>(o, f.wg, sP_s, smem_u32(sV + buf * nhb * kTile), 2, 1u);  // O += P_j V_j
+    __syncthreads();  // both warpgroups are done with V_j (and with this P_j)
     if (NBUF == 1 && t == 0 && j + 1 < n_kv) load_v(j + 1, 0);
   }
   // ---------------- O -> bf16 -> global ----------------
-  bf16* orow = p.O + ((long long)b * p.Sq + qi) * p.ldo + (long long)h * p.hd;
-  for (int c = 0; c < p.hd / 32; ++c) {
-    uint32_t rr[32];
-    if (n_kv > 0) {
-      tmem_ld_32x32(lane_addr + (uint32_t)(128 + c * 32), rr);
-      tmem_ld_wait();
-    } else {
-#pragma unroll
-      for (int e = 0; e < 32; ++e) rr[e] = 0u;
-    }
-    if (row_ok) {
-#pragma unroll
-      for (int e = 0; e < 32; e += 8) {
-        float f[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) f[k] = __uint_as_float(rr[e + k]);
-        *reinterpret_cast<uint4*>(orow + c * 32 + e) = pack8f(f);
-      }
-    }
-  }
+  store_rows<HD>(f, o, p.O + ((long long)b * p.Sq + q0) * p.ldo + (long long)h * HD, p.ldo, p.Sq - q0, nullptr, 0);
   // rows of P beyond this tile's last key tile (causal) are zeros in the materialised layout
-  if (prow != nullptr && row_ok) {
+  if (p.P != nullptr && t < 128 && q0 + t < p.Sq) {
+    bf16* prow = p.P + (((long long)b * p.H + h) * p.Sq + q0 + t) * p.ldP;
     for (int col = n_kv * 128; col < p.ldP; col += 8) *reinterpret_cast<uint4*>(prow + col) = make_uint4(0, 0, 0, 0);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    if (NBUF == 2) tmem_dealloc<256>(tmem);
-    else tmem_dealloc<512>(tmem);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// short-key forward: the WHOLE key range (Sk <= 384 at head_dim 64, <= 256 at head_dim 128) resident on chip
-// ---------------------------------------------------------------------------------------------
-// The ViT case (T = 257 keys, head_dim 64, no mask; 24 layers x B x 16 heads per step). The two-sweep kernel above is a
-// chain of ~18 dependent TMA / MMA / softmax round trips per CTA for three key tiles (measured 94 us per launch at
-// B = 8: profiles/r02_launches_step_flash_v1_summary.txt — no faster than the GEMM + softmax + GEMM path it replaced).
-// Here Q, every K tile and every V tile are loaded at once, the NKT score tiles are issued back to back into NKT x 128
-// TMEM columns behind ONE commit, each thread (= query row) makes three passes over its row in TMEM — maximum;
-// e = exp(s - max) written back in place with tcgen05.st, and the sum; p = bf16(e / sum) into the P operand tiles — and
-// the NKT P V products accumulate behind one more commit: 3 synchronisation points per CTA. Same rounding points as the
-// materialised softmax (fp32 scores, fp32 exp / sum, probabilities rounded to bf16 before P V).
-template <int NKT>
-__global__ void __launch_bounds__(kAttThreads, 1)
-attn_fwd_short_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                      const __grid_constant__ CUtensorMap tmV, const FlashParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nhb = p.hd >> 6;
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + nhb * kTile;             // NKT tiles
-  uint8_t* sV = sK + NKT * nhb * kTile;       // NKT tiles
-  uint8_t* sP = sV + NKT * nhb * kTile;       // NKT x 2 k-blocks of 64 keys
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + NKT * 2 * kTile);
-  uint64_t* bar_qk = bars + 0;
-  uint64_t* bar_v = bars + 1;
-  uint64_t* bar_s = bars + 2;
-  uint64_t* bar_o = bars + 3;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 4);
-
-  const int t = threadIdx.x, warp = t >> 5;
-  const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
-  const int qi = q0 + t;
-
-  pdl_trigger();
-  if (t == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
-    mbar_fence_init();
-  }
-  __syncwarp();
-  if (warp == 0) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-  const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-  const uint32_t tmem_o = tmem + 384;
-  pdl_wait();
-
-  if (t == 0) {
-    mbar_expect_tx(bar_qk, (1 + NKT) * nhb * kTile);
-    for (int kb = 0; kb < nhb; ++kb) tma_load_4d(sQ + kb * kTile, &tmQ, bar_qk, kb * 64, q0, h, b);
-    for (int j = 0; j < NKT; ++j)
-      for (int kb = 0; kb < nhb; ++kb) tma_load_4d(sK + (j * nhb + kb) * kTile, &tmK, bar_qk, kb * 64, j * 128, h, b);
-    mbar_expect_tx(bar_v, NKT * nhb * kTile);
-    for (int j = 0; j < NKT; ++j)
-      for (int kb = 0; kb < nhb; ++kb) tma_load_4d(sV + (j * nhb + kb) * kTile, &tmV, bar_v, kb * 64, j * 128, h, b);
-    mbar_wait(bar_qk, 0);
-    tc_fence_after();
-#pragma unroll
-    for (int j = 0; j < NKT; ++j)
-      issue_mma<false, false>(tmem + (uint32_t)(j * 128), smem_u32(sQ), smem_u32(sK + j * nhb * kTile), nhb, 128);
-    umma_commit(bar_s);
-  }
-  const int row_lim = !p.causal ? p.Sk : min(p.Sk, qi + p.kv_off + 1);  // keys [0, row_lim) are visible to this row
-  const bool row_ok = qi < p.Sq;
-  mbar_wait(bar_s, 0);
-  tc_fence_after();
-  // (tcgen05.ld / .st are warp-collective: every loop bound and branch around them below is warp-uniform; what differs
-  // per row — the causal limit — only masks values)
-  const int nch = min(NKT * 4, (p.Sk + 31) >> 5);  // 32-column chunks that contain keys
-  // pass 1: row maximum
-  float m = -INFINITY;
-#pragma unroll 1
-  for (int c = 0; c < nch; ++c) {
-    uint32_t rr[32];
-    tmem_ld_32x32(lane_addr + (uint32_t)(c * 32), rr);
-    tmem_ld_wait();
-#pragma unroll
-    for (int e = 0; e < 32; ++e)
-      if (c * 32 + e < row_lim) m = fmaxf(m, __uint_as_float(rr[e]) * p.scale);
-  }
-  if (m == -INFINITY) m = 0.f;
-  // pass 2: e = exp(s - max) written back in place, and the sum
-  float l = 0.f;
-#pragma unroll 1
-  for (int c = 0; c < NKT * 4; ++c) {
-    uint32_t rr[32];
-    if (c < nch) {
-      tmem_ld_32x32(lane_addr + (uint32_t)(c * 32), rr);
-      tmem_ld_wait();
-#pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        const float ev = c * 32 + e < row_lim ? __expf(__uint_as_float(rr[e]) * p.scale - m) : 0.f;
-        l += ev;
-        rr[e] = __float_as_uint(ev);
-      }
-    } else {
-#pragma unroll
-      for (int e = 0; e < 32; ++e) rr[e] = 0u;
-    }
-    tmem_st_32x32(lane_addr + (uint32_t)(c * 32), rr);
-  }
-  tmem_st_wait();
-  const float inv = (row_ok && l > 0.f) ? 1.f / l : 0.f;
-  if (p.stats != nullptr && row_ok) p.stats[((long long)b * p.H + h) * p.Sq + qi] = make_float2(m, inv);
-  // pass 3: probabilities -> bf16 -> P operand tiles (and global P when asked for)
-  bf16* prow = p.P ? p.P + (((long long)b * p.H + h) * p.Sq + qi) * p.ldP : nullptr;
-  const uint32_t sP_s = smem_u32(sP);
-#pragma unroll 1
-  for (int c = 0; c < NKT * 4; ++c) {
-    uint32_t rr[32];
-    tmem_ld_32x32(lane_addr + (uint32_t)(c * 32), rr);
-    tmem_ld_wait();
-#pragma unroll
-    for (int g8 = 0; g8 < 4; ++g8) {
-      float f[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(rr[g8 * 8 + e]) * inv;
-      const uint4 u = pack8f(f);
-      const int col = c * 32 + g8 * 8;  // key index
-      st_operand_chunk(sP_s + (uint32_t)((col >> 7) * 2 * kTile), t, (col & 127) >> 6, (col & 63) >> 3, u);
-      if (prow != nullptr && row_ok && col < p.ldP) *reinterpret_cast<uint4*>(prow + col) = u;
-    }
-  }
-  if (prow != nullptr && row_ok)
-    for (int col = NKT * 128; col < p.ldP; col += 8) *reinterpret_cast<uint4*>(prow + col) = make_uint4(0, 0, 0, 0);
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  if (t == 0) {
-    tc_fence_after();
-    mbar_wait(bar_v, 0);
-    tc_fence_after();
-#pragma unroll
-    for (int j = 0; j < NKT; ++j)
-      issue_mma<false, true>(tmem_o, sP_s + (uint32_t)(j * 2 * kTile), smem_u32(sV + j * nhb * kTile), 2, p.hd,
-                             j > 0 ? 1u : 0u);
-    umma_commit(bar_o);
-  }
-  mbar_wait(bar_o, 0);
-  tc_fence_after();
-  bf16* orow = p.O + ((long long)b * p.Sq + qi) * p.ldo + (long long)h * p.hd;
-  for (int c = 0; c < p.hd / 32; ++c) {
-    uint32_t rr[32];
-    tmem_ld_32x32(lane_addr + (uint32_t)(384 + c * 32), rr);
-    tmem_ld_wait();
-    if (row_ok) {
-#pragma unroll
-      for (int e = 0; e < 32; e += 8) {
-        float f[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) f[k] = __uint_as_float(rr[e + k]);
-        *reinterpret_cast<uint4*>(orow + c * 32 + e) = pack8f(f);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem);
   }
 }
 
@@ -806,6 +526,8 @@ static int tile_map(CUtensorMap* m, const void* ptr, long long ld, long long bs0
   op.static_data = 0;
   return make_operand_map(m, op, rows, cols, H, B, 128);
 }
+
+static constexpr int smem_max = 232448;  // 227 KB: the sm_90 per-block opt-in limit
 
 bool attn_tile_supported(int S, int hd) { return S >= 1 && S <= 128 && hd >= 64 && hd <= 256 && hd % 64 == 0; }
 
@@ -829,12 +551,22 @@ int attn_fwd_tile(const bf16* qkv, long long ld_qkv, bf16* P, long long ldP, bf1
   p.O = O;
   p.ldo = ldo;
   const int smem = (3 * (hd / 64) + 2) * kTile + 1024 + 128;
-  static bool set = false;
-  if (!set) {
-    MB_CUDA(cudaFuncSetAttribute(attn_fwd_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    set = true;
+#define MB_FWD(HD)                                                                                                   \
+  {                                                                                                                  \
+    static bool set = false;                                                                                         \
+    if (!set) {                                                                                                      \
+      MB_CUDA(cudaFuncSetAttribute(attn_fwd_tile_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)); \
+      set = true;                                                                                                    \
+    }                                                                                                                \
+    MB_CUDA(launch_pdl(attn_fwd_tile_kernel<HD>, dim3(B * H), dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, p));  \
   }
-  MB_CUDA(launch_pdl(attn_fwd_tile_kernel, dim3(B * H), dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, p));
+  switch (hd) {
+    case 64: MB_FWD(64) break;
+    case 128: MB_FWD(128) break;
+    case 192: MB_FWD(192) break;
+    default: MB_FWD(256) break;
+  }
+#undef MB_FWD
   count_launch();
   return 0;
 }
@@ -864,12 +596,23 @@ int attn_bwd_tile(const bf16* qkv, long long ld_qkv, const bf16* dO, long long l
   p.ld_dqkv = ld_dqkv;
   p.rope_tab = reinterpret_cast<const float2*>(rope_tab);
   const int smem = (2 * (hd / 64) + 4) * kTile + 1024 + 128;
-  static bool set = false;
-  if (!set) {
-    MB_CUDA(cudaFuncSetAttribute(attn_bwd_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    set = true;
+#define MB_BWD(HD)                                                                                                   \
+  {                                                                                                                  \
+    static bool set = false;                                                                                         \
+    if (!set) {                                                                                                      \
+      MB_CUDA(cudaFuncSetAttribute(attn_bwd_tile_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)); \
+      set = true;                                                                                                    \
+    }                                                                                                                \
+    MB_CUDA(launch_pdl(attn_bwd_tile_kernel<HD>, dim3(B * H), dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, tdo,  \
+                       tp, p));                                                                                      \
   }
-  MB_CUDA(launch_pdl(attn_bwd_tile_kernel, dim3(B * H), dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, tdo, tp, p));
+  switch (hd) {
+    case 64: MB_BWD(64) break;
+    case 128: MB_BWD(128) break;
+    case 192: MB_BWD(192) break;
+    default: MB_BWD(256) break;
+  }
+#undef MB_BWD
   count_launch();
   return 0;
 }
@@ -909,48 +652,26 @@ int attn_fwd_flash(const bf16* q, long long ldq, long long q_bsh, long long q_bs
   p.P = P;
   p.ldP = ldP;
   p.stats = reinterpret_cast<float2*>(stats);
-  const int nhb = hd / 64;
   const dim3 grid((Sq + 127) / 128, H, B);
-  // short key ranges (the ViT: 257 keys, head_dim 64) stay entirely on chip: one pass, three synchronisation points
-  const int nkt = (Sk + 127) / 128;
-  static int use_short = -1;
-  if (use_short < 0) {
-    const char* e = getenv("MB200_ATTN_SHORT");
-    use_short = e ? atoi(e) : 1;
-  }
-  if (use_short && ((hd == 64 && nkt <= 3) || (hd == 128 && nkt <= 2))) {
-    const int smem = ((1 + 2 * nkt) * nhb + 2 * nkt) * kTile + 1024 + 128;
-#define MB_SHORT(NK)                                                                                                 \
+  // K / V double-buffered up to head_dim 128; one buffer each at 192 / 256 (smem)
+#define MB_FLASH(HD, NB)                                                                                             \
   {                                                                                                                  \
+    const int smem = ((1 + 2 * NB) * (HD / 64) + 2) * kTile + 1024 + 128;                                           \
     static bool set = false;                                                                                         \
     if (!set) {                                                                                                      \
-      MB_CUDA(cudaFuncSetAttribute(attn_fwd_short_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448)); \
+      MB_CUDA(cudaFuncSetAttribute(attn_fwd_flash_kernel<HD, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
+                                   smem_max));                                                                       \
       set = true;                                                                                                    \
     }                                                                                                                \
-    MB_CUDA(launch_pdl(attn_fwd_short_kernel<NK>, grid, dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, p));        \
+    MB_CUDA(launch_pdl(attn_fwd_flash_kernel<HD, NB>, grid, dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, p));    \
   }
-    if (nkt == 1) MB_SHORT(1) else if (nkt == 2) MB_SHORT(2) else MB_SHORT(3)
-#undef MB_SHORT
-    count_launch();
-    return 0;
+  switch (hd) {
+    case 64: MB_FLASH(64, 2) break;
+    case 128: MB_FLASH(128, 2) break;
+    case 192: MB_FLASH(192, 1) break;
+    default: MB_FLASH(256, 1) break;
   }
-  if (hd <= 128) {
-    const int smem = (5 * nhb + 2) * kTile + 1024 + 128;
-    static bool set = false;
-    if (!set) {
-      MB_CUDA(cudaFuncSetAttribute(attn_fwd_flash_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-      set = true;
-    }
-    MB_CUDA(launch_pdl(attn_fwd_flash_kernel<2>, grid, dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, p));
-  } else {
-    const int smem = (3 * nhb + 2) * kTile + 1024 + 128;
-    static bool set = false;
-    if (!set) {
-      MB_CUDA(cudaFuncSetAttribute(attn_fwd_flash_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-      set = true;
-    }
-    MB_CUDA(launch_pdl(attn_fwd_flash_kernel<1>, grid, dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, p));
-  }
+#undef MB_FLASH
   count_launch();
   return 0;
 }

@@ -27,14 +27,14 @@ int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
 
 // SMs the persistent GEMM kernels may occupy (0 = all). Data-parallel training can leave a few SMs to NCCL's CTAs so the
-// gradient all-reduce overlaps the backward GEMMs instead of waiting for gaps between them (DESIGN.md §4).
+// gradient all-reduce overlaps the backward GEMMs instead of waiting for gaps between them.
 static int g_gemm_sm_limit = -1;
 int gemm_sms() {
   if (g_gemm_sm_limit < 0) {
@@ -66,8 +66,8 @@ int check_arch() {
       set_error("no usable CUDA device (%s); magma_b200 has no CPU fallback", cudaGetErrorString(e));
       return MB200_E_ARCH;
     }
-    if (major != 10) {
-      set_error("device compute capability %d.x is not sm_100; magma_b200 kernels are sm_100a only", major);
+    if (major != 9) {
+      set_error("device compute capability %d.x is not sm_90; magma_b200 kernels are sm_90a (Hopper) only", major);
       return MB200_E_ARCH;
     }
     cached = 0;

@@ -634,7 +634,7 @@ __global__ void peer_reduce_bcast_kernel(PeerBufs bufs, int world, long long off
 // Deterministic: per-block partial sums land in a fixed slot each and the LAST block to finish adds them in a fixed order
 // — every data-parallel rank holds bit-identical gradients after the all-reduce and must derive the bit-identical clipping
 // coefficient from them, or the replicas' parameters drift apart by an ulp per step (an atomicAdd of the block sums, the
-// previous version, is order-dependent in its last bits; tests/test_dp_gpu.py caught exactly that on 2 B200s).
+// previous version, is order-dependent in its last bits; tests/test_dp_gpu.py caught exactly that on 2 GPUs).
 static constexpr int kSumsqMaxBlocks = 2048;
 __device__ float g_sumsq_part[kSumsqMaxBlocks];
 __device__ unsigned int g_sumsq_ticket = 0;

@@ -1,19 +1,18 @@
-// magma_b200 — bf16 GEMM core for sm_100a.
+// magma_b200 — bf16 GEMM core for sm_90a (Hopper).
 //
 //   C[b][M,N] = epilogue(alpha * A[b][M,K] * B[b][N,K]^T)
 //
-// Design (B200-first, not a translation of anything in the reference, which only calls cuBLAS through
-// torch.nn.Linear — e.g. magma/adapters.py:19-23, magma/image_prefix.py:72):
+// Design (not a translation of anything in the reference, which only calls cuBLAS through torch.nn.Linear — e.g.
+// magma/adapters.py:19-23, magma/image_prefix.py:72):
 //   * persistent grid (<= one CTA per SM), static round-robin tile scheduler, m-fastest tile order so
-//     CTAs that run concurrently share the same weight (B) tile through the 126 MB L2;
-//   * warp-specialised: warp 0 = TMA producer (one lane), warp 1 = tcgen05.mma issuer (one lane),
-//     warp 2 = TMEM allocator, warps 4..7 = epilogue (TMEM -> registers -> fused epilogue -> HBM);
+//     CTAs that run concurrently share the same weight (B) tile through L2;
+//   * warp-specialised: warpgroup 0 = TMA producer (one lane), warpgroups 1 and 2 = consumers, each owning 64 rows of
+//     the 128-row tile: wgmma.mma_async m64nBNk16 with fp32 accumulators in registers, then the fused epilogue
+//     straight from the accumulator fragment (gemm_common.cuh);
 //   * operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a multi-stage smem ring,
-//     completion tracked with mbarriers; smem slots are released by tcgen05.commit;
-//   * fp32 accumulators live in TMEM, double-buffered (2 x BN columns) so the epilogue of tile i
-//     overlaps the MMAs of tile i+1;
-//   * both operand majors (K-major and MN-major) are supported through the UMMA shared-memory
-//     descriptors, so dgrad (dY*W) and wgrad (dY^T*X) read the original tensors — no transposes.
+//     completion tracked with mbarriers; a consumer releases a slot once the wgmma reading it has retired;
+//   * both operand majors (K-major and MN-major) are supported through the wgmma shared-memory descriptors and the
+//     transpose bits, so dgrad (dY*W) and wgrad (dY^T*X) read the original tensors — no transposes.
 #include <mutex>
 #include <stdlib.h>
 
@@ -21,12 +20,11 @@
 
 namespace mb200 {
 
-template <int BN, bool A_MN, bool B_MN, typename OutT, int AROWS = BM>
+template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ GemmKernelParams p) {
-  static_assert(AROWS == BM || !A_MN, "the 32-row A ring is only implemented for K-major A");
-  using C_ = Cfg<BN, AROWS>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ GemmKernelParams p) {
+  using C_ = Cfg<BN>;
   constexpr int kStages = C_::kStages;
 
   extern __shared__ uint8_t smem_raw[];
@@ -34,48 +32,32 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * C_::kABytes;
-  float* epi_stage = reinterpret_cast<float*>(smem + kStages * C_::kStageBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * C_::kStageBytes + C_::kEpiBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * C_::kStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int num_kb = (p.K + BK - 1) / BK;
+  const int items = p.total_tiles * p.split_k;
 
   pdl_trigger();  // the next kernel may start its prologue on SMs as they become free
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
     mbar_fence_init();
   }
-  if (warp == 2) {
-    tmem_alloc<C_::kTmemCols>(tmem_ptr_smem);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();  // everything above overlapped the previous kernel; global memory is touched only from here on
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int w = blockIdx.x; w < p.total_tiles * p.split_k; w += gridDim.x) {
+      for (int w = blockIdx.x; w < items; w += gridDim.x) {
         const int t = w / p.split_k, ks = w - t * p.split_k;
         const int kb0 = ks * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
         const int tpb = p.tiles_m * p.tiles_n;
@@ -84,28 +66,25 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const int m_blk = r % p.tiles_m;
         const int n_blk = r / p.tiles_m;
         const int z0 = z % p.nb0, z1 = z / p.nb0;
-        for (int kb = kb0; kb < kb1; kb += C_::kKS) {
-          const int nsub = min(C_::kKS, kb1 - kb);  // k-blocks carried by this stage
+        for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], (uint32_t)(nsub * (C_::kASub + C_::kBSub)));
-          for (int j = 0; j < nsub; ++j) {
-            uint8_t* sa = smem_a + stage * C_::kABytes + j * C_::kASub;
-            uint8_t* sb = smem_b + stage * C_::kBBytes + j * C_::kBSub;
-            const int kc = (kb + j) * BK;
-            if constexpr (A_MN) {
+          mbar_expect_tx(&full_bar[stage], (uint32_t)C_::kStageBytes);
+          uint8_t* sa = smem_a + stage * C_::kABytes;
+          uint8_t* sb = smem_b + stage * C_::kBBytes;
+          const int kc = kb * BK;
+          if constexpr (A_MN) {
 #pragma unroll
-              for (int i = 0; i < BM / 64; ++i)
-                tma_load_4d(sa + i * 8192, &tmA, &full_bar[stage], m_blk * BM + i * 64, kc, z0, z1);
-            } else {
-              tma_load_4d(sa, &tmA, &full_bar[stage], kc, m_blk * BM, z0, z1);
-            }
-            if constexpr (B_MN) {
+            for (int i = 0; i < BM / 64; ++i)
+              tma_load_4d(sa + i * 8192, &tmA, &full_bar[stage], m_blk * BM + i * 64, kc, z0, z1);
+          } else {
+            tma_load_4d(sa, &tmA, &full_bar[stage], kc, m_blk * BM, z0, z1);
+          }
+          if constexpr (B_MN) {
 #pragma unroll
-              for (int i = 0; i < BN / 64; ++i)
-                tma_load_4d(sb + i * 8192, &tmB, &full_bar[stage], n_blk * BN + i * 64, kc, z0, z1);
-            } else {
-              tma_load_4d(sb, &tmB, &full_bar[stage], kc, n_blk * BN, z0, z1);
-            }
+            for (int i = 0; i < BN / 64; ++i)
+              tma_load_4d(sb + i * 8192, &tmB, &full_bar[stage], n_blk * BN + i * 64, kc, z0, z1);
+          } else {
+            tma_load_4d(sb, &tmB, &full_bar[stage], kc, n_blk * BN, z0, z1);
           }
           if (++stage == kStages) {
             stage = 0;
@@ -114,112 +93,56 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (single thread) =====================
-    if (lane == 0) {
-      // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=bf16, majors, N>>3, M>>4
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) |
-                             ((B_MN ? 1u : 0u) << 16) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      // K-major SW128: 8-row atoms of 128 B rows -> SBO = 1024, LBO unused; advance K by 16 elems = 32 B.
-      // MN-major SW128: atom = 64 MN-elements (128 B) x 8 k-rows; SBO = 1024 between k-groups of 8,
-      //                 LBO = 8192 between 64-wide MN chunks (one TMA box each); advance K by 16 rows = 2048 B.
-      constexpr uint32_t a_lbo = A_MN ? 8192u : 0u, b_lbo = B_MN ? 8192u : 0u;
-      constexpr uint32_t a_kadv = A_MN ? 2048u : 32u, b_kadv = B_MN ? 2048u : 32u;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int w = blockIdx.x; w < p.total_tiles * p.split_k; w += gridDim.x, ++it) {
-        const int ks = w % p.split_k;
-        const int kb0 = ks * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; kb += C_::kKS) {
-          const int nsub = min(C_::kKS, kb1 - kb);
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          for (int j = 0; j < nsub; ++j) {
-            const uint32_t sa = smem_u32(smem_a + stage * C_::kABytes + j * C_::kASub);
-            const uint32_t sb = smem_u32(smem_b + stage * C_::kBBytes + j * C_::kBSub);
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t da = make_smem_desc(sa + k * a_kadv, a_lbo, 1024);
-              const uint64_t db = make_smem_desc(sb + k * b_kadv, b_lbo, 1024);
-              umma_bf16(d_tmem, da, db, idesc, ((kb - kb0) | j | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs have read it
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue warps =====================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    int it = 0;
-    for (int w = blockIdx.x; w < p.total_tiles * p.split_k; w += gridDim.x, ++it) {
-      const int t = w / p.split_k;
+  } else {
+    // ===================== consumers: wgmma + epilogue =====================
+    const int cw = wg - 1;  // rows [64 cw, 64 cw + 64) of the tile
+    const bool leader = (threadIdx.x & 127) == 0;
+    // K-major SW128: 8-row atoms of 128 B rows -> SBO = 1024, LBO unused; advance K by 16 elems = 32 B; this
+    //                warpgroup's 64 rows of A start 64 x 128 B into the slot.
+    // MN-major SW128: atom = 64 MN-elements (128 B) x 8 k-rows; SBO = 1024 between k-groups of 8,
+    //                 LBO = 8192 between 64-wide MN chunks (one TMA box each); advance K by 16 rows = 2048 B;
+    //                 this warpgroup's 64 rows of A are the cw-th box.
+    constexpr uint32_t b_lbo = B_MN ? 8192u : 0u;
+    constexpr uint32_t a_kadv = A_MN ? 2048u : 32u, b_kadv = B_MN ? 2048u : 32u;
+    const uint32_t a_off = (uint32_t)cw * 8192u;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int w = blockIdx.x; w < items; w += gridDim.x) {
+      const int t = w / p.split_k, ks = w - t * p.split_k;
+      const int kb0 = ks * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
       const int tpb = p.tiles_m * p.tiles_n;
       const int z = t / tpb;
       const int r = t - z * tpb;
       const int m_blk = r % p.tiles_m;
       const int n_blk = r / p.tiles_m;
       const int z0 = z % p.nb0, z1 = z / p.nb0;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      EpiCtx c;
-      c.tmem_acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-      c.stg_s = smem_u32(epi_stage + q * (32 * C_::kEpiPitch));
-      c.tmem_full = &tmem_full[acc];
-      c.tmem_empty = &tmem_empty[acc];
-      c.empty_remote = 0;
-      c.ks = w - t * p.split_k;
-      c.full_phase = acc_phase;
-      c.boff = (long long)z0 * p.c_bs0 + (long long)z1 * p.c_bs1;
-      c.row0 = m_blk * BM + q * 32;
-      c.nrows = max(0, min(32, p.M - c.row0));
-      c.n_blk = n_blk;
-      c.lane = lane;
-#define MB_EPI(ACT, DACT, NRES, AUX, ROPE, ACCUM) epi_tile<BN, ACT, DACT, NRES, AUX, ROPE, ACCUM, false, OutT>(p, c)
-      if constexpr (sizeof(OutT) == 4) {
-        // fp32 outputs are attention scores and weight gradients: only plain / accumulate are specialised
-        switch (p.epi_kind) {
-          case EK_SPLITK:
-          case EK_PLAIN: MB_EPI(0, 0, 0, false, false, false); break;
-          case EK_ACCUM: MB_EPI(0, 0, 0, false, false, true); break;
-          default: epi_tile<BN, 0, 0, 0, false, false, false, true, OutT>(p, c); break;
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem_a + stage * C_::kABytes) + a_off;
+        const uint32_t sb = smem_u32(smem_b + stage * C_::kBBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WG_K; ++k) {
+          const uint64_t da = make_smem_desc(sa + k * a_kadv, 0u, 1024);
+          const uint64_t db = make_smem_desc(sb + k * b_kadv, b_lbo, 1024);
+          wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u);
         }
-      } else {
-        switch (p.epi_kind) {
-          case EK_SPLITK:
-          case EK_PLAIN: MB_EPI(0, 0, 0, false, false, false); break;
-          case EK_ROPE: MB_EPI(0, 0, 0, false, true, false); break;
-          case EK_GELU: MB_EPI(MB200_ACT_GELU_NEW, 0, 0, false, false, false); break;
-          case EK_GELU_AUX: MB_EPI(MB200_ACT_GELU_NEW, 0, 0, true, false, false); break;
-          case EK_QGELU: MB_EPI(MB200_ACT_QUICK_GELU, 0, 0, false, false, false); break;
-          case EK_RELU: MB_EPI(MB200_ACT_RELU, 0, 0, false, false, false); break;
-          case EK_DGELU: MB_EPI(0, MB200_DACT_GELU_NEW, 0, false, false, false); break;
-          case EK_DRELU: MB_EPI(0, MB200_DACT_RELU, 0, false, false, false); break;
-          case EK_RES1: MB_EPI(0, 0, 1, false, false, false); break;
-          case EK_RES2: MB_EPI(0, 0, 2, false, false, false); break;
-          default: epi_tile<BN, 0, 0, 0, false, false, false, true, OutT>(p, c); break;
+        wgmma_commit();
+        wgmma_wait<1>();  // the group of the previous k-block has retired: its slot may be refilled
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
         }
       }
-#undef MB_EPI
+      wgmma_wait<0>();
+      if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+      const long long boff = (long long)z0 * p.c_bs0 + (long long)z1 * p.c_bs1;
+      epi_fragment<BN>(p, acc, boff, m_blk * BM + cw * 64, n_blk * BN, ks);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<C_::kTmemCols>(tmem_base);
   }
 }
 
@@ -352,39 +275,13 @@ int make_operand_map(CUtensorMap* out, const mb200_operand& op, int rows, int K,
   return 0;
 }
 
-// rank-4 tensor map over an output (C / aux_out) for the TMA-store epilogue: dims (N, M, nb0, nb1), box = one
-// [128 rows x 128 bytes] SWIZZLE_128B staging slot (64 bf16 or 32 fp32 columns). Stores are clipped at N and M.
-int make_store_map(CUtensorMap* out, const void* ptr, bool f32, int N, int M, int nb0, int nb1, long long ld,
-                   long long bs0, long long bs1) {
-  PFN_encodeTiled enc = get_encode_fn();
-  MB_REQUIRE(enc != nullptr, MB200_E_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
-  const long long esz = f32 ? 4 : 2;
-  MB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && (ld * esz) % 16 == 0 &&
-                 (nb0 == 1 || (bs0 * esz) % 16 == 0) && (nb1 == 1 || (bs1 * esz) % 16 == 0),
-             MB200_E_ALIGN, "gemm output must be 16B aligned in pointer, row stride and batch strides");
-  // TMA stores clip at 16-byte granules: the map ends at N rounded DOWN to 16 bytes; the epilogue's threads write the
-  // remaining N % 8 (bf16) / N % 4 (fp32) columns themselves (epi_tile_v3). At least one granule so the map stays legal.
-  const int n16 = f32 ? (N & ~3) : (N & ~7);
-  cuuint64_t dims[4] = {(cuuint64_t)(n16 > 0 ? n16 : (f32 ? 4 : 8)), (cuuint64_t)M, (cuuint64_t)nb0, (cuuint64_t)nb1};
-  cuuint64_t strides[3] = {(cuuint64_t)(ld * esz), (cuuint64_t)((nb0 > 1 ? bs0 : ld) * esz),
-                           (cuuint64_t)((nb1 > 1 ? bs1 : ld) * esz)};
-  cuuint32_t box[4] = {(cuuint32_t)(f32 ? 32 : 64), 128, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
-                   const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  MB_REQUIRE(r == CUDA_SUCCESS, MB200_E_CUDA, "cuTensorMapEncodeTiled (output) failed (%d): N=%d M=%d ld=%lld", (int)r, N, M,
-             ld);
-  return 0;
-}
-
-template <int BN, bool A_MN, bool B_MN, typename OutT, int AROWS = BM>
+template <int BN, bool A_MN, bool B_MN>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKernelParams& kp,
                        cudaStream_t stream) {
-  auto kern = gemm_tcgen05_kernel<BN, A_MN, B_MN, OutT, AROWS>;
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
-    MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN, AROWS>::kSmemBytes));
+    MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes));
     attr_set = true;
   }
   const long long items = (long long)kp.total_tiles * kp.split_k;
@@ -392,44 +289,44 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   {
     const double nb = (double)kp.total_tiles / ((double)kp.tiles_m * kp.tiles_n);
     const double flops = 2.0 * kp.M * (double)kp.N * kp.K * nb;
-    const double bytes = nb * (2.0 * ((double)kp.M * kp.K + (double)kp.N * kp.K) + (double)sizeof(OutT) * kp.M * kp.N);
+    const double bytes = nb * (2.0 * ((double)kp.M * kp.K + (double)kp.N * kp.K) + (kp.c_f32 ? 4.0 : 2.0) * kp.M * kp.N);
     GemmProfScope prof(stream, flops, bytes);
-    MB_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), Cfg<BN, AROWS>::kSmemBytes, stream, tmA, tmB, kp));
+    MB_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), Cfg<BN>::kSmemBytes, stream, tmA, tmB, kp));
   }
   count_launch();
   MB_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <int BN, typename OutT>
+template <int BN>
 static int dispatch_major(bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
                           const GemmKernelParams& kp, cudaStream_t s) {
-  if (!a_mn && !b_mn) return launch_gemm<BN, false, false, OutT>(tmA, tmB, kp, s);
-  if (!a_mn && b_mn) return launch_gemm<BN, false, true, OutT>(tmA, tmB, kp, s);
-  if (a_mn && !b_mn) return launch_gemm<BN, true, false, OutT>(tmA, tmB, kp, s);
-  return launch_gemm<BN, true, true, OutT>(tmA, tmB, kp, s);
+  if (!a_mn && !b_mn) return launch_gemm<BN, false, false>(tmA, tmB, kp, s);
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true>(tmA, tmB, kp, s);
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false>(tmA, tmB, kp, s);
+  return launch_gemm<BN, true, true>(tmA, tmB, kp, s);
 }
 
-// small-M (M <= 32, K-major A, bf16 out): 32-row A ring
-template <int BN>
-static int dispatch_small(bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKernelParams& kp,
-                          cudaStream_t s) {
-  if (b_mn) return launch_gemm<BN, false, true, bf16, 32>(tmA, tmB, kp, s);
-  return launch_gemm<BN, false, false, bf16, 32>(tmA, tmB, kp, s);
+static int dispatch_bn(int bn, bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                       const GemmKernelParams& kp, cudaStream_t s) {
+  switch (bn) {
+    case 64: return dispatch_major<64>(a_mn, b_mn, tmA, tmB, kp, s);
+    case 128: return dispatch_major<128>(a_mn, b_mn, tmA, tmB, kp, s);
+    default: return dispatch_major<256>(a_mn, b_mn, tmA, tmB, kp, s);
+  }
 }
 
-static int pick_bn(int M, int N, int K, int batches) {
+static int pick_bn(int M, int N, int batches) {
   if (N <= 64) return 64;
-  // Model: time ~ waves * (cost of one tile). A 256-wide tile streams A once per 256 columns and runs the tensor
-  // pipe at 96 B/clk of smem demand; narrower tiles re-read A and are smem-bound (128 B/clk at BN=128, more at 64),
-  // so they only win when wide tiles leave most of the 148 SMs idle (few tiles) — e.g. the adapter down-projection
-  // (M=1024, N=1024: 32 tiles at BN=256, 128 at BN=64).
+  // Model: time ~ waves * (cost of one tile). A wide tile streams A once per BN columns and keeps more MMA work per
+  // smem byte; narrower tiles only win when wide tiles leave most SMs idle (few tiles) — e.g. the adapter
+  // down-projection (M=1024, N=1024: 64 tiles at BN=128, 128 at BN=64). The relative tile costs are estimates.
   const int tiles_m = (M + BM - 1) / BM;
   const int sms = num_sms();
   double best = 1e300;
   int best_bn = 256;
   const int cands[3] = {256, 128, 64};
-  const double tile_cost[3] = {1.0, 0.75, 0.5};  // relative time of one (BM x BN x K) tile (BN=128 measured: 0.70-0.79)
+  const double tile_cost[3] = {1.0, 0.55, 0.3};  // relative time of one (BM x BN x K) tile
   for (int i = 0; i < 3; ++i) {
     const int bn = cands[i];
     if (bn > 64 && N <= bn / 2) continue;
@@ -441,32 +338,22 @@ static int pick_bn(int M, int N, int K, int batches) {
       best_bn = bn;
     }
   }
-  (void)K;
   return best_bn;
-}
-
-static bool use_gemm2() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MB200_GEMM2");  // set MB200_GEMM2=0 to fall back to the 1-CTA kernel everywhere
-    v = e ? atoi(e) : 1;
-  }
-  return v != 0;
 }
 
 // Small-M (decode, M = batch <= 32) GEMMs stream their weight matrix once and are HBM-bound: what matters is bytes in
 // flight, i.e. every SM pulling weights all the time. The plan picks the tile width and a K split so that
-// tiles x splits covers the 148 SMs evenly. Time model, constants fitted to tools/smallm_bench.py --grid on B200
-// (profiles/r01_smallm_grid.log):
+// tiles x splits covers the SMs evenly:
 //   t = t_item + waves * bytes_per_item / rate_per_sm + (split > 1 ? t_finalize : 0),
 //   rate_per_sm = min(per-SM TMA streaming rate (bytes in flight / latency), all-SM HBM rate / active SMs).
+// The HBM rate is the H100 SXM data-sheet figure; the per-SM rates and fixed costs are estimates.
 struct SmallPlan {
   int bn, split;
 };
 static SmallPlan plan_small_m(int N, int K, int M, size_t ws_bytes) {
   const int sms = num_sms();
   const int num_kb = (K + BK - 1) / BK;
-  const double kHbmRate = 5.3e12, kItem = 4e-6, kFinalize = 4e-6;
+  const double kHbmRate = 3.35e12, kItem = 4e-6, kFinalize = 4e-6;
   SmallPlan best{64, 1};
   double best_t = 1e300;
   const int cands[3] = {256, 128, 64};
@@ -484,9 +371,8 @@ static SmallPlan plan_small_m(int N, int K, int M, size_t ws_bytes) {
       const long long items = (long long)tiles * eff_split;
       const long long waves = (items + sms - 1) / sms;
       const double active = (double)(items < sms ? items : sms);
-      const double sm_rate = bn == 64 ? 46e9 : 62e9;  // 96 KB vs 128 KB of weights in flight per SM
-      const double eff = bn == 64 ? 0.88 : (bn == 256 ? 0.95 : 1.0);  // same decomposition, measured relative rate
-      const double rate = eff * (sm_rate < kHbmRate / active ? sm_rate : kHbmRate / active);
+      const double sm_rate = bn == 64 ? 40e9 : 50e9;  // more weight bytes in flight per SM with the deeper B ring
+      const double rate = sm_rate < kHbmRate / active ? sm_rate : kHbmRate / active;
       const double t = kItem + waves * ((double)kb_per * bn * BK * 2 / rate) + (eff_split > 1 ? kFinalize : 0.0);
       if (t < best_t - 1e-12) {
         best_t = t;
@@ -494,31 +380,7 @@ static SmallPlan plan_small_m(int N, int K, int M, size_t ws_bytes) {
       }
     }
   }
-  // experiments: MB200_SMALLM_BN / MB200_SMALLM_SPLIT override the plan (tools/smallm_bench.py)
-  if (const char* e = getenv("MB200_SMALLM_BN")) {
-    const int v = atoi(e);
-    if (v == 64 || v == 128 || v == 256) best.bn = v;
-  }
-  if (const char* e = getenv("MB200_SMALLM_SPLIT")) {
-    int v = atoi(e);
-    if (v >= 1) {
-      while (v > 1 && ((size_t)v * M * ((N + 3) / 4 * 4) * sizeof(float) > ws_bytes || num_kb / v < 1)) --v;
-      const int kb_per = (num_kb + v - 1) / v;
-      best.split = (num_kb + kb_per - 1) / kb_per;
-    }
-  }
   return best;
-}
-
-// Scratch lent by the caller (mb200_gemm_args.splitk_ws) serves two users that never meet in one launch but do follow each
-// other on a stream: split-K partial slices (front of the buffer) and stream-K flags + partial tiles (the LAST
-// kStreamKRegion bytes, when the buffer is large enough to keep kStreamKMinFront for split-K) — separate regions, so
-// split-K data never lands on stream-K's epoch flags.
-static constexpr size_t kStreamKRegion = (size_t)64 << 20;
-static constexpr size_t kStreamKMinFront = (size_t)32 << 20;
-static inline size_t splitk_budget(const mb200_gemm_args* a) {
-  const size_t b = a->splitk_ws ? (size_t)a->splitk_ws_bytes : 0;
-  return b >= kStreamKRegion + kStreamKMinFront ? b - kStreamKRegion : b;
 }
 
 int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
@@ -539,33 +401,28 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
   int rc = check_arch();
   if (rc) return rc;
 
-  const bool force2 = a->force_bn == 512 || a->force_bn == 768;  // testing: force the CTA-pair kernel (768: + stream-K)
-  int bn = force2 ? 256 : (a->force_bn ? a->force_bn : pick_bn(a->M, a->N, a->K, a->nb0 * a->nb1));
-  MB_REQUIRE(bn == 64 || bn == 128 || bn == 256, MB200_E_ARG, "gemm: force_bn must be 64/128/256 (or 512 / 768 = 2-CTA)");
+  int bn = a->force_bn ? a->force_bn : pick_bn(a->M, a->N, a->nb0 * a->nb1);
+  MB_REQUIRE(bn == 64 || bn == 128 || bn == 256, MB200_E_ARG, "gemm: force_bn must be 64, 128 or 256");
 
   CUtensorMap tmA, tmB;
-  // small-M problems (decode: M = batch <= 32) stage only a 32-row A box per k-block (see Cfg<BN, AROWS>)
-  const bool small_m = a->M <= 32 && a->A.mn_major == 0 && a->nb0 * a->nb1 == 1 && a->c_dtype == MB200_BF16 &&
-                       a->force_bn != 512;
+  // small-M problems (decode: M = batch <= 32) are planned for weight streaming (tile width + K split)
+  const bool small_m = a->M <= 32 && a->A.mn_major == 0 && a->nb0 * a->nb1 == 1 && a->c_dtype == MB200_BF16;
   int plan_split = 1;
   if (small_m && !a->force_bn) {
-    const SmallPlan pl = plan_small_m(a->N, a->K, a->M, splitk_budget(a));
+    const SmallPlan pl = plan_small_m(a->N, a->K, a->M, a->splitk_ws ? (size_t)a->splitk_ws_bytes : 0);
     bn = pl.bn;
     plan_split = pl.split;
   }
-  rc = make_operand_map(&tmA, a->A, a->M, a->K, a->nb0, a->nb1, small_m ? 32 : BM);
-  if (rc) return rc;
-  rc = make_operand_map(&tmB, a->B, a->N, a->K, a->nb0, a->nb1, bn);
+  rc = make_operand_map(&tmA, a->A, a->M, a->K, a->nb0, a->nb1, BM);
   if (rc) return rc;
 
   GemmKernelParams kp;
+  memset(&kp, 0, sizeof(kp));
   kp.M = a->M;
   kp.N = a->N;
   kp.K = a->K;
   kp.nb0 = a->nb0;
   kp.tiles_m = (a->M + BM - 1) / BM;
-  kp.tiles_n = (a->N + bn - 1) / bn;
-  kp.total_tiles = kp.tiles_m * kp.tiles_n * a->nb0 * a->nb1;
   kp.C = a->C;
   kp.ldc = a->ldc;
   kp.c_bs0 = a->c_bs0;
@@ -580,28 +437,8 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
   kp.res1 = reinterpret_cast<const bf16*>(a->res1);
   kp.res2 = reinterpret_cast<const bf16*>(a->res2);
   kp.ld_res = a->ld_res;
-  {
-    // pick the specialised epilogue when the request matches one exactly (bias and alpha are free in all of them)
-    const bool rope = a->rope_tab && a->rope_mode != 0;
-    const int nres = (a->res1 ? 1 : 0) + (a->res2 ? 1 : 0);
-    const bool aux = a->aux_out != nullptr;
-    int k = EK_GENERIC;
-    if (!rope && !a->act && !a->dact && nres == 0 && !aux) k = a->accumulate ? EK_ACCUM : EK_PLAIN;
-    else if (rope && !a->act && !a->dact && nres == 0 && !aux && !a->accumulate) k = EK_ROPE;
-    else if (!rope && !a->dact && nres == 0 && !a->accumulate) {
-      if (a->act == MB200_ACT_GELU_NEW) k = aux ? EK_GELU_AUX : EK_GELU;
-      else if (a->act == MB200_ACT_QUICK_GELU && !aux) k = EK_QGELU;
-      else if (a->act == MB200_ACT_RELU && !aux) k = EK_RELU;
-    } else if (!rope && !a->act && nres == 0 && !aux && !a->accumulate) {
-      if (a->dact == MB200_DACT_GELU_NEW) k = EK_DGELU;
-      else if (a->dact == MB200_DACT_RELU) k = EK_DRELU;
-    } else if (!rope && (!a->act || a->act == MB200_ACT_RELU_POST) && !a->dact && !aux && !a->accumulate &&
-               nres > 0) {
-      if (nres == 2) k = EK_RES2;
-      else if (a->res1) k = EK_RES1;
-    }
-    kp.epi_kind = k;
-  }
+  kp.epi_kind = EK_GENERIC;
+  kp.c_f32 = a->c_dtype == MB200_F32 ? 1 : 0;
   kp.rope_tab = reinterpret_cast<const float2*>(a->rope_tab);
   kp.rope_mode = a->rope_tab ? a->rope_mode : 0;
   kp.rope_S = a->rope_S;
@@ -615,44 +452,30 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
 
   const bool amn = a->A.mn_major != 0, bmn = a->B.mn_major != 0;
   const bool f32 = a->c_dtype == MB200_F32;
-  {
-    static int preload = -1;
-    if (preload < 0) {
-      const char* e = getenv("MB200_B_PRELOAD");  // 0 = never fetch weight tiles ahead of the PDL wait (A/B switch)
-      preload = e ? atoi(e) : 1;
-    }
-    kp.b_static = (a->B.static_data != 0 && preload) ? 1 : 0;
-  }
-  kp.sk_on = 0;
-  kp.sk_ws = nullptr;
-  kp.sk_flags = nullptr;
   kp.split_k = 1;
   kp.kb_per_split = (a->K + BK - 1) / BK;
-  kp.splitk_ws = nullptr;
-  kp.ld_ws = 0;
-  // Split-K for small M (see plan_small_m; for 32 < M <= 128 only the long-K / narrow-N shape, GPT-J fc_out, is split:
-  // measured 80 -> 49 us at M = 32). Partials go to per-split fp32 slices; a small finalize kernel sums them in fixed
-  // order (deterministic) and applies the fused epilogue.
+  // Split-K for small M (see plan_small_m; for 32 < M <= 128 only the long-K / narrow-N shape, GPT-J fc_out, is split).
+  // Partials go to per-split fp32 slices; a small finalize kernel sums them in fixed order (deterministic) and applies
+  // the fused epilogue.
   const bool split_mid = !small_m && a->splitk_ws && a->M <= 128 && a->nb0 * a->nb1 == 1 && a->K >= 8192 &&
                          a->N <= 8192 && !a->force_bn;
   // Larger M with few tiles and a long K (conv-trunk 3x3 convolutions of the late stages: M = 1152, N = 768,
-  // K = 6912 -> 27 tiles of 108 k-blocks): one SM pulls operands at <= ~60 GB/s, so 27 busy SMs are bandwidth-starved
-  // (measured 115 us, ~100 TFLOP/s); split K until tiles x splits covers the machine.
+  // K = 6912 -> 27 tiles of 108 k-blocks) leave most SMs idle: split K until tiles x splits covers the machine.
   const int bn_few = a->N >= 256 ? 256 : (a->N > 64 ? 128 : 64);
+  const int tiles_m = kp.tiles_m;
   const bool split_few = !small_m && !split_mid && a->splitk_ws && a->M > 128 && a->nb0 * a->nb1 == 1 &&
-                         a->K >= 2048 && !a->force_bn &&
-                         2 * kp.tiles_m * ((a->N + bn_few - 1) / bn_few) <= num_sms();
+                         a->K >= 2048 && !a->force_bn && 2 * tiles_m * ((a->N + bn_few - 1) / bn_few) <= num_sms();
   if (plan_split > 1 || split_mid || split_few) {
     const int bn_s = small_m ? bn : bn_few;
     const int tiles = (a->N + bn_s - 1) / bn_s;
     const int num_kb = (a->K + BK - 1) / BK;
     int split = plan_split;
     if (split_mid || split_few) {
-      split = num_sms() / (tiles * kp.tiles_m);
+      split = num_sms() / (tiles * tiles_m);
       if (split > num_kb / 4) split = num_kb / 4;
     }
     const long long ld_ws = (a->N + 3) / 4 * 4;
-    while (split > 1 && (size_t)split * a->M * ld_ws * sizeof(float) > splitk_budget(a)) --split;
+    while (split > 1 && (size_t)split * a->M * ld_ws * sizeof(float) > (size_t)a->splitk_ws_bytes) --split;
     if (split > 1) {
       const int kb_per = (num_kb + split - 1) / split;
       split = (num_kb + kb_per - 1) / kb_per;  // every split owns at least one k-block
@@ -660,29 +483,15 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
       rc = make_operand_map(&tmB, a->B, a->N, a->K, a->nb0, a->nb1, bn);
       if (rc) return rc;
       kp.tiles_n = tiles;
-      kp.total_tiles = kp.tiles_m * tiles;
+      kp.total_tiles = tiles_m * tiles;
       kp.split_k = split;
       kp.kb_per_split = kb_per;
       kp.splitk_ws = reinterpret_cast<float*>(a->splitk_ws);
       kp.ld_ws = ld_ws;
-      GemmKernelParams kg = kp;  // the GEMM itself only accumulates partials
+      GemmKernelParams kg = kp;  // the GEMM itself only writes partials (alpha applied)
       kg.epi_kind = EK_SPLITK;
-      kg.bias = nullptr;
-      int r2;
-      if (small_m) {
-        switch (bn) {
-          case 64: r2 = dispatch_small<64>(bmn, tmA, tmB, kg, stream); break;
-          case 128: r2 = dispatch_small<128>(bmn, tmA, tmB, kg, stream); break;
-          default: r2 = dispatch_small<256>(bmn, tmA, tmB, kg, stream); break;
-        }
-      } else {
-        switch (bn) {
-          case 64: r2 = dispatch_major<64, bf16>(amn, bmn, tmA, tmB, kg, stream); break;
-          case 128: r2 = dispatch_major<128, bf16>(amn, bmn, tmA, tmB, kg, stream); break;
-          default: r2 = dispatch_major<256, bf16>(amn, bmn, tmA, tmB, kg, stream); break;
-        }
-      }
-      if (r2) return r2;
+      rc = dispatch_bn(bn, amn, bmn, tmA, tmB, kg, stream);
+      if (rc) return rc;
       const long long n4 = (long long)a->M * ((a->N + 3) / 4);
       const int fgrid = (int)((n4 + 255) / 256 > 2048 ? 2048 : (n4 + 255) / 256);
       kp.alpha = 1.f;  // already applied to the partials
@@ -692,113 +501,11 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
       return 0;
     }
   }
-  // (short-K problems are dominated by per-tile fixed cost, where the 1-CTA kernel with narrower tiles does better)
-  if (force2 || (bn == 256 && a->M > 128 && a->N >= 256 && a->K >= 512 && !a->force_bn && use_gemm2())) {
-    // CTA-pair kernel: 256x256 tile per pair, each SM stages its own 128 A rows and HALF of the B tile
-    // (64 B/clk of L2->SM traffic per SM instead of 96), 6-stage ring
-    rc = make_operand_map(&tmB, a->B, a->N, a->K, a->nb0, a->nb1, 128);
-    if (rc) return rc;
-    kp.tiles_m = (a->M + 255) / 256;  // cluster tiles along M
-    kp.total_tiles = kp.tiles_m * kp.tiles_n * a->nb0 * a->nb1;
-    // the rotary epilogue of the row-per-thread path works on whole 32-column chunks
-    if (kp.epi_kind == EK_ROPE && (a->rope_hd % 32 != 0 || a->rope_rot % 32 != 0 || a->rope_ncols % 32 != 0))
-      kp.epi_kind = EK_GENERIC;
-    // ---- stream-K of the last wave (see GemmKernelParams::sk_*): only when the caller lent scratch memory ----
-    kp.sk_on = 0;
-    CUtensorMap tmWs;
-    {
-      // OFF by default. Measured on a B200 (profiles/r02_streamk_ab.log): correct and bit-reproducible, but no faster —
-      // 28.9 vs 28.0 us at N = K = 4096, 96.5 vs 97.1 us at K = 16384, and slower on the multi-wave shapes (96 vs 75 us
-      // for qkv, 132 vs 100 us for fc_in) where the owners' partial-tile reads sit on the critical path. The long-K
-      // GEMMs already run at the POWER-limited rate (1.42 - 1.47 PFLOP/s = cuBLAS's sustained figure, sw_power_cap
-      // active): filling the 20 idle SMs lowers the clock of the other 128. MB200_STREAMK=1 (or force_bn = 768 for one
-      // call) turns it on; the parity group `streamk` of tools/gemm_check.py keeps it honest.
-      static int sk_env = -1;
-      if (sk_env < 0) {
-        const char* e = getenv("MB200_STREAMK");
-        sk_env = e ? atoi(e) : 0;
-      }
-      const bool sk_forced = a->force_bn == 768;
-      const int ncl = gemm_sms() / 2;
-      const int T = kp.total_tiles, KBn = (a->K + BK - 1) / BK;
-      const int W = T / ncl, R = T - W * ncl;
-      if ((sk_env || sk_forced) && !amn && !f32 && a->splitk_ws && a->nb0 * a->nb1 == 1 && kp.epi_kind != EK_GENERIC && R > 0 && R < ncl &&
-          KBn >= 16 && (!a->force_bn || sk_forced)) {
-        const int h = (int)(((long long)R * KBn + ncl - 1) / ncl);
-        const int tail = KBn - h, nh = ncl - R;
-        const long long U = (long long)R * tail;
-        // pieces per helper (slots) and per tile (the owner's partial list) must stay small: every partial is a
-        // 256 KB L2 round trip on the owner's critical path
-        int pmax = 0, per_tile = 0;
-        if (h >= 8 && tail >= 1 && h < KBn) {
-          for (int j = 0; j < nh; ++j) {
-            const long long lo = (long long)j * U / nh, hi = (long long)(j + 1) * U / nh;
-            const int np = hi > lo ? (int)((hi - 1) / tail - lo / tail) + 1 : 0;
-            if (np > pmax) pmax = np;
-          }
-          for (int ti = 0; ti < R; ++ti) {
-            const long long x0 = (long long)ti * tail, x1 = x0 + tail;
-            int n = 0;
-            for (int j = 0; j < nh; ++j) {
-              const long long lo = (long long)j * U / nh, hi = (long long)(j + 1) * U / nh;
-              if (hi > lo && lo < x1 && hi > x0) ++n;
-            }
-            if (n > per_tile) per_tile = n;
-          }
-        }
-        const size_t flag_bytes = 65536;
-        const size_t need = flag_bytes + (size_t)nh * (size_t)(pmax > 0 ? pmax : 1) * 256 * 256 * sizeof(float);
-        uint8_t* sk_base = reinterpret_cast<uint8_t*>(a->splitk_ws) + (a->splitk_ws_bytes - (long long)kStreamKRegion);
-        if (pmax >= 1 && pmax <= 4 && per_tile >= 1 && per_tile <= 3 && need <= kStreamKRegion &&
-            (size_t)a->splitk_ws_bytes >= kStreamKRegion + kStreamKMinFront &&
-            (size_t)nh * pmax * 2 * sizeof(unsigned int) <= flag_bytes) {
-          static unsigned int epoch = 0x5eed0000u;
-          kp.sk_on = 1;
-          kp.sk_W = W;
-          kp.sk_R = R;
-          kp.sk_h = h;
-          kp.sk_tail = tail;
-          kp.sk_nh = nh;
-          kp.sk_pmax = pmax;
-          kp.sk_U = U;
-          kp.sk_flags = reinterpret_cast<unsigned int*>(sk_base);
-          kp.sk_ws = reinterpret_cast<float*>(sk_base + flag_bytes);
-          kp.sk_epoch = ++epoch;
-          rc = make_store_map(&tmWs, kp.sk_ws, true, 256, nh * pmax * 256, 1, 1, 256, 0, 0);
-          if (rc) return rc;
-        }
-      }
-    }
-    CUtensorMap tmC, tmAux;
-    rc = make_store_map(&tmC, a->C, f32, a->N, a->M, a->nb0, a->nb1, a->ldc, a->c_bs0, a->c_bs1);
-    if (rc) return rc;
-    if (!kp.sk_on) tmWs = tmC;
-    if (a->aux_out) {
-      rc = make_store_map(&tmAux, a->aux_out, false, a->N, a->M, a->nb0, a->nb1, a->ldc, a->c_bs0, a->c_bs1);
-      if (rc) return rc;
-    } else {
-      tmAux = tmC;
-    }
-    return launch_gemm2(tmA, tmB, tmC, tmAux, tmWs, kp, amn, bmn, f32, stream);
-  }
-  if (small_m) {
-    switch (bn) {
-      case 64: return dispatch_small<64>(bmn, tmA, tmB, kp, stream);
-      case 128: return dispatch_small<128>(bmn, tmA, tmB, kp, stream);
-      default: return dispatch_small<256>(bmn, tmA, tmB, kp, stream);
-    }
-  }
-  switch (bn) {
-    case 64:
-      return f32 ? dispatch_major<64, float>(amn, bmn, tmA, tmB, kp, stream)
-                 : dispatch_major<64, bf16>(amn, bmn, tmA, tmB, kp, stream);
-    case 128:
-      return f32 ? dispatch_major<128, float>(amn, bmn, tmA, tmB, kp, stream)
-                 : dispatch_major<128, bf16>(amn, bmn, tmA, tmB, kp, stream);
-    default:
-      return f32 ? dispatch_major<256, float>(amn, bmn, tmA, tmB, kp, stream)
-                 : dispatch_major<256, bf16>(amn, bmn, tmA, tmB, kp, stream);
-  }
+  rc = make_operand_map(&tmB, a->B, a->N, a->K, a->nb0, a->nb1, bn);
+  if (rc) return rc;
+  kp.tiles_n = (a->N + bn - 1) / bn;
+  kp.total_tiles = tiles_m * kp.tiles_n * a->nb0 * a->nb1;
+  return dispatch_bn(bn, amn, bmn, tmA, tmB, kp, stream);
 }
 
 }  // namespace mb200

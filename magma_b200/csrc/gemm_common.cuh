@@ -1,40 +1,24 @@
-// magma_b200 — pieces shared by the 1-CTA (gemm.cu) and 2-CTA (gemm2.cu) tcgen05 GEMM kernels: tile configuration,
-// kernel parameter block, UMMA shared-memory descriptor, and the fused epilogue.
+// magma_b200 — pieces shared by the GEMM core (gemm.cu) and the fused attention kernels (attention.cu): tile
+// configuration, kernel parameter block and the fused epilogue applied to wgmma accumulator fragments.
 #pragma once
 #include "common.cuh"
 
 namespace mb200 {
 
-static constexpr int BM = 128;       // UMMA M (cta_group::1)
-static constexpr int BK = 64;        // 64 bf16 = 128 bytes = one SWIZZLE_128B row
-static constexpr int UMMA_K = 16;    // fixed for 16-bit inputs
-static constexpr int kThreads = 256; // 8 warps
-static constexpr int kSmemBudget = 192 * 1024;  // operand ring; + 34 KB epilogue staging + barriers < 227 KB
+static constexpr int BM = 128;        // tile M: two consumer warpgroups x wgmma M = 64
+static constexpr int BK = 64;         // 64 bf16 = 128 bytes = one SWIZZLE_128B row
+static constexpr int WG_K = 16;       // wgmma K for 16-bit inputs
+static constexpr int kThreads = 384;  // warpgroup 0 = TMA producer, warpgroups 1, 2 = MMA + epilogue
+static constexpr int kSmemBudget = 200 * 1024;  // operand ring; + alignment slack and barriers < 227 KB
 
-// AROWS = rows of A actually staged per k-block. 128 normally. 32 for small-M (decode) problems: only a 32-row TMA box
-// is loaded per stage and the A slots are packed 4 KB apart; the UMMA descriptor still spans 128 rows (16 KB), so
-// rows 32..127 of the product are computed from whatever follows in shared memory — those TMEM lanes are never stored.
-// The freed shared memory goes to deeper rings: what bounds a weight-streaming GEMM is bytes of B in flight per SM.
-//
-// In that mode a ring stage also carries kKS consecutive k-blocks (4 at BN = 64, 2 at BN = 128): the single MMA-issuing
-// thread spends ~350 cycles per barrier round trip (try_wait + fence + 4 tcgen05.mma + commit), which hides under the
-// 512 tensor-pipe cycles of a 128x256 k-block but not under the 128 cycles of a 128x64 one.
-template <int BN, int AROWS = BM>
+template <int BN>
 struct Cfg {
-  static constexpr int kKS = AROWS == BM ? 1 : (BN == 64 ? 4 : (BN == 128 ? 2 : 1));  // k-blocks per ring stage
-  static constexpr int kASub = AROWS * BK * 2;    // bytes of one k-block of A (sub-slot stride)
-  static constexpr int kBSub = BN * BK * 2;
-  static constexpr int kABytes = kASub * kKS;     // slot stride of the A ring
-  static constexpr int kBBytes = kBSub * kKS;
+  static constexpr int kABytes = BM * BK * 2;
+  static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kAWindow = BM * BK * 2;    // bytes an MMA reads starting at an A slot
-  static constexpr int kMaxStages = AROWS == BM ? 8 : 16;
-  static constexpr int kStagesRaw = (kSmemBudget - (kAWindow - kASub)) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > kMaxStages ? kMaxStages : kStagesRaw;
-  static constexpr int kTmemCols = 2 * BN;  // two accumulator buffers; 128/256/512 — powers of two
-  static constexpr int kEpiPitch = 64;      // floats per staged row; 16-byte chunks XOR-swizzled by (row & 15)
-  static constexpr int kEpiBytes = 4 * 32 * kEpiPitch * 4;  // per-warp [32 rows][64 cols] fp32 staging, 4 warps
-  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align slack*/ + 512 /*barriers*/;
+  static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
+  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 struct GemmKernelParams {
@@ -55,755 +39,149 @@ struct GemmKernelParams {
   const float2* rope_tab;  // [rope_S][rope_rot/2] (cos, sin) of the position of row (row % rope_S)
   int rope_mode;           // +1 forward, -1 inverse (transpose rotation)
   int rope_S, rope_hd, rope_rot, rope_ncols;
-  int epi_kind;  // EK_*: which specialised epilogue handles full float4 column groups (0 = generic only)
+  int epi_kind;  // EK_GENERIC, or EK_SPLITK for the partial tiles of a split-K GEMM
+  int c_f32;     // C is fp32 (else bf16)
   // split-K (small-M / weight-streaming GEMMs, e.g. decode): work item = (tile, k-range); partial tiles are reduced
   // written to splitk_ws [split][M][ld_ws] (fp32) and summed in fixed order, with the fused epilogue, by
   // splitk_finalize_kernel
   int split_k, kb_per_split;
   float* splitk_ws;
   long long ld_ws;
-  int b_static;  // B is never written by a kernel of this stream (frozen weights): its first tiles load before the PDL wait
-  // stream-K of the last (partial) wave — CTA-pair kernel only, see gemm2.cu. W full waves of whole tiles, then the R
-  // remaining tiles: cluster c < R accumulates k-blocks [0, h) of tile W*ncl + c ("owner"), the nh = ncl - R other
-  // clusters ("helpers") share the k-blocks [h, num_kb) of those R tiles in contiguous ranges of the tail space
-  // (tile-major, `tail` = num_kb - h positions per tile) and hand their fp32 partial tiles to the owners through sk_ws.
-  int sk_on, sk_W, sk_R, sk_h, sk_tail, sk_nh, sk_pmax;
-  long long sk_U;          // R * tail
-  float* sk_ws;            // [nh * pmax slots][256 rows][256 cols] fp32
-  unsigned int* sk_flags;  // [nh * pmax slots][2 CTAs]: == sk_epoch once the slot's half has landed
-  unsigned int sk_epoch;
 };
 
-struct WorkItem {
-  int tile, kb0, kb1;
-  int kind;   // 0 = a whole tile, 1 = head of a split tile (owner: adds the helpers' partials, then the fused epilogue),
-              // 2 = a tail piece (helper: fp32 partial tile -> sk_ws slot)
-  int slot;   // kind 2: workspace slot
-};
-
-// the i-th work item of cluster `cid` (same sequence for the producer, the MMA issuer and the epilogue warps)
-template <bool SK = true>
-__device__ __forceinline__ bool next_item(const GemmKernelParams& p, int cid, int ncl, int num_kb, int i, WorkItem& w) {
-  w.kb0 = 0;
-  w.kb1 = num_kb;
-  w.kind = 0;
-  w.slot = 0;
-  if (!SK || !p.sk_on) {  // the default kernel is instantiated with SK = false: none of the split bookkeeping exists there
-    w.tile = cid + i * ncl;
-    return w.tile < p.total_tiles;
-  }
-  if (cid < p.sk_R) {  // owner: whole tiles first, the head of its split tile last (partials are long there by then)
-    if (i < p.sk_W) {
-      w.tile = cid + i * ncl;
-      return true;
-    }
-    if (i > p.sk_W) return false;
-    w.tile = p.sk_W * ncl + cid;
-    w.kb1 = p.sk_h;
-    w.kind = 1;
-    return true;
-  }
-  // helper: its tail pieces first (so that no owner ever waits), then whole tiles
-  const int j = cid - p.sk_R;
-  const long long a = (long long)j * p.sk_U / p.sk_nh, b = (long long)(j + 1) * p.sk_U / p.sk_nh;
-  const int np = b > a ? (int)((b - 1) / p.sk_tail - a / p.sk_tail) + 1 : 0;
-  if (i < np) {
-    const long long ti = a / p.sk_tail + i;
-    const long long u0 = a > ti * p.sk_tail ? a : ti * p.sk_tail;
-    const long long u1 = b < (ti + 1) * p.sk_tail ? b : (ti + 1) * p.sk_tail;
-    w.tile = p.sk_W * ncl + (int)ti;
-    w.kb0 = p.sk_h + (int)(u0 - ti * p.sk_tail);
-    w.kb1 = p.sk_h + (int)(u1 - ti * p.sk_tail);
-    w.kind = 2;
-    w.slot = j * p.sk_pmax + i;
-    return true;
-  }
-  if (i - np >= p.sk_W) return false;
-  w.tile = cid + (i - np) * ncl;
-  return true;
-}
-
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout, SWIZZLE_128B, version 1)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
-  return d;
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// Epilogue. Accumulator rows live one-per-thread in TMEM; outputs (and residual / aux inputs) want row-contiguous
-// global access. Per 64-column group: phase 1 moves TMEM -> registers -> a per-warp XOR-swizzled smem block, phase 2
-// re-reads it so that 16 lanes x 4 columns cover one row segment (full 128-byte lines per row).
-// The four epilogue warps run ONE warp per scheduler, so phase 2 is latency-bound unless it is straight-line with
-// high ILP: epi_tile<> is specialised at compile time on what the epilogue does, fully unrolled over the 16 row pairs,
-// uses pointer bumps instead of per-row address arithmetic, and issues ALL global loads of a group (residuals, aux)
-// before anything is stored (a store may alias a later load as far as the compiler knows, which would serialise one
-// DRAM round trip per row pair). The kernel dispatches once per tile on p.epi_kind (chosen on the host).
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float4 lds128(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t saddr, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-__device__ __forceinline__ void bf16x4_to_f32(const uint2& u, float (&f)[4]) {
-  const float2 f0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-  const float2 f1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-  f[0] = f0.x; f[1] = f0.y; f[2] = f1.x; f[3] = f1.y;
-}
-__device__ __forceinline__ uint2 f32x4_to_bf16(const float (&v)[4]) {
-  __nv_bfloat162 h0 = __floats2bfloat162_rn(v[0], v[1]), h1 = __floats2bfloat162_rn(v[2], v[3]);
-  uint2 u;
-  u.x = *reinterpret_cast<uint32_t*>(&h0);
-  u.y = *reinterpret_cast<uint32_t*>(&h1);
+__device__ __forceinline__ uint32_t ldg32(const bf16* ptr) {
+  uint32_t u;
+  asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(u) : "l"(ptr));
   return u;
 }
-__device__ __forceinline__ uint2 ldg64(const bf16* ptr) {
-  uint2 u;
-  asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(u.x), "=r"(u.y) : "l"(ptr));
-  return u;
+__device__ __forceinline__ float2 bf16x2_to_f32(uint32_t u) {
+  return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
+}
+__device__ __forceinline__ uint32_t f32x2_to_bf16(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
 }
 
-enum { EK_GENERIC = 0, EK_PLAIN, EK_ROPE, EK_GELU, EK_GELU_AUX, EK_QGELU, EK_RELU, EK_DGELU, EK_DRELU, EK_RES1,
-       EK_RES2, EK_ACCUM, EK_SPLITK };
+enum { EK_GENERIC = 0, EK_SPLITK };
 
-struct EpiCtx {
-  uint32_t tmem_acc;  // TMEM address of this warp's lanes, column 0 of the accumulator buffer
-  uint32_t stg_s;     // smem address of this warp's staging block
-  uint64_t* tmem_full;
-  uint64_t* tmem_empty;
-  int empty_remote;   // 0: arrive on the local tmem_empty barrier; 1: arrive on the leader CTA's (2-CTA kernel, peer CTA)
-  uint32_t full_phase;
-  long long boff;     // batch offset in C (elements)
-  int row0, nrows, n_blk, lane;
-  int ks;             // split-K index of this work item (0 when K is not split)
-};
-
-// slow per-lane path: any combination of epilogue options, any number (1..4) of valid columns. Used for float4
-// groups cut by the N edge and for option combinations without a specialised instantiation.
-template <typename OutT>
-__device__ __noinline__ void epi_lane_generic(const GemmKernelParams& p, const EpiCtx& c, int col, int nvalid, int rsub,
-                                              int c4) {
-  float bv[4] = {0.f, 0.f, 0.f, 0.f};
+// ---------------------------------------------------------------------------------------------
+// Epilogue on the accumulator fragment of one consumer warpgroup (64 rows x BN columns, wgmma.cuh layout): every thread
+// owns column pairs (c, c + 1), c even, of two rows. A pair is also a rotary pair (rotate_every_two), so alpha / bias /
+// rotary / saved pre-activation / activation / activation-derivative / residuals / store are all applied in registers
+// on 8-byte (fp32) or 4-byte (bf16) chunks without any exchange between threads. All branches on p are warp-uniform.
+// Split-K work items store the fp32 partial tile into their slice of the workspace instead (EK_SPLITK).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void epi_pair(const GemmKernelParams& p, long long boff, int row, int col, float v0, float v1,
+                                         int ks) {
+  if (row >= p.M || col >= p.N) return;
+  const bool two = col + 1 < p.N;
+  v0 *= p.alpha;
+  v1 *= p.alpha;
+  if (p.epi_kind == EK_SPLITK) {
+    float* w = p.splitk_ws + ((long long)ks * p.M + row) * p.ld_ws + col;  // ld_ws % 4 == 0: the padded column exists
+    *reinterpret_cast<float2*>(w) = make_float2(v0, v1);
+    return;
+  }
   if (p.bias) {
-#pragma unroll
-    for (int e = 0; e < 4; ++e)
-      if (e < nvalid) bv[e] = __bfloat162float(p.bias[col + e]);
+    v0 += __bfloat162float(p.bias[col]);
+    if (two) v1 += __bfloat162float(p.bias[col + 1]);
   }
-  int rope_p = -1;
   if (p.rope_mode != 0 && col < p.rope_ncols) {
     const int dim = col % p.rope_hd;
-    if (dim < p.rope_rot) rope_p = dim >> 1;
-  }
-  for (int it = 0; it < 16; ++it) {
-    const int rl = it * 2 + rsub;
-    if (rl >= c.nrows) continue;
-    const int row = c.row0 + rl;
-    const float4 sv = lds128(c.stg_s + (uint32_t)(rl * 256 + ((((c4 >> 2)) ^ (rl & 15)) << 4)));
-    float v[4] = {sv.x + bv[0], sv.y + bv[1], sv.z + bv[2], sv.w + bv[3]};
-    const long long coff = c.boff + (long long)row * p.ldc + col;
-    if (rope_p >= 0) {  // pairs never straddle the float4 (col % 4 == 0, rot % 4 == 0)
-      const float2* tp = p.rope_tab + (long long)(row % p.rope_S) * (p.rope_rot >> 1) + rope_p;
-      const float2 cs0 = __ldg(tp), cs1 = __ldg(tp + 1);
+    if (dim < p.rope_rot) {
+      const float2 cs = __ldg(p.rope_tab + (long long)(row % p.rope_S) * (p.rope_rot >> 1) + (dim >> 1));
       const float sg = p.rope_mode > 0 ? 1.f : -1.f;
-      const float a0 = v[0], a1 = v[1], a2 = v[2], a3 = v[3];
-      v[0] = a0 * cs0.x - a1 * cs0.y * sg;
-      v[1] = a1 * cs0.x + a0 * cs0.y * sg;
-      v[2] = a2 * cs1.x - a3 * cs1.y * sg;
-      v[3] = a3 * cs1.x + a2 * cs1.y * sg;
-    }
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      if (e >= nvalid) continue;
-      float x = v[e];
-      if (p.aux_out) p.aux_out[coff + e] = __float2bfloat16(x);
-      if (p.act == MB200_ACT_GELU_NEW) x = gelu_new_f(x);
-      else if (p.act == MB200_ACT_QUICK_GELU) x = quick_gelu_f(x);
-      else if (p.act == MB200_ACT_RELU) x = fmaxf(x, 0.f);
-      if (p.dact) {
-        const float a = __bfloat162float(p.aux_in[coff + e]);
-        x = p.dact == MB200_DACT_GELU_NEW ? x * gelu_new_grad_f(a) : (a > 0.f ? x : 0.f);
-      }
-      const long long roff = c.boff + (long long)row * p.ld_res + col + e;
-      if (p.res1) x += __bfloat162float(p.res1[roff]);
-      if (p.res2) x += __bfloat162float(p.res2[roff]);
-      if (p.act == MB200_ACT_RELU_POST) x = fmaxf(x, 0.f);
-      if constexpr (sizeof(OutT) == 4) {
-        float* dst = reinterpret_cast<float*>(p.C) + coff + e;
-        *dst = p.accumulate ? *dst + x : x;
-      } else {
-        reinterpret_cast<bf16*>(p.C)[coff + e] = __float2bfloat16(x);
-      }
+      const float a0 = v0, a1 = v1;
+      v0 = a0 * cs.x - a1 * cs.y * sg;
+      v1 = a1 * cs.x + a0 * cs.y * sg;
     }
   }
-}
-
-template <int BN, int DACT, int NRES, bool ACCUM, bool GENERIC, int NLD>
-__device__ __forceinline__ void epi_preload(const GemmKernelParams& p, const EpiCtx& c, int g, int c4, int rsub,
-                                            long long cstep, long long rstep, uint2 (&pre)[NLD > 0 ? NLD : 1][16]) {
-  if constexpr (NLD > 0 && !GENERIC) {
-    const int col = c.n_blk * BN + g * 64 + c4;
-    if (col + 4 > p.N) return;
-    const long long aoff = c.boff + (long long)(c.row0 + rsub) * p.ldc + col;
-    const long long roff = c.boff + (long long)(c.row0 + rsub) * p.ld_res + col;
-    constexpr int kD = 0, kR1 = (DACT != 0 ? 1 : 0), kR2 = kR1 + 1, kA = kR1 + NRES;
-#pragma unroll
-    for (int it = 0; it < 16; ++it) {
-      if (it * 2 + rsub < c.nrows) {
-        if constexpr (DACT != 0) pre[kD][it] = ldg64(p.aux_in + aoff + it * cstep);
-        if constexpr (NRES >= 1) pre[kR1][it] = ldg64(p.res1 + roff + it * rstep);
-        if constexpr (NRES >= 2) pre[kR2][it] = ldg64(p.res2 + roff + it * rstep);
-        if constexpr (ACCUM) {
-          const float4 o = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.C) + aoff + it * cstep);
-          pre[kA][it] = make_uint2(__float_as_uint(o.x), __float_as_uint(o.y));
-          pre[kA + 1][it] = make_uint2(__float_as_uint(o.z), __float_as_uint(o.w));
-        }
-      }
-    }
+  const long long coff = boff + (long long)row * p.ldc + col;
+  if (p.aux_out) {
+    if (two) *reinterpret_cast<uint32_t*>(p.aux_out + coff) = f32x2_to_bf16(v0, v1);
+    else p.aux_out[coff] = __float2bfloat16(v0);
   }
-}
-
-template <int BN, int ACT, int DACT, int NRES, bool AUX, bool ROPE, bool ACCUM, bool GENERIC, typename OutT>
-__device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const EpiCtx& c) {
-  constexpr int NLD = (DACT != 0 ? 1 : 0) + NRES + (ACCUM ? 2 : 0);  // uint2 loads per row pair
-  const int lane = c.lane;
-  const int c4 = (lane & 15) * 4;
-  const int rsub = lane >> 4;
-  const int n_tile_end = min(p.N, (c.n_blk + 1) * BN);
-  const long long cstep = 2 * p.ldc, rstep = 2 * p.ld_res;
-  uint2 pre[NLD > 0 ? NLD : 1][16];
-
-  epi_preload<BN, DACT, NRES, ACCUM, GENERIC, NLD>(p, c, 0, c4, rsub, cstep, rstep, pre);  // overlaps the accumulator wait
-  mbar_wait(c.tmem_full, c.full_phase);
-  tc_fence_after();
-
-#pragma unroll 1
-  for (int g = 0; g < BN / 64; ++g) {
-    const int n0 = c.n_blk * BN + g * 64;
-    if (n0 >= p.N) break;  // warp-uniform
-    // ---- phase 1: TMEM -> registers -> per-warp smem staging (thread i owns accumulator row i) ----
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t rr[32];
-      tmem_ld_32x32(c.tmem_acc + (uint32_t)(g * 64 + h * 32), rr);
-      tmem_ld_wait();
-      const uint32_t drow = c.stg_s + (uint32_t)(lane * 256);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        sts128(drow + (uint32_t)(((((h * 32 + j) >> 2) ^ (lane & 15)) << 4)), __uint_as_float(rr[j]) * p.alpha,
-               __uint_as_float(rr[j + 1]) * p.alpha, __uint_as_float(rr[j + 2]) * p.alpha,
-               __uint_as_float(rr[j + 3]) * p.alpha);
-    }
-    if (n0 + 64 >= n_tile_end) {
-      // last column group: the accumulator has been fully read -> hand the TMEM buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (c.empty_remote) mbar_arrive_remote(c.tmem_empty, 0);
-        else mbar_arrive(c.tmem_empty);
-      }
-    }
-    __syncwarp();
-    // ---- phase 2 ----
-    const int col = n0 + c4;
-    const int nvalid = p.N - col;
-    if (p.epi_kind == EK_SPLITK) {
-      // partial tile of a split-K work item: plain fp32 stores into this split's slice of the workspace (deterministic:
-      // the finalize kernel sums the slices in a fixed order and applies the fused epilogue)
-      if (nvalid > 0) {
-        float* wrow = p.splitk_ws + ((long long)c.ks * p.M + (c.row0 + rsub)) * p.ld_ws + col;
-#pragma unroll 4
-        for (int it = 0; it < 16; ++it) {
-          const int rl = it * 2 + rsub;
-          if (rl < c.nrows) {
-            const float4 sv = lds128(c.stg_s + (uint32_t)(rl * 256 + ((((c4 >> 2)) ^ (rl & 15)) << 4)));
-            *reinterpret_cast<float4*>(wrow + (long long)it * 2 * p.ld_ws) = sv;  // ld_ws % 4 == 0: padded columns exist
-          }
-        }
-      }
-    } else if (nvalid >= 4 && !GENERIC) {
-      float bv[4] = {0.f, 0.f, 0.f, 0.f};
-      if (p.bias) bf16x4_to_f32(ldg64(p.bias + col), bv);
-      int rope_p = -1;
-      if constexpr (ROPE) {
-        if (col < p.rope_ncols) {
-          const int dim = col % p.rope_hd;
-          if (dim < p.rope_rot) rope_p = dim >> 1;
-        }
-      }
-      const long long aoff = c.boff + (long long)(c.row0 + rsub) * p.ldc + col;
-      OutT* cptr = reinterpret_cast<OutT*>(p.C) + aoff;
-      bf16* auxo = AUX ? p.aux_out + aoff : nullptr;
-      constexpr int kFence = (ACT == MB200_ACT_GELU_NEW || ACT == MB200_ACT_QUICK_GELU || DACT == MB200_DACT_GELU_NEW) ? 1 : 4;
-#pragma unroll
-      for (int it = 0; it < 16; ++it) {
-        // compiler scheduling fence: keeps the fully unrolled body from hoisting every smem read / conversion of all 16
-        // row pairs at once (register pressure); the global loads were all issued by epi_preload already
-        if (it % kFence == 0) asm volatile("" ::: "memory");
-        const int rl = it * 2 + rsub;
-        if (rl < c.nrows) {
-          const float4 sv = lds128(c.stg_s + (uint32_t)(rl * 256 + ((((c4 >> 2)) ^ (rl & 15)) << 4)));
-          float v[4] = {sv.x + bv[0], sv.y + bv[1], sv.z + bv[2], sv.w + bv[3]};
-          if constexpr (ROPE) {
-            if (rope_p >= 0) {
-              const float2* tp = p.rope_tab + (long long)((c.row0 + rl) % p.rope_S) * (p.rope_rot >> 1) + rope_p;
-              const float2 cs0 = __ldg(tp), cs1 = __ldg(tp + 1);
-              const float sg = p.rope_mode > 0 ? 1.f : -1.f;
-              const float a0 = v[0], a1 = v[1], a2 = v[2], a3 = v[3];
-              v[0] = a0 * cs0.x - a1 * cs0.y * sg;
-              v[1] = a1 * cs0.x + a0 * cs0.y * sg;
-              v[2] = a2 * cs1.x - a3 * cs1.y * sg;
-              v[3] = a3 * cs1.x + a2 * cs1.y * sg;
-            }
-          }
-          if constexpr (AUX) *reinterpret_cast<uint2*>(auxo + it * cstep) = f32x4_to_bf16(v);
-          if constexpr (ACT == MB200_ACT_GELU_NEW) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] = gelu_new_f(v[e]);
-          } else if constexpr (ACT == MB200_ACT_QUICK_GELU) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] = quick_gelu_f(v[e]);
-          } else if constexpr (ACT == MB200_ACT_RELU) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] = fmaxf(v[e], 0.f);
-          }
-          constexpr int kD = 0, kR1 = (DACT != 0 ? 1 : 0), kR2 = kR1 + 1, kA = kR1 + NRES;
-          if constexpr (DACT != 0) {
-            float a[4];
-            bf16x4_to_f32(pre[kD][it], a);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              if constexpr (DACT == MB200_DACT_GELU_NEW) v[e] *= gelu_new_grad_f(a[e]);
-              else v[e] = a[e] > 0.f ? v[e] : 0.f;
-            }
-          }
-          if constexpr (NRES >= 1) {
-            float a[4];
-            bf16x4_to_f32(pre[kR1][it], a);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] += a[e];
-          }
-          if constexpr (NRES >= 2) {
-            float a[4];
-            bf16x4_to_f32(pre[kR2][it], a);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] += a[e];
-          }
-          if constexpr (NRES >= 1) {
-            if (p.act == MB200_ACT_RELU_POST) {  // warp-uniform
-#pragma unroll
-              for (int e = 0; e < 4; ++e) v[e] = fmaxf(v[e], 0.f);
-            }
-          }
-          if constexpr (sizeof(OutT) == 4) {
-            float4 o = make_float4(v[0], v[1], v[2], v[3]);
-            if constexpr (ACCUM) {
-              o.x += __uint_as_float(pre[kA][it].x);
-              o.y += __uint_as_float(pre[kA][it].y);
-              o.z += __uint_as_float(pre[kA + 1][it].x);
-              o.w += __uint_as_float(pre[kA + 1][it].y);
-            }
-            *reinterpret_cast<float4*>(reinterpret_cast<float*>(cptr) + it * cstep) = o;
-          } else {
-            *reinterpret_cast<uint2*>(reinterpret_cast<bf16*>(cptr) + it * cstep) = f32x4_to_bf16(v);
-          }
-        }
-      }
-    } else if (GENERIC && nvalid > 0) {
-      epi_lane_generic<OutT>(p, c, col, nvalid < 4 ? nvalid : 4, rsub, c4);
-    }
-    __syncwarp();  // staging block is reused by the next column group
-    if (g + 1 < BN / 64)  // latency overlaps phase 1 of the next group
-      epi_preload<BN, DACT, NRES, ACCUM, GENERIC, NLD>(p, c, g + 1, c4, rsub, cstep, rstep, pre);
+  if (p.act == MB200_ACT_GELU_NEW) {
+    v0 = gelu_new_f(v0);
+    v1 = gelu_new_f(v1);
+  } else if (p.act == MB200_ACT_QUICK_GELU) {
+    v0 = quick_gelu_f(v0);
+    v1 = quick_gelu_f(v1);
+  } else if (p.act == MB200_ACT_RELU) {
+    v0 = fmaxf(v0, 0.f);
+    v1 = fmaxf(v1, 0.f);
   }
-  if constexpr (!GENERIC) {
-    if (p.epi_kind == EK_SPLITK) return;
-    // a float4 column group cut by the N edge (N % 4 != 0, e.g. the 50258-wide LM head) can only be in the LAST group
-    // of the tile, whose staging block is still intact: finish those lanes on the slow path, outside the hot loop.
-    if (p.N & 3) {
-      const int lastg = (n_tile_end - 1 - c.n_blk * BN) >> 6;
-      const int col = c.n_blk * BN + lastg * 64 + c4;
-      const int nvalid = p.N - col;
-      if (nvalid > 0 && nvalid < 4) epi_lane_generic<OutT>(p, c, col, nvalid, rsub, c4);
-    }
-  }
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// Epilogue v3 (CTA-pair kernel): row-per-thread all the way, output through TMA.
-//
-// Measured on the v2 epilogue above (tools/epi_bench.py, profiles/r02_epi_bench_before.log): 6.7 us per 128x256 tile for
-// a plain bf16 store and 17-18 us with a residual or GELU + saved pre-activation — its phase 2 re-reads the tile from
-// shared memory transposed, one row pair per iteration behind a per-row branch, with generic-address global loads and
-// stores on the threads' critical path. A single-wave GEMM (64 tiles on 74 clusters: every N = 4096 shape of the GPT-J
-// block) pays all of that after its last MMA, and a short-K GEMM (ViT K = 1024, adapter up-projection) is bound by it.
-//
-// Here every epilogue thread keeps the accumulator row TMEM gave it: 32 columns at a time it applies
-// alpha / bias / rotary / activation / activation-derivative / residuals in registers, packs, and writes 16-byte chunks
-// into a SWIZZLE_128B staging slot (conflict-free: the 8 lanes of a quarter-warp hold 8 consecutive rows, whose XOR
-// patterns differ). When a slot holds a [128 rows x 128 bytes] box, one thread hands it to the TMA unit
-// (cp.async.bulk.tensor store; fp32 accumulate = cp.reduce ... add) and the threads move on — no global store, no
-// transposition, no per-row control flow. Inputs that are row-shaped (residuals, saved pre-activations) are read by the
-// owning thread as 64 contiguous bytes per 32 columns, issued one chunk ahead. Two 16 KB slots alternate; the only
-// synchronisation is one 128-thread named barrier per box.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2,
-                                                  int c3) {
-  asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }  // the 4 epilogue warps
-__device__ __forceinline__ uint4 ldg128(const void* ptr) {
-  uint4 u;
-  asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(ptr));
-  return u;
-}
-__device__ __forceinline__ void sts128u(uint32_t saddr, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void bf16x8_to_f32(const uint4& u, float* f) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float2 t = __bfloat1622float2(h[e]);
-    f[2 * e] = t.x;
-    f[2 * e + 1] = t.y;
-  }
-}
-__device__ __forceinline__ uint4 f32x8_to_bf16(const float* v) {
-  __nv_bfloat162 h0 = __floats2bfloat162_rn(v[0], v[1]), h1 = __floats2bfloat162_rn(v[2], v[3]);
-  __nv_bfloat162 h2 = __floats2bfloat162_rn(v[4], v[5]), h3 = __floats2bfloat162_rn(v[6], v[7]);
-  uint4 u;
-  u.x = *reinterpret_cast<uint32_t*>(&h0);
-  u.y = *reinterpret_cast<uint32_t*>(&h1);
-  u.z = *reinterpret_cast<uint32_t*>(&h2);
-  u.w = *reinterpret_cast<uint32_t*>(&h3);
-  return u;
-}
-
-struct Epi3Ctx {
-  uint32_t tmem_acc;   // TMEM address of this warp's lanes, column 0 of the accumulator buffer
-  uint32_t pool_s;     // smem address of the CTA's 32 KB staging pool (1024-byte aligned): two 16 KB slots
-  uint64_t* tmem_full;
-  uint64_t* tmem_empty;
-  int empty_remote;
-  uint32_t full_phase;
-  long long boff;      // batch offset of this tile in C / aux / residuals (elements)
-  int row_cta0;        // first global row (within the batch) of this CTA's 128-row block
-  int q, lane;         // epilogue warp 0..3 (TMEM lane quarter), lane
-  int n_blk, z0, z1;
-  const CUtensorMap* tmC;
-  const CUtensorMap* tmAux;
-  // stream-K owner: fp32 partial tiles of the same rows (row stride 256 floats, this CTA's 128 rows) to add to the
-  // accumulator before alpha / bias / ...; summed in this fixed order (deterministic)
-  int npart;
-  const float* part[6];
-};
-
-__device__ __forceinline__ float4 ldcg128f(const float* ptr) {  // L2-coherent: written by another SM during this kernel
-  float4 v;
-  asm volatile("ld.global.cg.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(ptr));
-  return v;
-}
-
-// one [128 x 128-byte] box of the CTA's tile is complete in `slot`: make the generic-proxy writes visible to the TMA
-// unit, wait until the box stored TWO boxes ago has been read out (so that the other slot is free for the next writer),
-// meet, and let one thread issue the store
-template <bool ACCUM>
-__device__ __forceinline__ void epi3_publish(const Epi3Ctx& c, const CUtensorMap* tm, uint32_t slot_s, int col0,
-                                             bool elected) {
-  fence_proxy_async_smem();
-  if (elected) tma_store_wait_read0();
-  epi_bar_sync();
-  if (elected) {
-    if constexpr (ACCUM) tma_reduce_add_4d(tm, slot_s, col0, c.row_cta0, c.z0, c.z1);
-    else tma_store_4d(tm, slot_s, col0, c.row_cta0, c.z0, c.z1);
-    tma_store_commit();
-  }
-}
-
-// `box` counts the boxes this CTA has published so far (slot = box & 1); it lives across tiles.
-template <int BN, int ACT, int DACT, int NRES, bool AUX, bool ROPE, bool ACCUM, typename OutT, bool SK = false>
-__device__ __forceinline__ void epi_tile_v3(const GemmKernelParams& p, const Epi3Ctx& c, uint32_t& box) {
-  constexpr bool F32 = sizeof(OutT) == 4;
-  static_assert(!F32 || (!AUX && !ROPE && ACT == 0 && DACT == 0 && NRES == 0), "fp32 output: plain / accumulate only");
-  static_assert(!ACCUM || F32, "accumulate needs fp32 output");
-  constexpr int NIN = (DACT != 0 ? 1 : 0) + NRES;  // row-shaped bf16 inputs read by the owning thread
-  constexpr int NCH = BN / 32;
-  const int lane = c.lane;
-  const int r_cta = c.q * 32 + lane;
-  const int grow = c.row_cta0 + r_cta;
-  const bool row_ok = grow < p.M;
-  const bool elected = c.q == 0 && lane == 0;
-  const int n_tile0 = c.n_blk * BN;
-  const uint32_t row_s = (uint32_t)(r_cta * 128);
-  const uint32_t sw = (uint32_t)(r_cta & 7);
-  const long long in_row = c.boff + (long long)grow * (DACT != 0 ? p.ldc : p.ld_res);  // aux_in shares C's geometry
-  const bf16* in_ptr[NIN > 0 ? NIN : 1];
-  if constexpr (DACT != 0) in_ptr[0] = p.aux_in + c.boff + (long long)grow * p.ldc;
-  if constexpr (NRES >= 1) in_ptr[DACT != 0 ? 1 : 0] = p.res1 + c.boff + (long long)grow * p.ld_res;
-  if constexpr (NRES >= 2) in_ptr[(DACT != 0 ? 1 : 0) + 1] = p.res2 + c.boff + (long long)grow * p.ld_res;
-  (void)in_row;
-  int rope_pos = 0;
-  if constexpr (ROPE) rope_pos = grow % p.rope_S;
-
-  // row-shaped inputs are fetched TWO chunks ahead (an L2 round trip under load is about two chunks of epilogue work;
-  // the first two fetches are issued before the accumulator wait and ride under the mainloop)
-  uint4 cur[NIN > 0 ? NIN : 1][4], nxt[NIN > 0 ? NIN : 1][4], nx2[NIN > 0 ? NIN : 1][4];
-  auto load_inputs = [&](int ch, uint4 (&dst)[NIN > 0 ? NIN : 1][4]) {
-    if constexpr (NIN > 0) {
-      const int n0 = n_tile0 + ch * 32;
-#pragma unroll
-      for (int i = 0; i < NIN; ++i) {
-        if (row_ok && n0 + 32 <= p.N) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) dst[i][k] = ldg128(in_ptr[i] + n0 + k * 8);
-        } else {
-          // N edge (or a padding row): element-wise, zero beyond the matrix
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            __nv_bfloat16 t[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-              t[e] = (row_ok && n0 + k * 8 + e < p.N) ? in_ptr[i][n0 + k * 8 + e] : __float2bfloat16(0.f);
-            dst[i][k] = *reinterpret_cast<uint4*>(t);
-          }
-        }
-      }
-    }
-  };
-  load_inputs(0, cur);
-  if (NCH > 1) load_inputs(1, nxt);
-  mbar_wait(c.tmem_full, c.full_phase);
-  tc_fence_after();
-  const int n_valid_ch = min(NCH, (p.N - n_tile0 + 31) / 32);  // chunks of this tile that start inside the matrix
-
-#pragma unroll 1
-  for (int ch = 0; ch < n_valid_ch; ++ch) {
-    const int n0 = n_tile0 + ch * 32;
-    if (ch + 2 < n_valid_ch) load_inputs(ch + 2, nx2);
-    uint32_t rr[32];
-    tmem_ld_32x32(c.tmem_acc + (uint32_t)(ch * 32), rr);
-    tmem_ld_wait();
-    if (ch + 1 == n_valid_ch) {
-      // the accumulator has been fully read: hand the TMEM buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (c.empty_remote) mbar_arrive_remote(c.tmem_empty, 0);
-        else mbar_arrive(c.tmem_empty);
-      }
-    }
-    float v[32];
-    if constexpr (SK) {
-      // stream-K owner: accumulator + the helpers' partial tiles (fixed order), then alpha
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[j]);
-      for (int k = 0; k < c.npart; ++k) {
-        const float* src = c.part[k] + (long long)r_cta * 256 + ch * 32;
-        float4 t4[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) t4[e] = ldcg128f(src + 4 * e);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          v[4 * e] += t4[e].x;
-          v[4 * e + 1] += t4[e].y;
-          v[4 * e + 2] += t4[e].z;
-          v[4 * e + 3] += t4[e].w;
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
+  if (p.dact) {
+    float2 a;
+    if (two) a = bf16x2_to_f32(ldg32(p.aux_in + coff));
+    else a = make_float2(__bfloat162float(p.aux_in[coff]), 0.f);
+    if (p.dact == MB200_DACT_GELU_NEW) {
+      v0 *= gelu_new_grad_f(a.x);
+      v1 *= gelu_new_grad_f(a.y);
     } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[j]) * p.alpha;
-    }
-    if (p.bias) {
-      if (n0 + 32 <= p.N) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float b8[8];
-          bf16x8_to_f32(ldg128(p.bias + n0 + k * 8), b8);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) v[k * 8 + e] += b8[e];
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (n0 + j < p.N) v[j] += __bfloat162float(p.bias[n0 + j]);
-      }
-    }
-    if constexpr (ROPE) {
-      // rope_hd % 32 == 0 and rope_rot % 32 == 0 (host-checked for this path): a 32-column chunk is rotary or not
-      if (n0 < p.rope_ncols && (n0 % p.rope_hd) < p.rope_rot) {
-        const float4* tp = reinterpret_cast<const float4*>(p.rope_tab + (long long)rope_pos * (p.rope_rot >> 1) +
-                                                           ((n0 % p.rope_hd) >> 1));
-        const float sg = p.rope_mode > 0 ? 1.f : -1.f;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float4 cs = __ldg(tp + k);  // (cos, sin) of two adjacent pairs
-          const float a0 = v[4 * k], a1 = v[4 * k + 1], a2 = v[4 * k + 2], a3 = v[4 * k + 3];
-          v[4 * k] = a0 * cs.x - a1 * cs.y * sg;
-          v[4 * k + 1] = a1 * cs.x + a0 * cs.y * sg;
-          v[4 * k + 2] = a2 * cs.z - a3 * cs.w * sg;
-          v[4 * k + 3] = a3 * cs.z + a2 * cs.w * sg;
-        }
-      }
-    }
-    // Columns [N16, N) — the last N % 8 bf16 (N % 4 fp32) columns of a ragged N such as the 50258-wide LM head: a TMA
-    // store clips at 16-byte granules, not at elements (measured: a [.., 1002]-wide bf16 store also wrote columns
-    // 1002..1007), so the output maps end at N16 = N rounded down to 16 bytes and the thread that owns the row writes
-    // those few elements itself. AUX stores its pre-activation tail below, before the activation is applied.
-    const int n16 = F32 ? (p.N & ~3) : (p.N & ~7);
-    const bool has_tail = n0 + 32 > n16 && n0 < p.N && row_ok;
-    if constexpr (AUX) {
-      if (has_tail) {  // (fully unrolled with static indices: a runtime index would move v[] to local memory)
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (n0 + j >= n16 && n0 + j < p.N) p.aux_out[c.boff + (long long)grow * p.ldc + n0 + j] = __float2bfloat16(v[j]);
-      }
-    }
-    if constexpr (F32) {
-      if (has_tail) {
-        float* crow = reinterpret_cast<float*>(p.C) + c.boff + (long long)grow * p.ldc + n0;
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (n0 + j >= n16 && n0 + j < p.N) crow[j] = ACCUM ? crow[j] + v[j] : v[j];
-      }
-      // one 32-column chunk = one [128 x 32] fp32 box
-      const uint32_t slot_s = c.pool_s + (box & 1u) * 16384u;
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        sts128(slot_s + row_s + (((uint32_t)k ^ sw) << 4), v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-      epi3_publish<ACCUM>(c, c.tmC, slot_s, n0, elected);
-      ++box;
-    } else {
-      const int half = ch & 1;
-      uint32_t slot_out, slot_aux = 0;
-      if constexpr (AUX) {
-        // two outputs: slot 0 = C, slot 1 = aux, both single-buffered -> the previous pair must have been read out
-        // before the first write of a new 64-column group
-        if (half == 0) {
-          if (elected) tma_store_wait_read0();
-          epi_bar_sync();
-        }
-        slot_out = c.pool_s;
-        slot_aux = c.pool_s + 16384u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          sts128u(slot_aux + row_s + (((uint32_t)(half * 4 + k) ^ sw) << 4), f32x8_to_bf16(v + 8 * k));
-      } else {
-        slot_out = c.pool_s + (box & 1u) * 16384u;
-      }
-      if constexpr (ACT == MB200_ACT_GELU_NEW) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_new_f(v[j]);
-      } else if constexpr (ACT == MB200_ACT_QUICK_GELU) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = quick_gelu_f(v[j]);
-      } else if constexpr (ACT == MB200_ACT_RELU) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      }
-      if constexpr (DACT != 0) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float a8[8];
-          bf16x8_to_f32(cur[0][k], a8);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            if constexpr (DACT == MB200_DACT_GELU_NEW) v[k * 8 + e] *= gelu_new_grad_f(a8[e]);
-            else v[k * 8 + e] = a8[e] > 0.f ? v[k * 8 + e] : 0.f;
-          }
-        }
-      }
-      if constexpr (NRES >= 1) {
-        constexpr int r0 = DACT != 0 ? 1 : 0;
-#pragma unroll
-        for (int i = 0; i < NRES; ++i) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float a8[8];
-            bf16x8_to_f32(cur[r0 + i][k], a8);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[k * 8 + e] += a8[e];
-          }
-        }
-        if (p.act == MB200_ACT_RELU_POST) {  // warp-uniform
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-      }
-      if (has_tail) {
-        bf16* crow = reinterpret_cast<bf16*>(p.C) + c.boff + (long long)grow * p.ldc + n0;
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (n0 + j >= n16 && n0 + j < p.N) crow[j] = __float2bfloat16(v[j]);
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        sts128u(slot_out + row_s + (((uint32_t)(half * 4 + k) ^ sw) << 4), f32x8_to_bf16(v + 8 * k));
-      if (half == 1 || ch + 1 == n_valid_ch) {
-        const int col0 = n0 - half * 32;
-        if constexpr (AUX) {
-          fence_proxy_async_smem();
-          epi_bar_sync();
-          if (elected) {
-            tma_store_4d(c.tmC, slot_out, col0, c.row_cta0, c.z0, c.z1);
-            tma_store_4d(c.tmAux, slot_aux, col0, c.row_cta0, c.z0, c.z1);
-            tma_store_commit();
-          }
-        } else {
-          epi3_publish<false>(c, c.tmC, slot_out, col0, elected);
-        }
-        ++box;
-      }
-    }
-    if constexpr (NIN > 0) {
-#pragma unroll
-      for (int i = 0; i < NIN; ++i)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          cur[i][k] = nxt[i][k];
-          nxt[i][k] = nx2[i][k];
-        }
+      v0 = a.x > 0.f ? v0 : 0.f;
+      v1 = a.y > 0.f ? v1 : 0.f;
     }
   }
-  if (n_valid_ch <= 0) {  // (cannot happen: tiles start inside the matrix) keep the TMEM protocol intact regardless
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-      if (c.empty_remote) mbar_arrive_remote(c.tmem_empty, 0);
-      else mbar_arrive(c.tmem_empty);
+  const long long roff = boff + (long long)row * p.ld_res + col;
+  if (p.res1) {
+    if (two) {
+      const float2 r = bf16x2_to_f32(ldg32(p.res1 + roff));
+      v0 += r.x;
+      v1 += r.y;
+    } else {
+      v0 += __bfloat162float(p.res1[roff]);
     }
+  }
+  if (p.res2) {
+    if (two) {
+      const float2 r = bf16x2_to_f32(ldg32(p.res2 + roff));
+      v0 += r.x;
+      v1 += r.y;
+    } else {
+      v0 += __bfloat162float(p.res2[roff]);
+    }
+  }
+  if (p.act == MB200_ACT_RELU_POST) {
+    v0 = fmaxf(v0, 0.f);
+    v1 = fmaxf(v1, 0.f);
+  }
+  if (p.c_f32) {
+    float* dst = reinterpret_cast<float*>(p.C) + coff;
+    if (two) {
+      float2 o = make_float2(v0, v1);
+      if (p.accumulate) {
+        const float2 old = *reinterpret_cast<const float2*>(dst);
+        o.x += old.x;
+        o.y += old.y;
+      }
+      *reinterpret_cast<float2*>(dst) = o;
+    } else {
+      dst[0] = p.accumulate ? dst[0] + v0 : v0;
+    }
+  } else {
+    bf16* dst = reinterpret_cast<bf16*>(p.C) + coff;
+    if (two) *reinterpret_cast<uint32_t*>(dst) = f32x2_to_bf16(v0, v1);
+    else dst[0] = __float2bfloat16(v0);
   }
 }
 
-// host helpers shared by gemm.cu / gemm2.cu
+// row0: first row (within the batch) of this warpgroup's 64-row slab; col0: first column of the tile
+template <int BN>
+__device__ __forceinline__ void epi_fragment(const GemmKernelParams& p, const float (&acc)[BN / 2], long long boff,
+                                             int row0, int col0, int ks) {
+  const int wt = threadIdx.x & 127;
+  const int r = row0 + (wt >> 5) * 16 + ((wt & 31) >> 2);
+  const int c = col0 + 2 * (wt & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    if (col0 + 8 * j >= p.N) break;  // warp-uniform
+    epi_pair(p, boff, r, c + 8 * j, acc[4 * j], acc[4 * j + 1], ks);
+    epi_pair(p, boff, r + 8, c + 8 * j, acc[4 * j + 2], acc[4 * j + 3], ks);
+  }
+}
+
+// host helper shared by gemm.cu / attention.cu
 int make_operand_map(CUtensorMap* out, const mb200_operand& op, int rows, int K, int nb0, int nb1, int box_rows);
-int make_store_map(CUtensorMap* out, const void* ptr, bool f32, int N, int M, int nb0, int nb1, long long ld,
-                   long long bs0, long long bs1);
-int launch_gemm2(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmAux,
-                 const CUtensorMap& tmWs, const GemmKernelParams& kp, bool a_mn, bool b_mn, bool f32, cudaStream_t stream);
 
 }  // namespace mb200

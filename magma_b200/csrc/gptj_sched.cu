@@ -20,9 +20,8 @@
 // GEMM, wgrad only for adapters.
 //
 // No kernels and no CUDA calls here (sched_rt.h): tests/test_sched_emul_cpu.py compiles this file as plain C++ against
-// oracle/cabi_emul.cpp and checks every adapter form against torch autograd of the oracle on the CPU; on the B200 it is
-// the path every LM test and the benchmark run (measured equal to the round-1 engine.cu schedule it replaced:
-// profiles/r02_bench_n1_general_schedule.json.log).
+// oracle/cabi_emul.cpp and checks every adapter form against torch autograd of the oracle on the CPU; on the GPU it is
+// the path every LM test and the benchmark run.
 #include "sched_rt.h"
 
 #include <math.h>

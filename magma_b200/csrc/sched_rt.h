@@ -14,7 +14,7 @@
 
 namespace mb200 {
 void set_error(const char* fmt, ...);
-int rt_check_arch();                                                   // 0 on sm_100, else MB200_E_ARCH
+int rt_check_arch();                                                   // 0 on sm_90, else MB200_E_ARCH
 int rt_copy(void* dst, const void* src, size_t bytes, void* stream);   // device-to-device, stream-ordered
 int rt_zero(void* dst, size_t bytes, void* stream);                    // stream-ordered memset(0)
 }  // namespace mb200

@@ -5,12 +5,12 @@
 // image encoder on the training path: loss.backward() (magma/train_loop.py:18) then runs through
 // ImagePrefix.proj into the encoder, and the optimizer gives the encoder its own learning rate
 // (magma/utils.py:173-177). The training schedule is the ViT half of that: the inference forward below with every
-// layer's activations kept, and the matching backward — dgrad and wgrad of every linear on the tcgen05 GEMM core with
+// layer's activations kept, and the matching backward — dgrad and wgrad of every linear on the GEMM core with
 // MN-major operands (no transposed copies), attention backward as strided batched GEMMs on the fused qkv buffer,
 // LayerNorm / softmax / QuickGELU backward and the bias / LN-parameter / positional reductions as HBM-bound kernels.
 //
 // Reference arithmetic (absent openai/CLIP; stand-in hf:clip/modeling_clip.py:138-219,282-386,647-694,1015-1069 —
-// SURVEY.md §8c); the backward is the autograd of that forward and is checked against torch autograd of the oracle.
+// the oracle); the backward is the autograd of that forward and is checked against torch autograd of the oracle.
 //
 // This file contains no kernels and no CUDA calls (see sched_rt.h): tests/ dry-run it on the CPU against
 // oracle/cabi_emul.cpp. Attention (T = 257 for ViT-L/14, head_dim 64, no mask) runs in the fused multi-tile kernel

@@ -1,6 +1,6 @@
 """Data-parallel host logic (pure Python, device-agnostic so it is testable with gloo on CPU).
 
-The reference's only parallelism is DP under DeepSpeed ZeRO-2 (train.py:103-111, SURVEY.md §2.1). Here every rank
+The reference's only parallelism is DP under DeepSpeed ZeRO-2 (train.py:103-111). Here every rank
 holds the full (frozen) model and a flat fp32 gradient arena for the ~0.24 B trainable parameters; the arena is
 laid out in the order gradients become ready in backward (last GPT-J layer first, image prefix last) and is
 all-reduced slice by slice as backward proceeds."""
@@ -63,8 +63,8 @@ def allreduce_slice(flat_grad: torch.Tensor, lo, hi, group=None, comm_dtype=None
 
 
 def exchange_mode() -> str:
-    """'nccl' (default) or 'peer' (MB200_DP_EXCHANGE): which mechanism carries the gradient exchange. Both are built,
-    parity-tested on 2 GPUs and measured (DESIGN.md section 4 / 6)."""
+    """'nccl' (default) or 'peer' (MB200_DP_EXCHANGE): which mechanism carries the gradient exchange. Both are built
+    and parity-tested on 2 GPUs."""
     import os
 
     m = os.environ.get("MB200_DP_EXCHANGE", "nccl").lower()
@@ -109,10 +109,8 @@ class PeerExchange:
 
     Why: NCCL's all-reduce kernels need shared memory, so each of their CTAs needs an SM of its own; the persistent GEMM
     grids of backward own every SM, the collective only gets SMs at kernel boundaries, and the GEMM whose CTAs it
-    displaces runs a second wave — measured on 2 x B200 the exchange cost the step its full isolated duration (1.8 ms of
-    31.2) whatever the NCCL channel count, bucket count, SM carve-out or wire dtype (profiles/r02_n2_dp_sweep.log,
-    r02_scaling_n2.log). The kernel here uses no shared memory and ~40 registers, so its blocks sit BESIDE the GEMM CTAs
-    (the pair GEMM leaves 26 k registers per SM free, csrc/gemm2.cu).
+    displaces runs a second wave. The kernel here uses no shared memory and ~40 registers, so its blocks can sit BESIDE
+    the GEMM CTAs.
 
     Layout: the arena's fp32 gradient buffer is symmetric memory (torch.distributed._symmetric_memory: allocation, handle
     exchange and the device-side barrier are torch's; the data path is ours), so the exchange works IN PLACE. Per slice,
@@ -156,7 +154,7 @@ class PeerExchange:
 
 
 def shard_batch(global_batch: int, rank: int, world: int) -> Tuple[int, int]:
-    """Rank `rank` takes samples [lo, hi) of the global batch (SURVEY.md §8e: rank i takes [8i, 8i+8))."""
+    """Rank `rank` takes samples [lo, hi) of the global batch (rank i takes [8i, 8i+8))."""
     per = global_batch // world
     assert per * world == global_batch, "global batch must divide evenly across ranks"
     return rank * per, (rank + 1) * per

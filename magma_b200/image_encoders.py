@@ -2,13 +2,13 @@
 
 The reference obtains its encoders from openai/CLIP (`clip.load(name)[0].visual`, image_encoders.py:65) and timm;
 neither package is vendored. This module implements CLIP's VisionTransformer family natively (patchify-conv as
-im2col + tcgen05 GEMM, 24x [LN -> QKV GEMM+bias -> attention -> out GEMM+bias+residual -> LN -> fc GEMM+bias+
+im2col + GEMM, 24x [LN -> QKV GEMM+bias -> attention -> out GEMM+bias+residual -> LN -> fc GEMM+bias+
 QuickGELU -> proj GEMM+bias+residual], ln_post(CLS) @ proj) with openai/CLIP's parameter names, and extends the
 reference's name table with `clip_vit_large` (ViT-L/14, BASELINE.json config 2) following the reference's own ViT
 convention (pooled [b, D] features; `"clip"` = ViT-B/32 -> 512, image_prefix.py:18).
 
 CLIP's conv trunks (`clip_resnet` = RN50x4, `clip_resnet_large` = RN50x16, the encoder MAGMA_v1.yml ships with) are
-implemented as `B200ModifiedResNet`: NHWC bf16 activations, 1x1 convolutions as plain tcgen05 GEMMs, 3x3 convolutions
+implemented as `B200ModifiedResNet`: NHWC bf16 activations, 1x1 convolutions as plain GEMMs, 3x3 convolutions
 as im2col + GEMM, eval-mode BatchNorm folded into the packed weights / GEMM bias, ReLU and the bottleneck residual in
 the GEMM epilogue, the anti-aliasing average pools as one HBM-bound kernel; attention pool replaced by the
 "b d h w -> b (h w) d" reshape exactly as the reference does (image_encoders.py:69-74). timm's `nfresnet50` raises.
@@ -27,7 +27,7 @@ from ._lib import MB200Error, VitGradsC, VitLayerC, VitLayerGradsC, VitModelC, c
 VIT_CONFIGS = {
     "clip": (768, 12, 12, 32, 224, 3072, 512),             # ViT-B/32 (image_encoders.py:56-57)
     "ViT-B/32": (768, 12, 12, 32, 224, 3072, 512),
-    "clip_vit_large": (1024, 24, 16, 14, 224, 4096, 768),  # ViT-L/14 (extension, SURVEY.md fact 2)
+    "clip_vit_large": (1024, 24, 16, 14, 224, 4096, 768),  # ViT-L/14 (extension)
     "ViT-L/14": (1024, 24, 16, 14, 224, 4096, 768),
 }
 
@@ -384,15 +384,15 @@ class B200ModifiedResNet(nn.Module):
     statistics by `col_moments`, normalisation + residual + ReLU by `channel_affine`, running statistics updated with
     momentum 0.1) and a hand-scheduled backward — BatchNorm / ReLU backward from the same two kernels, convolution
     wgrad and dgrad as GEMMs over the saved im2col matrix (MN-major operands), `col2im3x3` and `avgpool_nhwc_bwd` as
-    the adjoints of the layout kernels. NOT YET RUN ON A B200 (DESIGN.md §3.10); dry-run on the CPU against the
-    oracle's autograd in tests/test_host_dryrun_cpu.py."""
+    the adjoints of the layout kernels. Checked on the GPU in tests/test_training_paths_gpu.py and dry-run on the CPU
+    against the oracle's autograd in tests/test_host_dryrun_cpu.py."""
 
     supports_training = True
     bn_momentum = 0.1
     # The reference never puts a frozen encoder in eval(): under model.train() its BatchNorm layers use batch statistics
     # and keep updating their running statistics even when freeze_img_encoder is true (magma/magma.py:98-100 only clears
     # requires_grad). Setting this to True reproduces that (forward through the training-mode schedule, no backward);
-    # the default keeps the frozen trunk on the GPU-verified folded path until the training kernels have run on a B200.
+    # the default keeps the frozen trunk on the folded (eval-mode BatchNorm) path.
     bn_batch_stats_when_frozen = False
 
     def __init__(self, layers, width, input_resolution, device=None):
@@ -689,7 +689,7 @@ def clip_encoder(device=None, name: str = "clip") -> nn.Module:
 def get_image_encoder(name: str, device=None, pretrained: bool = False) -> nn.Module:
     """magma/image_encoders.py:79-91. Weights are uninitialised/random: no checkpoint source exists offline."""
     if name == "nfresnet50":
-        raise NotImplementedError("nfresnet50 (timm NF-ResNet conv trunk) is not re-backed (SURVEY.md §8f rank 1)")
+        raise NotImplementedError("nfresnet50 (timm NF-ResNet conv trunk) is not re-backed")
     if "clip" in name or name in VIT_CONFIGS or name in RESNET_CONFIGS:
         return clip_encoder(device=device, name=name)
     raise ValueError(f"image encoder {name} not recognized")

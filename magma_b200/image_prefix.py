@@ -1,5 +1,5 @@
 """ImagePrefix — drop-in for magma/image_prefix.py: enc(x) -> Linear(enc_dim, out_dim*seq) -> reshape -> Dropout ->
-LayerNorm, with the projection on the tcgen05 GEMM core (bias fused), dropout and LayerNorm as bf16 kernels, and a
+LayerNorm, with the projection on the wgmma GEMM core (bias fused), dropout and LayerNorm as bf16 kernels, and a
 hand-written backward (wgrad GEMM with MN-major operands, bias/LN-parameter reductions) that writes fp32 gradients
 straight into the trainable-parameter arena."""
 import torch

@@ -1,6 +1,6 @@
 """GPT-J language model — drop-in for magma/language_model.py (`get_gptj`) re-backed by the C++/CUDA runtime.
 
-`get_gptj()` returns an object that honours every use the reference makes of its LM (SURVEY.md §8b):
+`get_gptj()` returns an object that honours every use the reference makes of its LM:
 `.config.{max_position_embeddings,hidden_size,pad_token_id}`, `.resize_token_embeddings(n)`, `.transformer.wte`
 (callable on int64 ids), `.transformer.h[l].{mlp,attn}` (get/settable — the seam `Magma.add_adapters` rewires,
 magma/magma.py:128-169), `named_parameters()` with "adapter" in adapter names, and
@@ -8,7 +8,7 @@ magma/magma.py:128-169), `named_parameters()` with "adapter" in adapter names, a
 object with `.loss`, `.logits`, `.past_key_values`.
 
 All frozen weights are bf16 tensors on the GPU; parameter names follow HF GPT-J (`attn.q_proj.weight`, `mlp.fc_in.*`,
-`ln_1`, `ln_f`, `lm_head`) — the executable stand-in for the reference's fork (SURVEY.md §8c). The whole
+`ln_1`, `ln_f`, `lm_head`) — the executable stand-in for the reference's fork. The whole
 28-block forward and backward run inside libmagma_b200.so (csrc/gptj_sched.cu); this file only owns tensors and plumbing.
 """
 import ctypes
@@ -229,7 +229,7 @@ class B200GPTJForCausalLM(nn.Module):
     # ---- construction helpers -------------------------------------------------------------
     @torch.no_grad()
     def init_weights(self, seed=0, std=0.02):
-        """Synthetic weights of the benchmark protocol (SURVEY.md §8d): N(0, 0.02) linears, LN ~ (1, 0)."""
+        """Synthetic weights of the benchmark protocol: N(0, 0.02) linears, LN ~ (1, 0)."""
         g = torch.Generator(device=self._device).manual_seed(seed)
         for name, p in self.named_parameters():
             if "adapter" in name:

@@ -1,9 +1,9 @@
 """Magma — same public API as magma/magma.py (`Magma(config, device)`, `forward`, `embed`, `preprocess_inputs`,
 `generate`, `add_adapters`, `from_checkpoint`), assembled from the re-backed components.
 
-Differences from the reference, all deliberate and documented in DESIGN.md:
+Differences from the reference, all deliberate:
   * the LM is really frozen when `freeze_lm` is set (the reference only sets requires_grad=True on adapters and
-    never False on anything, magma/magma.py:93-96 — SURVEY.md fact 4);
+    never False on anything, magma/magma.py:93-96);
   * `seq_len` defaults to the LM's max_position_embeddings (2048) like the reference but honours `config.seq_len`
     and stays a plain attribute (`model.seq_len = 128`);
   * the word embedding is gathered straight into the fused [B,S,d] input buffer (the reference embeds the full
@@ -90,7 +90,7 @@ class Magma(nn.Module):
 
             self.transforms = get_transforms(config.image_size, config.encoder_name,
                                              input_resolution=self.image_prefix.enc.input_resolution)
-        except Exception as e:  # torchvision / PIL preprocessing is host-side and optional (SURVEY.md §2 row 16)
+        except Exception as e:  # torchvision / PIL preprocessing is host-side and optional
             self.transforms, self._transforms_error = None, e
 
         if config.adapter_config:
@@ -125,7 +125,7 @@ class Magma(nn.Module):
 
     def _require_cuda(self):
         if self.device.type != "cuda":
-            raise RuntimeError("magma_b200 has no CPU path: construct Magma on a CUDA (sm_100) device")
+            raise RuntimeError("magma_b200 has no CPU path: construct Magma on a CUDA (sm_90) device")
 
     # ------------------------------------------------------------------------------------------
     def finalize(self):
@@ -255,7 +255,7 @@ class Magma(nn.Module):
     @classmethod
     def from_checkpoint(cls, config_path, checkpoint_path, device="cuda"):
         """magma/magma.py:278-301. The published checkpoint uses the fork's parameter names; checkpoint.py maps them
-        onto this module's names (SURVEY.md §8f rank 2) and a mismatch raises instead of loading partially."""
+        onto this module's names and a mismatch raises instead of loading partially."""
         import os
 
         if not os.path.exists(checkpoint_path):

@@ -61,7 +61,7 @@ def gemm(
     splitk_ws=None,
     b_static=False,
 ):
-    """C[..., M, N] = epilogue(alpha * A @ B^T) on the tcgen05 GEMM core.
+    """C[..., M, N] = epilogue(alpha * A @ B^T) on the wgmma GEMM core.
 
     A is [..., M, K] (a_mn=False) or [..., K, M] (a_mn=True); B is [..., N, K] (b_mn=False) or
     [..., K, N] (b_mn=True). Up to two leading batch dims with arbitrary (8-element aligned) strides.

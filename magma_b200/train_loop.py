@@ -2,7 +2,7 @@
 stands where the DeepSpeed engine stood (train.py:103-111): `engine(images, captions)`, `engine.backward(loss)`,
 `engine.step()`.
 
-Data parallelism is the reference's only strategy (SURVEY.md §2.1). With the LM frozen the only exchange is the
+Data parallelism is the reference's only strategy. With the LM frozen the only exchange is the
 gradient of the ~0.24 B trainable parameters, which live in one flat fp32 arena: the engine sums contiguous arena
 slices across ranks (NCCL all-reduce, or this package's peer-memory kernel: dp.PeerExchange) on a side stream as soon as
 the backward pass has finished the layers they belong to (backward is issued in layer chunks), so the exchange overlaps
@@ -35,32 +35,29 @@ class B200Engine:
         # The optimizer (global-norm reduction + fused AdamW: 7.2 GB of HBM traffic, ~1.4 ms at 6 B scale) is issued on
         # its own stream, ordered after backward and the gradient exchange. Nothing in the next step reads a trainable
         # parameter before the image prefix projection, so with a frozen encoder it runs beside the next step's encoder
-        # forward, and at N > 1 the tail of the gradient exchange hides there too. Measured (DESIGN.md section 6): the
-        # overlap happens, the power-capped step itself moves by < 0.1 ms, end to end it is worth 0.3-0.5 ms. Consumers
-        # are ordered by ParamArena.wait_ready() (called from sync_shadow(), i.e. by every forward);
+        # forward, and at N > 1 the tail of the gradient exchange hides there too. Consumers are ordered by ParamArena.wait_ready() (called from sync_shadow(), i.e. by every forward);
         # MB200_PIPELINE_OPT=0 puts the optimizer back on the caller's stream.
         self.opt_stream = torch.cuda.Stream() if (on_gpu and os.environ.get("MB200_PIPELINE_OPT", "1") != "0") else None
         if self.opt_stream is not None:
-            # 2 optimizer blocks per SM fit in the registers a persistent GEMM CTA leaves free (csrc/gemm2.cu: 152 of 256
-            # per thread after setmaxnreg); the default 16 per SM would own every SM until the optimizer is done
+            # a few optimizer blocks per SM run beside the persistent GEMM grids; the default 16 per SM would own every
+            # SM until the optimizer is done
             from ._lib import lib
 
             n_sm = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
             lib().mb200_set_optimizer_grid(int(os.environ.get("MB200_OPT_BLOCKS_PER_SM", "2")) * n_sm)
-        # data-parallel knobs, both off by default and both measured without effect at N = 2 (DESIGN.md section 4,
-        # profiles/r02_n2_dp_sweep.log): exchange gradients as bf16, and keep a few SMs out of the persistent GEMM grids
-        # so NCCL's CTAs run beside the backward GEMMs
+        # data-parallel knobs, both off by default: exchange gradients as bf16, and keep a few SMs out of the persistent
+        # GEMM grids so NCCL's CTAs run beside the backward GEMMs
         self.comm_dtype = torch.bfloat16 if os.environ.get("MB200_DP_BF16", "0") == "1" else None
         # SM carve-out for the gradient exchange: while an all-reduce is in flight (from the first bucket issued in
-        # backward until the optimizer step has waited for the last one) the persistent GEMM grids leave 148 - n SMs
-        # alone, so NCCL's CTAs run BESIDE the backward GEMMs instead of queueing behind 148-CTA grids (each NCCL CTA
+        # backward until the optimizer step has waited for the last one) the persistent GEMM grids leave all but n SMs
+        # alone, so NCCL's CTAs run BESIDE the backward GEMMs instead of queueing behind full-width grids (each NCCL CTA
         # otherwise takes an SM at a kernel boundary and the next GEMM's last CTAs start only when it leaves).
         # Outside that window every kernel gets all SMs. MB200_DP_GEMM_SMS=0 disables it.
         self.dp_gemm_sms = int(os.environ.get("MB200_DP_GEMM_SMS", "0")) if self.world > 1 else 0
         self._carved = False
         # Gradient exchange: NCCL all-reduce per slice, or (MB200_DP_EXCHANGE=peer) this package's peer-memory kernel
         # (dp.PeerExchange); which one ran is in self.exchange_kind (bench.py prints it). dp.exchange_mode() has the
-        # default and DESIGN.md section 6 the measurements behind it.
+        # default.
         self.peer = None
         self.exchange_kind = "none" if self.world == 1 else "nccl"
         if self.world > 1 and on_gpu and self.comm_dtype is None and dp.exchange_mode() == "peer":

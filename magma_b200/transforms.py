@@ -1,5 +1,5 @@
 """Image preprocessing — drop-in for magma/transforms.py (`get_transforms`, `clip_preprocess`, `pad_to_size_tensor`).
-Host-side PIL / torch code: nothing here is on the accelerated path (SURVEY.md §8 row a3), it only has to hand the
+Host-side PIL / torch code: nothing here is on the accelerated path, it only has to hand the
 encoder the same [1, 3, R, R] tensor the reference does.
 
 `clip_preprocess` is written directly on PIL + torch (resize the short side with bicubic resampling, centre crop or

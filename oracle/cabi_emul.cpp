@@ -438,7 +438,7 @@ int mb200_prof_read(double* a, double* b, double* c, long long* n) {
   *n = 0;
   return 0;
 }
-int mb200_set_gemm_sm_limit(int) { return 148; }
+int mb200_set_gemm_sm_limit(int) { return 132; }
 int mb200_set_optimizer_grid(int n) { return n; }
 
 int mb200_rope(void* qkv_, int64_t ld, int32_t rows, int32_t S, int32_t H, int32_t hd, int32_t rot, int32_t pos0,

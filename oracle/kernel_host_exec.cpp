@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — executes CUDA KERNEL SOURCE of the product on the CPU.
 //
-// The kernels added after the last GPU session (magma_b200/csrc/train_kernels.cuh) have not run on a B200 yet. Their
-// schedules are dry-run with emulated operators (cabi_emul.cpp), but that says nothing about the kernel code itself.
+// The training kernels (magma_b200/csrc/train_kernels.cuh) are checked on the GPU by tests/test_training_paths_gpu.py. Their
+// schedules are also dry-run with emulated operators (cabi_emul.cpp), but that says nothing about the kernel code itself.
 // This file compiles the kernel source UNCHANGED (the same .cuh fragments elementwise.cu includes) as host C++ and runs
 // it with the CUDA execution model emulated: every thread of a block is an OS thread with its own threadIdx, blocks run
 // one after another, `__shared__` is block-shared static storage, `__syncthreads()` a block barrier,

@@ -3,14 +3,14 @@
 Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / `--impl reference` leg may import this
 module, and only as the checker / reported CPU baseline. Nothing in `magma_b200/` imports it.
 
-Parity status: the reference repository ships no tests or golden vectors (SURVEY.md §4), so this oracle is
-pinned against *outputs of the reference itself run in the build container*: `oracle/make_golden.py` imports
-the reference's own `magma.{adapters,image_prefix,magma,utils,sampling}` from /root/reference under shims
+Parity status: the reference repository ships no tests or golden vectors, so this oracle is
+pinned against *outputs of the reference itself*: `oracle/make_golden.py` imports
+the reference's own `magma.{adapters,image_prefix,magma,utils,sampling}` from a reference checkout under shims
 (oracle/ref_shims.py), with mainline HF `GPTJForCausalLM` / `CLIPVisionModelWithProjection` standing in for the
 un-vendored transformers fork / openai-CLIP, and writes the fixtures in tests/golden/. tests/test_oracle_golden.py
 checks every function below against those fixtures.
 
-Each function cites the reference lines it restates (paths relative to /root/reference, or
+Each function cites the reference lines it restates (paths relative to the reference repository's root, or
 `hf:` = site-packages/transformers).
 
 Weight naming follows the reference state dict (magma/magma.py:52-53,143-149; HF GPT-J names for the LM,
@@ -454,7 +454,7 @@ def remove_tokens_after_eos(tensor, eos_token, image_token):
 
 
 # ------------------------------------------------------------------------------------------------
-# synthetic weights (SURVEY.md §8d): normal(0, 0.02) linears, LN 1/0, adapters per adapters.py:28-36
+# synthetic weights: normal(0, 0.02) linears, LN 1/0, adapters per adapters.py:28-36
 # ------------------------------------------------------------------------------------------------
 def init_weights(cfg: OracleConfig, seed=0, with_vit=True, dtype=torch.float32) -> Dict[str, torch.Tensor]:
     g = torch.Generator().manual_seed(seed)
@@ -530,7 +530,7 @@ def init_weights(cfg: OracleConfig, seed=0, with_vit=True, dtype=torch.float32) 
 
 
 def synthetic_batch(cfg: OracleConfig, B, S, seed=1234, prefix_len=None):
-    """SURVEY.md §8d: images ~ N(0,1); captions randint(0, 50256) with per-row length U[S/4, S-L], EOS padded
+    """Synthetic batch: images ~ N(0,1); captions randint(0, 50256) with per-row length U[S/4, S-L], EOS padded
     (mimics tokenizer(..., padding='max_length') with pad=eos; datasets/dataset.py:136-142)."""
     g = torch.Generator().manual_seed(seed)
     L = cfg.image_seq_len if prefix_len is None else prefix_len

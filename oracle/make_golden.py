@@ -1,12 +1,12 @@
-"""TEST INFRASTRUCTURE — generates tests/golden/*.pt by running the REFERENCE ITSELF in the build container.
+"""TEST INFRASTRUCTURE — generates tests/golden/*.pt by running the REFERENCE ITSELF.
 
-    python oracle/make_golden.py          # needs /root/reference (read-only) and the offline HF transformers
+    python oracle/make_golden.py          # needs MAGMA_REFERENCE_ROOT (a reference checkout) and HF transformers
 
 What runs: the reference's own Python (`magma.adapters.Adapter*`, `magma.image_prefix.ImagePrefix`,
 `magma.utils.build_labels`, `magma.sampling.{top_k_filter,top_p_filter,generate}`, `magma.magma.Magma.__init__ /
-forward / embed / generate`) imported from /root/reference under the shims of oracle/ref_shims.py, with mainline HF
+forward / embed / generate`) imported from the reference checkout under the shims of oracle/ref_shims.py, with mainline HF
 `GPTJForCausalLM` (eager attention) standing in for the reference's un-vendored transformers fork and HF
-`CLIPVisionModelWithProjection` standing in for openai/CLIP's VisionTransformer (SURVEY.md §8c). Everything is fp32
+`CLIPVisionModelWithProjection` standing in for openai/CLIP's VisionTransformer. Everything is fp32
 on CPU with seeded random weights at tiny sizes, so the fixtures stay small. Inputs, weights (re-keyed to the
 oracle's naming = the reference state-dict naming) and outputs are stored; tests/test_oracle_golden.py replays the
 inputs through oracle/magma_oracle.py and compares.
@@ -172,7 +172,7 @@ def main():
                     p.copy_(torch.where(torch.rand(p.shape, generator=gm) < 0.5, -3.0, 3.0)
                             + 0.02 * torch.randn(p.shape, generator=gm))
         model.eval()
-        model.seq_len = S  # SURVEY.md fact 3: plain attribute
+        model.seq_len = S  # plain attribute
         gi = torch.Generator().manual_seed(100 + i)
         images = torch.randn(B, 3, 32, 32, generator=gi)
         caps = torch.randint(0, 250, (B, S), generator=gi)

@@ -1,6 +1,6 @@
-"""TEST INFRASTRUCTURE — golden vectors for the host-side image preprocessing (SURVEY.md §8 row a3), produced by the
-REFERENCE's own magma/transforms.py (loaded from /root/reference; it only needs torchvision + PIL, both present in the
-build container). Run here once; the fixture travels with the repo: tests/golden/clip_preprocess.pt."""
+"""TEST INFRASTRUCTURE — golden vectors for the host-side image preprocessing, produced by the
+REFERENCE's own magma/transforms.py (loaded from the checkout named by MAGMA_REFERENCE_ROOT; it only needs torchvision +
+PIL). Run once; the fixture travels with the repo: tests/golden/clip_preprocess.pt."""
 import importlib.util
 import os
 
@@ -27,7 +27,8 @@ def to_pil(arr, mode):
 
 
 def main():
-    spec = importlib.util.spec_from_file_location("ref_transforms", "/root/reference/magma/transforms.py")
+    spec = importlib.util.spec_from_file_location("ref_transforms", os.path.join(os.environ["MAGMA_REFERENCE_ROOT"], "magma",
+                                                                              "transforms.py"))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)
     rec = {"cases": [], "pad_to_size_tensor": []}

@@ -1,23 +1,25 @@
-"""TEST INFRASTRUCTURE — loads the *reference's own* Python (Aleph-Alpha/magma, /root/reference) under shims.
+"""TEST INFRASTRUCTURE — loads the *reference's own* Python (a checkout of Aleph-Alpha/magma whose root is given by the
+environment variable MAGMA_REFERENCE_ROOT) under shims.
 
-Only usable in the build container (where /root/reference is mounted); used by oracle/make_golden.py to pin
+Only usable where that checkout exists; used by oracle/make_golden.py to pin
 the CPU restatement in oracle/magma_oracle.py and to generate the committed fixtures under tests/golden/.
 Nothing on the product path, in `-m gpu` tests, smoke() or bench.py imports this module.
 
-The reference cannot be imported as-is (SURVEY.md §8c): torchtyping, deepspeed, gdown, clip, timm are absent
+The reference cannot be imported as-is: torchtyping, deepspeed, gdown, clip, timm are absent
 and it depends on a transformers fork. The stubs below only satisfy import-time names; the arithmetic that
 runs is the reference's own `magma.{adapters,image_prefix,magma,utils,sampling}` plus mainline HF GPT-J
 (`transformers.models.gptj`) standing in for the fork's GPTNeo(jax=True, rotary=True) and HF CLIP-ViT standing
 in for openai/CLIP's VisionTransformer.
 """
 import contextlib
+import os
 import sys
 import types
 
 import torch
 import torch.nn as nn
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("MAGMA_REFERENCE_ROOT", "")
 
 
 class _AnyType:
@@ -43,6 +45,8 @@ def install_stubs():
     clip.load = lambda *a, **k: (_ for _ in ()).throw(RuntimeError("clip is stubbed"))
     sys.modules.setdefault("clip", clip)
     sys.modules.setdefault("clip.model", clip.model)
+    if not os.path.isdir(os.path.join(REFERENCE_ROOT, "magma")):
+        raise RuntimeError("set MAGMA_REFERENCE_ROOT to a checkout of Aleph-Alpha/magma")
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)
 
@@ -80,7 +84,7 @@ def _bridge_attn_wrappers(magma_adapters):
 
 
 def load_reference(gptj_kwargs=None, encoder_factory=None, vocab=50258):
-    """Import the reference package and patch its three factory seams (SURVEY.md §8b):
+    """Import the reference package and patch its three factory seams:
     get_gptj -> HF GPTJForCausalLM, get_tokenizer -> StubTokenizer, get_image_encoder -> encoder_factory."""
     install_stubs()
     import magma.adapters as m_adapters

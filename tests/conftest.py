@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100 / B200) device; run with `-m gpu`")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90 / H100) device; run with `-m gpu`")
     config.addinivalue_line("markers", "timeout: per-test time limit (pytest-timeout; ignored when the plugin is absent)")
 
 
@@ -83,7 +83,7 @@ def emul_ops(monkeypatch):
 def kernel_ops(monkeypatch):
     """magma_b200/ops.py driven by KERNEL SOURCE executed on the CPU (oracle/kernel_host_exec.cpp: the product's .cuh kernel
     fragments compiled as host C++, CUDA thread model emulated) — for the elementwise / reduction operators only; there is
-    no GEMM or attention here (tcgen05 / TMA code cannot run on a CPU)."""
+    no GEMM or attention here (wgmma / TMA code cannot run on a CPU)."""
     import ctypes
 
     from magma_b200 import _lib, ops

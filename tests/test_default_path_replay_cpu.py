@@ -1,5 +1,5 @@
 """Replay of the DEFAULT paths on the CPU. The GPU parity harness itself (tools/model_check.py groups lm, lm_variants,
-vit, resnet, magma, generate — what tests/test_model_gpu.py runs on a B200), the reference-golden tests of that file and
+vit, resnet, magma, generate — what tests/test_model_gpu.py runs on the GPU), the reference-golden tests of that file and
 __graft_entry__.smoke() are executed here on CPU tensors. What runs is the product's own code: its Python, and its
 HOST-ONLY C++ schedules (csrc/gptj_sched.cu, csrc/vit_sched.cu — no kernels, no CUDA calls) compiled as plain C++ into
 the emulation library, issuing the primitive operators, which are what is emulated (oracle/cabi_emul.cpp). So a change

@@ -1,4 +1,4 @@
-"""CPU tests of the data-parallel host logic with torch.distributed(gloo), world_size 2 (SURVEY.md §8e):
+"""CPU tests of the data-parallel host logic with torch.distributed(gloo), world_size 2:
 sharding by batch + SUM all-reduce of contiguous arena slices in backward order reproduces the single-process
 gradient of the concatenated batch."""
 import os

@@ -1,4 +1,4 @@
-"""Hardware data-parallel parity (SURVEY.md section 4, "Distributed"): on 2 B200s, with the gradient exchange carried by
+"""Hardware data-parallel parity ("Distributed"): on 2 GPUs, with the gradient exchange carried by
 this package's peer-memory kernel (default), by NCCL, and by NCCL with a bf16 wire format, the gradients the engine
 holds after its overlapped exchange — divided by the world size, as the fused optimizer kernel does — equal the
 single-GPU gradients of the CONCATENATED batch, and one optimizer step leaves every rank with identical parameters
@@ -6,8 +6,7 @@ that equal the single-GPU step. Reference semantics: DeepSpeed data parallelism 
 gradients (train.py:103-111, magma/utils.py:26-34), which equals the gradient of the mean over the concatenated batch
 when every rank holds the same number of valid label tokens — the captions below are built that way.
 
-Needs 2 visible GPUs (run with `gpurun --gpus 2`); skipped otherwise. The 1-GPU driver run of `-m gpu` skips it; its
-logged outcome is profiles/r02_dp_parity_n2.log."""
+Needs 2 visible GPUs; skipped otherwise."""
 import os
 
 import pytest
@@ -95,7 +94,7 @@ def test_allreduced_gradients_equal_the_concatenated_batch(tmp_path, mode):
     import torch.multiprocessing as mp
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     world = 2
     comm_bf16 = mode == "nccl-bf16"
     port = 29500 + (os.getpid() % 1000) + {"peer": 0, "nccl": 7, "nccl-bf16": 14}[mode]

@@ -1,6 +1,6 @@
 """Host logic of the peer-memory gradient exchange (magma_b200/dp.py::PeerExchange): the shard partition, and the
 reduce + broadcast primitive's contract on the emulated C ABI — "ranks" are plain host buffers here; the kernel itself
-runs on 2 B200s in tests/test_dp_gpu.py."""
+runs on 2 GPUs in tests/test_dp_gpu.py."""
 import torch
 
 from magma_b200 import dp
@@ -34,7 +34,7 @@ def test_every_rank_ends_with_the_same_sum(emul_ops):
 
 
 def test_exchange_selection_and_plain_gradient_buffer_without_a_process_group(monkeypatch):
-    """NCCL is the default exchange (DESIGN.md section 4); the symmetric gradient buffer is only asked for in a multi-rank
+    """NCCL is the default exchange; the symmetric gradient buffer is only asked for in a multi-rank
     GPU job that selected the peer kernel — everywhere else (CPU, single process) the arena gets a plain zeroed buffer."""
     monkeypatch.delenv("MB200_DP_EXCHANGE", raising=False)
     assert dp.exchange_mode() == "nccl"

@@ -2,7 +2,7 @@
 every dry run in this suite is only as good as the emulation of mb200_gemm, so its operand majors, batch strides and the
 whole epilogue (bias, activations, saved pre-activation, derivative multipliers, residuals, fp32 accumulate, rotary
 embedding) are checked here on small shapes; the elementwise / reduction operators replay the same `group_ops` harness
-the real kernels are held to on a B200 (tests/test_ops_gpu.py)."""
+the real kernels are held to on the GPU (tests/test_ops_gpu.py)."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 GEMM core through the C ABI (mb200_gemm) against an fp32 matmul of the same bf16
+"""GPU parity tests of the wgmma GEMM core through the C ABI (mb200_gemm) against an fp32 matmul of the same bf16
 inputs. Tolerance: relative Frobenius error < 2e-2 (bf16 output rounding is ~2^-9 relative; fp32 outputs < 5e-3)."""
 import pytest
 

@@ -1,4 +1,4 @@
-"""The SOURCE of the kernels that have not run on a B200 yet (magma_b200/csrc/train_kernels.cuh), executed on the CPU.
+"""The SOURCE of the training kernels (magma_b200/csrc/train_kernels.cuh), executed on the CPU.
 
 oracle/kernel_host_exec.cpp compiles those kernels unchanged as host C++ and runs them with the CUDA execution model
 emulated (threads of a block = OS threads, __syncthreads = barrier, warp shuffles and atomicAdd emulated, blocks in
@@ -124,7 +124,7 @@ def test_avgpool_nhwc_bwd_kernel_source(kx):
 
 
 def test_gpu_verified_kernel_source_passes_the_gpu_ops_harness(kernel_ops, monkeypatch, capsys):
-    """Calibration of the executor itself: the kernels of csrc/elt_kernels.cuh ARE verified on a B200
+    """Calibration of the executor itself: the kernels of csrc/elt_kernels.cuh ARE verified on the GPU
     (tests/test_ops_gpu.py); executed on the CPU under the emulated thread model, their source passes the very same
     harness (LayerNorm fwd / bwd / parameter gradients, rotary, softmax fwd / bwd, build_labels bit-exact, cross-entropy,
     gathers, colsum, argmax tie rule, fused AdamW against torch.optim.AdamW, dropout) — so a pass of the NEW kernels under

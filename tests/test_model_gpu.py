@@ -2,7 +2,7 @@
 the drop-in Python API (Magma.forward / embed / generate, B200Engine) against the CPU oracle on identical seeded
 inputs, and against the golden fixtures produced by the REFERENCE ITSELF (tests/golden/, oracle/make_golden.py).
 
-Tolerances (bf16 kernels vs fp32 oracle, SURVEY.md §8c): |dloss| < 2e-2; logits rel-Frobenius < 3e-2; gradients
+Tolerances (bf16 kernels vs fp32 oracle): |dloss| < 2e-2; logits rel-Frobenius < 3e-2; gradients
 rel-Frobenius < 3e-2 — the reference-made fixtures and the full-size case use adapters whose ReLU masks are decided away
 from zero (down-projection biases of +-3), so that bf16 and fp32 agree on the mask; only tools/model_check.py's
 "free relu mask" case (a flipped mask entry is an O(1) relative error in that entry) uses a wider bound. Integer results
@@ -72,7 +72,7 @@ def test_vit_embed_generate_match_reference_golden(golden_dir):
     toks = model.generate(rec["embeddings"].to(dev).to(torch.bfloat16), max_steps=10, temperature=0.0, decode=False).cpu()
     ref = rec["greedy_tokens"]
     # Token ids are exact up to (not including) the first greedy step at which the reference's own top-1 / top-2 logit
-    # margin is a bf16 near-tie (SURVEY.md section 8c); logits here are O(1), one bf16 ulp of them is ~8e-3, and the
+    # margin is a bf16 near-tie; logits here are O(1), one bf16 ulp of them is ~8e-3, and the
     # accumulated bf16 error of the tiny model's logits is held to 3e-2 relative above.
     s0, tau = rec["embeddings"].shape[1], 0.05
     assert torch.equal(toks[:, :s0], ref[:, :s0])
@@ -145,7 +145,7 @@ def test_full_size_step_properties():
         if p.requires_grad:
             n_train += p.numel()
             assert p.grad is not None and torch.isfinite(p.grad).all(), n
-    assert n_train == 28 * 8_393_728 + 768 * 8192 + 8192 + 2 * 4096  # SURVEY.md §8d: 241.3 M trainable
+    assert n_train == 28 * 8_393_728 + 768 * 8192 + 8192 + 2 * 4096  # 241.3 M trainable
     g1 = model.arena.grad.clone()
     model(images, captions).loss.backward()  # grads live -> accumulate
     assert ((model.arena.grad - 2 * g1).norm() / (2 * g1).norm()).item() < 1e-2
@@ -235,7 +235,7 @@ def test_config2_full_size_matches_oracle():
     batch 2 (the oracle's fp32 forward + backward of 2 samples takes seconds on the host; the kernels, tile shapes and
     launch paths are those of the B = 8 benchmark step except for M = 256 instead of 1024 — the CTA-pair GEMM with
     K = 4096 / 16384, head_dim-256 fused attention, the 50258-wide LM head and cross-entropy).
-    Bars (SURVEY.md section 8c): |dloss| < 2e-2, logits rel-Frobenius < 3e-2, every trainable gradient < 3e-2."""
+    Bars: |dloss| < 2e-2, logits rel-Frobenius < 3e-2, every trainable gradient < 3e-2."""
     import torch
 
     from oracle import magma_oracle as O

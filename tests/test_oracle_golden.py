@@ -1,7 +1,7 @@
 """CPU tests: the oracle (oracle/magma_oracle.py) reproduces the outputs of the REFERENCE ITSELF.
 
 The fixtures in tests/golden/ were produced by oracle/make_golden.py, which runs the reference's own Python
-(imported from /root/reference under shims) with HF GPT-J / HF CLIP-ViT as the third-party arithmetic. fp32 on both
+(imported from a reference checkout under shims) with HF GPT-J / HF CLIP-ViT as the third-party arithmetic. fp32 on both
 sides, so tolerances are tight; integer results (labels, greedy token ids, filters' -inf pattern) must be identical.
 """
 import os
@@ -52,7 +52,7 @@ def test_sampling_filters_match_reference(golden_dir):
     assert torch.equal(O.top_k_filter(rec["logits"].clone(), 5), rec["top_k_5"])
     assert torch.equal(O.top_p_filter(rec["logits"].clone(), 0.9), rec["top_p_0.9"])
     assert torch.equal(O.top_p_filter(rec["logits"].clone(), 0.5), rec["top_p_0.5"])
-    # the inverted-nucleus behaviour of sampling.py:7-19 (SURVEY.md a15) is part of the contract
+    # the inverted-nucleus behaviour of sampling.py:7-19 is part of the contract
     q5 = O.top_p_filter(rec["quirk_probs"].clone(), 0.5)
     assert torch.equal(q5, rec["quirk_0.5"]) and torch.isinf(q5[0, 1]) and not torch.isinf(q5[0, 0])
     assert torch.equal(O.top_p_filter(rec["quirk_probs"].clone(), 0.9), rec["quirk_0.9"])

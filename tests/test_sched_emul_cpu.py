@@ -366,7 +366,7 @@ def test_gptj_schedule_fused_attention_tile_and_chunked_backward(emul):
 def test_launch_plan_trace_of_a_full_size_step():
     """tools/plan_trace.py: the product's own schedules issue a full-size training step (GPT-J-6B + ViT-L/14, B = 8,
     S = 128) on the emulation in trace mode — placeholder pointers, nothing touches memory — and the launch list carries the
-    algorithmic FLOPs of BASELINE.md §4 (LM forward + backward, frozen: 2 x 1.5635 + 0.0601 TFLOP/sample + ViT 0.162)."""
+    algorithmic FLOPs of bench.py (LM forward + backward, frozen: 2 x 1.5635 + 0.0601 TFLOP/sample + ViT 0.162)."""
     import os
     import sys
 
@@ -377,7 +377,7 @@ def test_launch_plan_trace_of_a_full_size_step():
     gemms = [r for r in rows if r["op"] == "gemm"]
     assert 650 < len(rows) < 900 and len(gemms) > 450
     tflop = sum(r["flops"] for r in rows) / 1e12
-    want = 8 * (2 * 1.5635 + 0.0601 + 0.1620)          # SURVEY.md §8d, per sample -> per step of 8
+    want = 8 * (2 * 1.5635 + 0.0601 + 0.1620)          # per sample -> per step of 8
     assert abs(tflop - want) / want < 0.03, (tflop, want)
     # the frozen-weight GEMMs of one block, forward: qkv, out, fc_in, fc_out at M = B*S = 1024
     shapes = {(int(r["args"]["M"]), int(r["args"]["N"]), int(r["args"]["K"])) for r in gemms}

@@ -1,8 +1,7 @@
 """GPU tests of the training paths beyond the frozen-encoder benchmark configuration: the ViT training schedule
 (csrc/vit_sched.cu), the add_layernorm / scaled_parallel adapter forms of the LM schedule (csrc/gptj_sched.cu),
 conv-trunk training (BatchNorm in training mode), the optimizer parameter groups, engine checkpoint resume, and the
-elementwise kernels written for them. All of them run on a B200 (first hardware run: round 2, gpurun call 1 —
-profiles/r02_training_paths_first_hw_run.log); nothing here is expected to fail.
+elementwise kernels written for them. Nothing here is expected to fail.
 tests/test_training_paths_twin_cpu.py replays the same bodies on emulated kernels."""
 import pytest
 
@@ -494,8 +493,7 @@ def test_conv_trunk_training_matches_oracle_like_with_like():
     pattern given to the oracle). Tolerances: the trunk stores 22 conv outputs + 22 unit outputs in bf16; once one
     stored value rounds the other way than the oracle's, everything downstream is a DIFFERENT set of bf16 roundings, so
     the two runs decorrelate at the 2^-8 level per store point and the features differ by ~sqrt(44) * 2^-8 ~ 2.6 % (the
-    first B200 run measured 2.4 %, the CPU emulation 0.6-2.1 % depending on the input size;
-    profiles/r02_training_paths_first_hw_run.log). That is the noise floor of an end-to-end comparison, not a kernel
+    CPU emulation gives 0.6-2.1 % depending on the input size). That is the noise floor of an end-to-end comparison, not a kernel
     error: test_conv_trunk_training_units_match_fp32_locally holds every unit to 5e-3 on the device's own inputs and
     test_conv_trunk_training_kernels_match_torch holds each backward kernel to 5e-3."""
     import torch

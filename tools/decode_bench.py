@@ -1,6 +1,6 @@
 """Decode benchmark (BASELINE.json config 5): Magma.generate, batch 32, 224x224 image prefix (+6 text tokens),
 256 autoregressive steps, temperature 0 (greedy), KV cache. Reports tokens/s and the HBM roofline fraction
-(algorithmic bytes/step = bf16 weights 12.16 GB + KV read; SURVEY.md §8d)."""
+(algorithmic bytes/step = bf16 weights 12.16 GB + KV read)."""
 import argparse
 import json
 import os

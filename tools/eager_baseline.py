@@ -1,4 +1,4 @@
-"""GPU-eager baseline (BASELINE.md §3 "GPU-eager"): the reference assembly in plain PyTorch on the same B200 —
+"""GPU-eager baseline: the reference assembly in plain PyTorch on the same GPU —
 HF GPTJForCausalLM (eager attention; the executable stand-in for the reference's transformers fork) with the
 reference's adapter wiring (mlp := Sequential(mlp, Adapter), magma/magma.py:143-148), HF CLIP ViT-L/14 as the image
 encoder, Linear+Dropout+LayerNorm prefix, bf16, LM and encoder frozen, batch 8, 224x224, seq_len 128, fwd+bwd+AdamW.

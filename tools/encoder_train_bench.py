@@ -4,7 +4,7 @@ frozen-encoder step of bench.py: BASELINE config 2 sizes (ViT-L/14 + GPT-J-6B + 
   python tools/encoder_train_bench.py [--steps 10]
 
 Prints one JSON line per variant: ms/step, samples/s, trainable parameters, and the ViT's share of algorithmic FLOPs
-(forward 0.162 TFLOP/image, backward 2x: SURVEY.md §8d)."""
+(forward 0.162 TFLOP/image, backward 2x)."""
 import argparse
 import json
 import os

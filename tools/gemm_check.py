@@ -1,6 +1,6 @@
-"""GPU diagnostic sweep for the tcgen05 GEMM core (development tool; the judged parity tests live in tests/).
+"""GPU diagnostic sweep for the wgmma GEMM core (development tool; the judged parity tests live in tests/).
 
-Usage on a B200 box:  python tools/gemm_check.py            # runs every group in its own subprocess
+Usage on an H100:  python tools/gemm_check.py            # runs every group in its own subprocess
                       python tools/gemm_check.py --group majors
 Each case prints max-abs / relative-Frobenius error against an fp32 torch matmul of the same bf16 inputs.
 """
@@ -186,26 +186,26 @@ def run_group(g):
         torch.cuda.synchronize()
         ok &= report("batched ViT PV T=257 (ragged K)", o2.permute(0, 2, 1, 3), pbuf[..., :T].float() @ v2.float())
     elif g == "pair":
-        # the CTA-pair (cta_group::2) kernel, forced with force_bn=512
+        # the 256-wide tile (force_bn=256) across every epilogue form
         import torch.nn.functional as F
 
         for a_mn in (False, True):
             for b_mn in (False, True):
                 M, N, K = 512, 768, 320
                 A, B = mk((M, K), a_mn, dev), mk((N, K), b_mn, dev)
-                C = ops.gemm(A, B, a_mn=a_mn, b_mn=b_mn, force_bn=512)
+                C = ops.gemm(A, B, a_mn=a_mn, b_mn=b_mn, force_bn=256)
                 torch.cuda.synchronize()
                 ok &= report(f"pair majors a_mn={int(a_mn)} b_mn={int(b_mn)}", C, ref_gemm(A, B, a_mn, b_mn))
                 M, N, K = (304 if a_mn else 300), (1000 if b_mn else 1002), 328  # MN-major operands need ld % 8 == 0
                 A, B = mk((M, K), a_mn, dev), mk((N, K), b_mn, dev)
                 buf = torch.full((M, 1008), 7.0, device=dev, dtype=torch.bfloat16)
-                ops.gemm(A, B, out=buf[:, :N], a_mn=a_mn, b_mn=b_mn, force_bn=512)
+                ops.gemm(A, B, out=buf[:, :N], a_mn=a_mn, b_mn=b_mn, force_bn=256)
                 torch.cuda.synchronize()
                 ok &= report(f"pair tails a_mn={int(a_mn)} b_mn={int(b_mn)} M={M} N={N} K=328", buf[:, :N], ref_gemm(A, B, a_mn, b_mn))
                 ok &= untouched(f"pair tails a_mn={int(a_mn)} b_mn={int(b_mn)} columns >= N", buf[:, N:], 7.0)
         M, N, K = 1024, 4096, 4096
         A, B = mk((M, K), False, dev), mk((N, K), False, dev)
-        C = ops.gemm(A, B, force_bn=512)
+        C = ops.gemm(A, B, force_bn=256)
         torch.cuda.synchronize()
         ok &= report("pair 1024x4096x4096", C, ref_gemm(A, B, False, False))
         M, N, K = 512, 1024, 256
@@ -214,41 +214,41 @@ def run_group(g):
         base = ref_gemm(A, B, False, False)
         pre = base + bias.float()
         aux = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, aux_out=aux, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, aux_out=aux, force_bn=256)
         ok &= report("pair bias+gelu_new+aux", C, F.gelu(pre, approximate="tanh"))
         ok &= report("pair aux_out", aux, pre)
         r1, r2 = mk((M, N), False, dev), mk((M, N), False, dev)
-        C = ops.gemm(A, B, bias=bias, res1=r1, res2=r2, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, res1=r1, res2=r2, force_bn=256)
         ok &= report("pair bias+res1+res2", C, pre + r1.float() + r2.float())
         x = mk((M, N), False, dev)
-        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_RELU, force_bn=512)
+        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_RELU, force_bn=256)
         ok &= report("pair dact relu", C, base * (x.float() > 0).float())
         Cf = torch.ones(M, N, device=dev, dtype=torch.float32)
-        ops.gemm(A, B, out=Cf, accumulate=True, force_bn=512)
+        ops.gemm(A, B, out=Cf, accumulate=True, force_bn=256)
         ok &= report("pair f32 accumulate", Cf, base + 1.0, tol=5e-3)
         # batched (2 x 3 batches of 256 x 512 x 192)
         Ab = mk((2, 3, 256, 192), False, dev)
         Bb = mk((2, 3, 512, 192), False, dev)
-        Cb = ops.gemm(Ab, Bb, force_bn=512)
+        Cb = ops.gemm(Ab, Bb, force_bn=256)
         torch.cuda.synchronize()
         ok &= report("pair batched", Cb, Ab.float() @ Bb.float().transpose(-1, -2))
         # every specialised epilogue of the row-per-thread / TMA-store path (epilogue v3)
-        C = ops.gemm(A, B, bias=bias, act=ops.ACT_RELU, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, act=ops.ACT_RELU, force_bn=256)
         ok &= report("pair bias+relu", C, F.relu(pre))
-        C = ops.gemm(A, B, bias=bias, act=ops.ACT_QUICK_GELU, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, act=ops.ACT_QUICK_GELU, force_bn=256)
         ok &= report("pair bias+quick_gelu", C, pre * torch.sigmoid(1.702 * pre))
-        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, force_bn=256)
         ok &= report("pair bias+gelu_new (no aux)", C, F.gelu(pre, approximate="tanh"))
         xf = x.float().requires_grad_(True)
         F.gelu(xf, approximate="tanh").sum().backward()
-        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_GELU_NEW, force_bn=512)
+        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_GELU_NEW, force_bn=256)
         ok &= report("pair dact gelu_new", C, base * xf.grad)
-        C = ops.gemm(A, B, bias=bias, res1=r1, alpha=0.5, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, res1=r1, alpha=0.5, force_bn=256)
         ok &= report("pair alpha+bias+res1", C, 0.5 * base + bias.float() + r1.float())
-        C = ops.gemm(A, B, bias=bias, res1=r1, act=ops.ACT_RELU_POST, force_bn=512)
+        C = ops.gemm(A, B, bias=bias, res1=r1, act=ops.ACT_RELU_POST, force_bn=256)
         ok &= report("pair bias+res1+relu_post", C, F.relu(pre + r1.float()))
         Cf = torch.full((M, N), 3.0, device=dev, dtype=torch.float32)
-        ops.gemm(A, B, out=Cf, force_bn=512)
+        ops.gemm(A, B, out=Cf, force_bn=256)
         ok &= report("pair f32 plain (overwrites)", Cf, base, tol=5e-3)
         # ragged N (not a multiple of 8, like the 50258-wide LM head) and ragged M, with bias / residual / aux / f32
         Mr, Nr, Kr = 520, 1002, 320
@@ -258,18 +258,18 @@ def run_group(g):
         rr_[:, :Nr] = mk((Mr, Nr), False, dev)
         baser = ref_gemm(Ar, Br, False, False) + br.float()
         buf = torch.full((Mr, 1008), 7.0, device=dev, dtype=torch.bfloat16)
-        ops.gemm(Ar, Br, out=buf[:, :Nr], bias=br, res1=rr_[:, :Nr], force_bn=512)
+        ops.gemm(Ar, Br, out=buf[:, :Nr], bias=br, res1=rr_[:, :Nr], force_bn=256)
         ok &= report("pair ragged M=520 N=1002 bias+res1", buf[:, :Nr], baser + rr_[:, :Nr].float())
         ok &= untouched("pair ragged bias+res1 columns >= N", buf[:, Nr:], 7.0)
         auxr = torch.full((Mr, 1008), 5.0, device=dev, dtype=torch.bfloat16)
         buf.fill_(7.0)
-        ops.gemm(Ar, Br, out=buf[:, :Nr], bias=br, act=ops.ACT_GELU_NEW, aux_out=auxr[:, :Nr], force_bn=512)
+        ops.gemm(Ar, Br, out=buf[:, :Nr], bias=br, act=ops.ACT_GELU_NEW, aux_out=auxr[:, :Nr], force_bn=256)
         ok &= report("pair ragged gelu+aux: C", buf[:, :Nr], F.gelu(baser, approximate="tanh"))
         ok &= report("pair ragged gelu+aux: aux", auxr[:, :Nr], baser)
         ok &= untouched("pair ragged gelu+aux C columns >= N", buf[:, Nr:], 7.0)
         ok &= untouched("pair ragged gelu+aux aux columns >= N", auxr[:, Nr:], 5.0)
         buff = torch.full((Mr, 1004), 2.0, device=dev, dtype=torch.float32)
-        ops.gemm(Ar, Br, out=buff[:, :Nr], accumulate=True, force_bn=512)
+        ops.gemm(Ar, Br, out=buff[:, :Nr], accumulate=True, force_bn=256)
         ok &= report("pair ragged f32 accumulate", buff[:, :Nr], baser - br.float() + 2.0, tol=5e-3)
         ok &= untouched("pair ragged f32 accumulate columns >= N", buff[:, Nr:], 2.0)
         # fused rotary epilogue (forward and inverse) on the pair kernel == rotation of the plain fp32 product
@@ -279,7 +279,7 @@ def run_group(g):
         tab = ops.rope_table(Sx, rot, pos0=7, device=dev)
         for mode in (1, -1):
             fused = ops.gemm(A2, B2, rope_tab=tab, rope_mode=mode, rope_S=Sx, rope_hd=hd, rope_rot=rot,
-                             rope_ncols=2 * H * hd, force_bn=512)
+                             rope_ncols=2 * H * hd, force_bn=256)
             plain = ops.gemm(A2, B2, out_dtype=torch.float32)
             qq = plain.view(Mx // Sx, Sx, 3, H, hd).clone()
             cs = tab[None, :, None, None, :, 0]
@@ -293,13 +293,13 @@ def run_group(g):
         pb = torch.softmax(torch.randn(Bsz, H_, S_, S_, device=dev), -1).to(torch.bfloat16)
         vb = (torch.randn(Bsz, S_, H_, hd_, device=dev) * 0.3).to(torch.bfloat16)
         ob = torch.empty(Bsz, S_, H_, hd_, device=dev, dtype=torch.bfloat16)
-        ops.gemm(pb, vb.permute(0, 2, 1, 3), out=ob.permute(0, 2, 1, 3), b_mn=True, force_bn=512)
+        ops.gemm(pb, vb.permute(0, 2, 1, 3), out=ob.permute(0, 2, 1, 3), b_mn=True, force_bn=256)
         ok &= report("pair batched PV into [B,S,H,hd]", ob.permute(0, 2, 1, 3), pb.float() @ vb.permute(0, 2, 1, 3).float())
         # perf vs 1-CTA
         for (M, N, K, bmn) in ((1024, 4096, 4096, False), (1024, 16384, 4096, False), (1024, 4096, 16384, True), (8192, 8192, 8192, False)):
             A, B = mk((M, K), False, dev), mk((N, K), bmn, dev)
             C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-            for bn in (256, 512):
+            for bn in (128, 256):
                 for _ in range(3):
                     ops.gemm(A, B, out=C, b_mn=bmn, force_bn=bn)
                 torch.cuda.synchronize()
@@ -326,13 +326,13 @@ def run_group(g):
             A, B = mk((M, K), False, dev, 0.5), mk((N, K), bmn, dev, 0.05)
             ldc = (N + 7) // 8 * 8
             C = torch.full((M, ldc), 7.0, device=dev, dtype=torch.bfloat16)
-            ops.gemm(A, B, out=C[:, :N], b_mn=bmn, splitk_ws=ws, force_bn=768)
+            ops.gemm(A, B, out=C[:, :N], b_mn=bmn, splitk_ws=ws, force_bn=256)
             want = ref_gemm(A, B, False, bmn)
             ok &= report(f"streamk plain M={M} N={N} K={K} ({what})", C[:, :N], want)
             if ldc > N:
                 ok &= untouched(f"streamk M={M} N={N} columns >= N", C[:, N:], 7.0)
             C2 = torch.full((M, ldc), 7.0, device=dev, dtype=torch.bfloat16)
-            ops.gemm(A, B, out=C2[:, :N], b_mn=bmn, splitk_ws=ws, force_bn=768)
+            ops.gemm(A, B, out=C2[:, :N], b_mn=bmn, splitk_ws=ws, force_bn=256)
             same = bool(torch.equal(C, C2))
             print(f"[{'OK' if same else 'FAIL'}] streamk M={M} N={N} K={K}: second run bit-identical", flush=True)
             ok &= same
@@ -342,23 +342,23 @@ def run_group(g):
         base = ref_gemm(A, B, False, False)
         pre = base + bias.float()
         r1, r2 = mk((M, N), False, dev), mk((M, N), False, dev)
-        C = ops.gemm(A, B, bias=bias, res1=r1, res2=r2, alpha=0.5, splitk_ws=ws, force_bn=768)
+        C = ops.gemm(A, B, bias=bias, res1=r1, res2=r2, alpha=0.5, splitk_ws=ws, force_bn=256)
         ok &= report("streamk alpha+bias+res1+res2", C, 0.5 * base + bias.float() + r1.float() + r2.float())
         aux = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, aux_out=aux, splitk_ws=ws, force_bn=768)
+        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, aux_out=aux, splitk_ws=ws, force_bn=256)
         ok &= report("streamk bias+gelu_new+aux: C", C, F.gelu(pre, approximate="tanh"))
         ok &= report("streamk bias+gelu_new+aux: aux", aux, pre)
         x = mk((M, N), False, dev)
-        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_RELU, splitk_ws=ws, force_bn=768)
+        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_RELU, splitk_ws=ws, force_bn=256)
         ok &= report("streamk dact relu", C, base * (x.float() > 0).float())
         Cf = torch.ones(M, N, device=dev, dtype=torch.float32)
-        ops.gemm(A, B, out=Cf, accumulate=True, splitk_ws=ws, force_bn=768)
+        ops.gemm(A, B, out=Cf, accumulate=True, splitk_ws=ws, force_bn=256)
         ok &= report("streamk f32 accumulate", Cf, base + 1.0, tol=5e-3)
         Sx, H, hd, rot = 128, 16, 256, 64
         A2, B2 = mk((8 * Sx, 4096), False, dev, 0.5), mk((3 * H * hd, 4096), False, dev, 0.05)
         tab = ops.rope_table(Sx, rot, pos0=0, device=dev)
         fused = ops.gemm(A2, B2, rope_tab=tab, rope_mode=1, rope_S=Sx, rope_hd=hd, rope_rot=rot, rope_ncols=2 * H * hd,
-                         splitk_ws=ws, force_bn=768)
+                         splitk_ws=ws, force_bn=256)
         plain = ops.gemm(A2, B2, out_dtype=torch.float32)
         qq = plain.view(8, Sx, 3, H, hd).clone()
         cs, sn = tab[None, :, None, None, :, 0], tab[None, :, None, None, :, 1]
@@ -371,7 +371,7 @@ def run_group(g):
             A, B = mk((M, K), False, dev), mk((N, K), bmn, dev)
             C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
             for tag, w in (("stream-K", ws), ("whole tiles", None)):
-                fb = 768 if w is not None else 0
+                fb = 256 if w is not None else 0
                 for _ in range(3):
                     ops.gemm(A, B, out=C, b_mn=bmn, splitk_ws=w, force_bn=fb)
                 torch.cuda.synchronize()

@@ -33,7 +33,7 @@ def small_cfg(**kw):
 
 
 def build_lm(cfg, w, dev):
-    """B200 GPT-J with the oracle's weights (names are shared with the reference state dict)."""
+    """This package's GPT-J with the oracle's weights (names are shared with the reference state dict)."""
     import torch
     import torch.nn as nn
     from magma_b200.adapters import Adapter, AdapterWrapper, ParallelAdapter, ParallelAdapterWrapper
@@ -305,7 +305,7 @@ def im2col3x3_reference(x_nhwc, stride):
 
 
 def group_resnet(dev):
-    """Conv-trunk row (SURVEY.md §8f rank 1): layout kernels bit-exact vs torch, RELU_POST epilogue, a small CLIP
+    """Conv-trunk row: layout kernels bit-exact vs torch, RELU_POST epilogue, a small CLIP
     ModifiedResNet against the oracle restatement, and Magma.forward/backward through the 3-D feature path."""
     import torch
     import torch.nn.functional as F

@@ -1,7 +1,7 @@
 """Driver for an ncu source-level capture of the CTA-pair GEMM on an epilogue-bound shape
 (M = N = 8192, K = 64: 13.8 tiles per cluster, one k-block each) and on a single-wave shape with a residual epilogue.
 
-  ncu --set full --import-source on --clock-control none -k regex:gemm2_tcgen05 -s 4 -c 2 -o gpurun_out/epi \
+  ncu --set full --import-source on --clock-control none -k regex:gemm_wgmma -s 4 -c 2 -o epi \
       python tools/ncu_epi.py"""
 import os
 import sys

@@ -1,8 +1,8 @@
 """One line per profiled launch from an `ncu --set full` report: time, DRAM bytes, tensor-pipe activity, L2 -> SM traffic,
 L2 hit rate, grid, registers, local-memory (spill) instructions, SM clock.
 
-  ncu -i gpurun_out/x.ncu-rep --page raw --csv > /tmp/raw.csv
-  python tools/ncu_summary.py /tmp/raw.csv [--labels qkv_fwd,out_fwd,...] [--out profiles/rNN_gemm_ncu_full_summary.txt]"""
+  ncu -i x.ncu-rep --page raw --csv > /tmp/raw.csv
+  python tools/ncu_summary.py /tmp/raw.csv [--labels qkv_fwd,out_fwd,...] [--out gemm_ncu_summary.txt]"""
 import argparse
 import csv
 

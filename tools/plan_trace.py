@@ -5,12 +5,12 @@ The host schedules (csrc/gptj_sched.cu, vit_sched.cu) are compiled as plain C++ 
 bytes) and returns without touching memory, so the schedule can be "issued" at BASELINE.json's sizes — GPT-J-6B, B = 8,
 S = 128 — with placeholder pointers in milliseconds. The result is the exact list of launches a step makes, which this
 tool summarises against the measured peaks (MEASURED_PEAKS.json): per-launch FLOPs / bytes, the roofline time of each
-launch, tile counts of the GEMMs and how full their last wave is on 148 SMs / 74 CTA pairs.
+launch, tile counts of the GEMMs and how full their last wave is on the 132 SMs of an H100 SXM.
 
-  python tools/plan_trace.py [--B 8] [--S 128] [--out profiles/r01_step_launch_plan.txt]
+  python tools/plan_trace.py [--B 8] [--S 128] [--out step_launch_plan.txt]
 
-This is an ANALYTIC plan (a lower bound per launch), not a measurement: compare it with the ncu launch list of the same
-step (profiles/r01_launches_step_summary_v5.txt)."""
+This is an ANALYTIC plan (a lower bound per launch), not a measurement: compare it with a measured launch list of the
+same step."""
 import argparse
 import collections
 import ctypes
@@ -122,15 +122,12 @@ def decode_step_plan(B, pos, S_max=264):
 
 
 def gemm_tiles(a):
-    """Tile counts of one GEMM launch under the dispatch rules of csrc/gemm.cu (CTA-pair 256x256 tiles when M > 128,
-    N >= 256, K >= 512; else 128 x BN tiles with BN = 256 unless N is small)."""
-    M, N, K, nb = int(a["M"]), int(a["N"]), int(a["K"]), int(a["nb"])
-    if M > 128 and N >= 256 and K >= 512:
-        t = math.ceil(M / 256) * math.ceil(N / 256) * nb
-        return "pair256x256", t, 74
+    """Tile counts of one GEMM launch of csrc/gemm.cu, approximated as 128 x BN tiles with BN = 256 unless N is small
+    (the kernel's own choice also weighs wave quantisation), on a persistent grid of one CTA per SM."""
+    M, N, nb = int(a["M"]), int(a["N"]), int(a["nb"])
     bn = 256 if N >= 256 else (128 if N > 64 else 64)
     t = math.ceil(M / 128) * math.ceil(N / bn) * nb
-    return f"128x{bn}", t, 148
+    return f"128x{bn}", t, 132
 
 
 def summarise(rows, B, S, peaks, out):
@@ -185,7 +182,7 @@ def main():
     ap.add_argument("--pos", type=int, default=136)
     a = ap.parse_args()
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peaks = json.load(open(p)) if os.path.exists(p) else {"bf16_tflops": 1684.7, "hbm_gbs": 6575.1}
+    peaks = json.load(open(p)) if os.path.exists(p) else {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}  # H100 SXM data sheet
     if a.decode:
         B = a.B if a.B != 8 else 32
         summarise(decode_step_plan(B, a.pos), B, 0, peaks, a.out)

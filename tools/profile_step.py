@@ -1,9 +1,9 @@
-"""Profiling driver for ncu (run under gpurun; see /opt/skills/guides/B200_PROFILING.md):
+"""Profiling driver for ncu :
 
   ncu --profile-from-start off --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum \
-      --clock-control none --csv --log-file gpurun_out/launches_step.csv python tools/profile_step.py
-  ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:gemm_tcgen05 \
-      -o gpurun_out/prof_gemm python tools/profile_step.py --gemm-only
+      --clock-control none --csv --log-file launches_step.csv python tools/profile_step.py
+  ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:gemm_wgmma \
+      -o prof_gemm python tools/profile_step.py --gemm-only
 
 Default mode: build the BASELINE config-2 model, warm up, then run exactly ONE train step inside a
 cudaProfilerStart/Stop range. --gemm-only: the main GEMM shapes of one GPT-J block, standalone, inside the range."""

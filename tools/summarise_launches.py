@@ -2,8 +2,8 @@
 --csv ...`) into a per-kernel table, and (with --traffic-json) the per-launch DRAM traffic of the GEMM core that
 bench.py reports as `roofline.traffic`.
 
-  python tools/summarise_launches.py gpurun_out/launches.csv --out profiles/rNN_launches_summary.txt \
-         --traffic-json profiles/gemm_dram_traffic.json"""
+  python tools/summarise_launches.py launches.csv --out launches_summary.txt \
+         --traffic-json gemm_dram_traffic.json"""
 import argparse
 import collections
 import csv
@@ -56,12 +56,12 @@ def main():
     if a.out:
         open(a.out, "w").write(text)
     if a.traffic_json:
-        g = [v for v in L if "gemm" in v["name"] and "tcgen05" in v["name"]]
+        g = [v for v in L if "gemm" in v["name"] and "wgmma" in v["name"]]
         if g:
             b = sum(v.get("dram__bytes_read.sum", 0.0) + v.get("dram__bytes_write.sum", 0.0) for v in g)
             json.dump({"bytes_per_launch": b / len(g), "gemm_launches": len(g), "total_dram_bytes": b,
                        "source": a.csv, "note": a.note or "dram__bytes_read.sum + dram__bytes_write.sum over every "
-                       "gemm*_tcgen05_kernel launch of one profiled train step / number of those launches"},
+                       "gemm_wgmma_kernel launch of one profiled train step / number of those launches"},
                       open(a.traffic_json, "w"), indent=1)
 
 
