@@ -128,6 +128,12 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, in
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ---- per-warpgroup register reallocation (all threads of a warpgroup execute the same one) ----
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- misc math ----
 // gelu_new(x) = 0.5 x (1 + tanh(u)), u = sqrt(2/pi) (x + 0.044715 x^3). With 0.5 (1 + tanh(u)) = sigmoid(2u) this is
 // x / (1 + exp(-2u)): one ex2 + one rcp on the SFU instead of tanhf's ~25-instruction branchy expansion, which was a

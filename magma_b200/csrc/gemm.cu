@@ -6,9 +6,10 @@
 // magma/adapters.py:19-23, magma/image_prefix.py:72):
 //   * persistent grid (<= one CTA per SM), static round-robin tile scheduler, m-fastest tile order so
 //     CTAs that run concurrently share the same weight (B) tile through L2;
-//   * warp-specialised: warpgroup 0 = TMA producer (one lane), warpgroups 1 and 2 = consumers, each owning 64 rows of
-//     the 128-row tile: wgmma.mma_async m64nBNk16 with fp32 accumulators in registers, then the fused epilogue
-//     straight from the accumulator fragment (gemm_common.cuh);
+//   * warp-specialised: warpgroup 0 = TMA producer (one lane, registers handed to the consumers with setmaxnreg),
+//     warpgroups 1 and 2 = consumers, each owning 64 rows of the 128-row tile: wgmma.mma_async m64nBNk16 with fp32
+//     accumulators in registers, then the fused epilogue, staged through shared memory 64 columns at a time so that
+//     one rolled copy of its code reads and writes global memory in contiguous row segments (gemm_common.cuh);
 //   * operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a multi-stage smem ring,
 //     completion tracked with mbarriers; a consumer releases a slot once the wgmma reading it has retired;
 //   * both operand majors (K-major and MN-major) are supported through the wgmma shared-memory descriptors and the
@@ -32,7 +33,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * C_::kABytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * C_::kStageBytes);
+  float* epi_stage = reinterpret_cast<float*>(smem + kStages * C_::kStageBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * C_::kStageBytes + kEpiBytes);
   uint64_t* empty_bar = full_bar + kStages;
 
   const int wg = threadIdx.x >> 7;
@@ -52,8 +54,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   __syncthreads();
   pdl_wait();  // everything above overlapped the previous kernel; global memory is touched only from here on
 
+  // Register split: 128 x 40 (producer) + 256 x 232 (consumers) <= 65536; the launch bound alone caps every thread
+  // at 168, which the BN = 256 accumulators (128 registers) leave little room above.
   if (wg == 0) {
     // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -95,6 +100,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
   } else {
     // ===================== consumers: wgmma + epilogue =====================
+    setmaxnreg_inc<232>();
     const int cw = wg - 1;  // rows [64 cw, 64 cw + 64) of the tile
     const bool leader = (threadIdx.x & 127) == 0;
     // K-major SW128: 8-row atoms of 128 B rows -> SBO = 1024, LBO unused; advance K by 16 elems = 32 B; this
@@ -141,7 +147,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>();
       if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
       const long long boff = (long long)z0 * p.c_bs0 + (long long)z1 * p.c_bs1;
-      epi_fragment<BN>(p, acc, boff, m_blk * BM + cw * 64, n_blk * BN, ks);
+      epi_tile<BN>(p, acc, epi_stage + cw * 64 * kEpiCols, 1 + cw, boff, m_blk * BM + cw * 64, n_blk * BN, ks);
     }
   }
 }
@@ -149,7 +155,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // ---------------------------------------------------------------------------------------------
 // split-K finalize: C = epilogue(sum over splits of ws[split]). One thread per float4 of the output.
 // ---------------------------------------------------------------------------------------------
-template <typename OutT>
 __global__ void splitk_finalize_kernel(const GemmKernelParams p) {
   pdl_trigger();
   pdl_wait();
@@ -158,7 +163,6 @@ __global__ void splitk_finalize_kernel(const GemmKernelParams p) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int row = (int)(i / ncol4);
     const int col = (int)(i - (long long)row * ncol4) * 4;
-    const int nvalid = min(4, p.N - col);
     float v[4] = {0.f, 0.f, 0.f, 0.f};
     for (int ks = 0; ks < p.split_k; ++ks) {  // fixed summation order -> bitwise reproducible
       const float4 w4 = *reinterpret_cast<const float4*>(p.splitk_ws + ((long long)ks * p.M + row) * p.ld_ws + col);
@@ -167,46 +171,7 @@ __global__ void splitk_finalize_kernel(const GemmKernelParams p) {
       v[2] += w4.z;
       v[3] += w4.w;
     }
-    if (p.bias) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e)
-        if (e < nvalid) v[e] += __bfloat162float(p.bias[col + e]);
-    }
-    if (p.rope_mode != 0 && col < p.rope_ncols && (col % p.rope_hd) < p.rope_rot) {
-      const int rp = (col % p.rope_hd) >> 1;
-      const float2* tp = p.rope_tab + (long long)(row % p.rope_S) * (p.rope_rot >> 1) + rp;
-      const float2 cs0 = __ldg(tp), cs1 = __ldg(tp + 1);
-      const float sg = p.rope_mode > 0 ? 1.f : -1.f;
-      const float a0 = v[0], a1 = v[1], a2 = v[2], a3 = v[3];
-      v[0] = a0 * cs0.x - a1 * cs0.y * sg;
-      v[1] = a1 * cs0.x + a0 * cs0.y * sg;
-      v[2] = a2 * cs1.x - a3 * cs1.y * sg;
-      v[3] = a3 * cs1.x + a2 * cs1.y * sg;
-    }
-    const long long coff = (long long)row * p.ldc + col;
-    const long long roff = (long long)row * p.ld_res + col;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      if (e >= nvalid) continue;
-      float x = v[e];
-      if (p.aux_out) p.aux_out[coff + e] = __float2bfloat16(x);
-      if (p.act == MB200_ACT_GELU_NEW) x = gelu_new_f(x);
-      else if (p.act == MB200_ACT_QUICK_GELU) x = quick_gelu_f(x);
-      else if (p.act == MB200_ACT_RELU) x = fmaxf(x, 0.f);
-      if (p.dact) {
-        const float a = __bfloat162float(p.aux_in[coff + e]);
-        x = p.dact == MB200_DACT_GELU_NEW ? x * gelu_new_grad_f(a) : (a > 0.f ? x : 0.f);
-      }
-      if (p.res1) x += __bfloat162float(p.res1[roff + e]);
-      if (p.res2) x += __bfloat162float(p.res2[roff + e]);
-      if (p.act == MB200_ACT_RELU_POST) x = fmaxf(x, 0.f);
-      if constexpr (sizeof(OutT) == 4) {
-        float* dst = reinterpret_cast<float*>(p.C) + coff + e;
-        *dst = p.accumulate ? *dst + x : x;
-      } else {
-        reinterpret_cast<bf16*>(p.C)[coff + e] = __float2bfloat16(x);
-      }
-    }
+    epi_store4(p, 0, row, col, v);
   }
 }
 
@@ -451,7 +416,6 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
                MB200_E_ARG, "gemm: bad rope epilogue parameters");
 
   const bool amn = a->A.mn_major != 0, bmn = a->B.mn_major != 0;
-  const bool f32 = a->c_dtype == MB200_F32;
   kp.split_k = 1;
   kp.kb_per_split = (a->K + BK - 1) / BK;
   // Split-K for small M (see plan_small_m; for 32 < M <= 128 only the long-K / narrow-N shape, GPT-J fc_out, is split).
@@ -495,8 +459,7 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
       const long long n4 = (long long)a->M * ((a->N + 3) / 4);
       const int fgrid = (int)((n4 + 255) / 256 > 2048 ? 2048 : (n4 + 255) / 256);
       kp.alpha = 1.f;  // already applied to the partials
-      if (f32) MB_CUDA(launch_pdl(splitk_finalize_kernel<float>, dim3(fgrid), dim3(256), 0, stream, kp));
-      else MB_CUDA(launch_pdl(splitk_finalize_kernel<bf16>, dim3(fgrid), dim3(256), 0, stream, kp));
+      MB_CUDA(launch_pdl(splitk_finalize_kernel, dim3(fgrid), dim3(256), 0, stream, kp));
       count_launch();
       return 0;
     }

@@ -9,7 +9,9 @@ static constexpr int BM = 128;        // tile M: two consumer warpgroups x wgmma
 static constexpr int BK = 64;         // 64 bf16 = 128 bytes = one SWIZZLE_128B row
 static constexpr int WG_K = 16;       // wgmma K for 16-bit inputs
 static constexpr int kThreads = 384;  // warpgroup 0 = TMA producer, warpgroups 1, 2 = MMA + epilogue
-static constexpr int kSmemBudget = 200 * 1024;  // operand ring; + alignment slack and barriers < 227 KB
+static constexpr int kEpiCols = 64;  // epilogue staging chunk: BM x 64 fp32, 64 rows per consumer warpgroup
+static constexpr int kEpiBytes = BM * kEpiCols * 4;
+static constexpr int kSmemBudget = 192 * 1024;  // operand ring; + staging, alignment slack and barriers <= 227 KB
 
 template <int BN>
 struct Cfg {
@@ -18,7 +20,8 @@ struct Cfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
 };
 
 struct GemmKernelParams {
@@ -49,11 +52,6 @@ struct GemmKernelParams {
   long long ld_ws;
 };
 
-__device__ __forceinline__ uint32_t ldg32(const bf16* ptr) {
-  uint32_t u;
-  asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(u) : "l"(ptr));
-  return u;
-}
 __device__ __forceinline__ float2 bf16x2_to_f32(uint32_t u) {
   return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
 }
@@ -62,122 +60,172 @@ __device__ __forceinline__ uint32_t f32x2_to_bf16(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// n (<= 4) consecutive bf16 -> fp32 (missing elements read as 0): one 8-byte read-only load when all four are in range
+// and 8-byte aligned (operand pointers other than C carry no alignment guarantee beyond the element).
+__device__ __forceinline__ void ld_bf16x4(const bf16* src, int n, float (&v)[4]) {
+  if (n == 4 && (reinterpret_cast<uintptr_t>(src) & 7) == 0) {
+    uint32_t u0, u1;
+    asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(u0), "=r"(u1) : "l"(src));
+    const float2 a = bf16x2_to_f32(u0), b = bf16x2_to_f32(u1);
+    v[0] = a.x;
+    v[1] = a.y;
+    v[2] = b.x;
+    v[3] = b.y;
+  } else {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] = e < n ? __bfloat162float(src[e]) : 0.f;
+  }
+}
+__device__ __forceinline__ void st_bf16x4(bf16* dst, int n, const float (&v)[4]) {
+  if (n == 4 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+    *reinterpret_cast<uint2*>(dst) = make_uint2(f32x2_to_bf16(v[0], v[1]), f32x2_to_bf16(v[2], v[3]));
+  } else {
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (e < n) dst[e] = __float2bfloat16(v[e]);
+  }
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 enum { EK_GENERIC = 0, EK_SPLITK };
 
 // ---------------------------------------------------------------------------------------------
-// Epilogue on the accumulator fragment of one consumer warpgroup (64 rows x BN columns, wgmma.cuh layout): every thread
-// owns column pairs (c, c + 1), c even, of two rows. A pair is also a rotary pair (rotate_every_two), so alpha / bias /
-// rotary / saved pre-activation / activation / activation-derivative / residuals / store are all applied in registers
-// on 8-byte (fp32) or 4-byte (bf16) chunks without any exchange between threads. All branches on p are warp-uniform.
-// Split-K work items store the fp32 partial tile into their slice of the workspace instead (EK_SPLITK).
+// Fused epilogue of columns [col, col + 4) of one output row (col % 4 == 0, col < N, row < M); v holds alpha x the
+// accumulators (or the summed split-K partials). Applied in this order: bias, rotary, saved pre-activation (aux_out),
+// activation, activation derivative (aux_in), residuals, ReLU-post, store (bf16, fp32 or fp32 accumulate). rope_hd,
+// rope_rot and rope_ncols are multiples of 4, so both rotary pairs (col, col + 1), (col + 2, col + 3) of the group are
+// rotated or neither is. Every branch on p is uniform across the kernel.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void epi_pair(const GemmKernelParams& p, long long boff, int row, int col, float v0, float v1,
-                                         int ks) {
-  if (row >= p.M || col >= p.N) return;
-  const bool two = col + 1 < p.N;
-  v0 *= p.alpha;
-  v1 *= p.alpha;
-  if (p.epi_kind == EK_SPLITK) {
-    float* w = p.splitk_ws + ((long long)ks * p.M + row) * p.ld_ws + col;  // ld_ws % 4 == 0: the padded column exists
-    *reinterpret_cast<float2*>(w) = make_float2(v0, v1);
-    return;
-  }
+__device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long boff, int row, int col, float (&v)[4]) {
+  const int n = min(4, p.N - col);
   if (p.bias) {
-    v0 += __bfloat162float(p.bias[col]);
-    if (two) v1 += __bfloat162float(p.bias[col + 1]);
+    float b[4];
+    ld_bf16x4(p.bias + col, n, b);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] += b[e];
   }
   if (p.rope_mode != 0 && col < p.rope_ncols) {
     const int dim = col % p.rope_hd;
     if (dim < p.rope_rot) {
-      const float2 cs = __ldg(p.rope_tab + (long long)(row % p.rope_S) * (p.rope_rot >> 1) + (dim >> 1));
+      const float2* tp = p.rope_tab + (long long)(row % p.rope_S) * (p.rope_rot >> 1) + (dim >> 1);
+      const float2 cs0 = __ldg(tp), cs1 = __ldg(tp + 1);
       const float sg = p.rope_mode > 0 ? 1.f : -1.f;
-      const float a0 = v0, a1 = v1;
-      v0 = a0 * cs.x - a1 * cs.y * sg;
-      v1 = a1 * cs.x + a0 * cs.y * sg;
+      const float a0 = v[0], a1 = v[1], a2 = v[2], a3 = v[3];
+      v[0] = a0 * cs0.x - a1 * cs0.y * sg;
+      v[1] = a1 * cs0.x + a0 * cs0.y * sg;
+      v[2] = a2 * cs1.x - a3 * cs1.y * sg;
+      v[3] = a3 * cs1.x + a2 * cs1.y * sg;
     }
   }
   const long long coff = boff + (long long)row * p.ldc + col;
-  if (p.aux_out) {
-    if (two) *reinterpret_cast<uint32_t*>(p.aux_out + coff) = f32x2_to_bf16(v0, v1);
-    else p.aux_out[coff] = __float2bfloat16(v0);
-  }
-  if (p.act == MB200_ACT_GELU_NEW) {
-    v0 = gelu_new_f(v0);
-    v1 = gelu_new_f(v1);
-  } else if (p.act == MB200_ACT_QUICK_GELU) {
-    v0 = quick_gelu_f(v0);
-    v1 = quick_gelu_f(v1);
-  } else if (p.act == MB200_ACT_RELU) {
-    v0 = fmaxf(v0, 0.f);
-    v1 = fmaxf(v1, 0.f);
+  if (p.aux_out) st_bf16x4(p.aux_out + coff, n, v);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    if (p.act == MB200_ACT_GELU_NEW) v[e] = gelu_new_f(v[e]);
+    else if (p.act == MB200_ACT_QUICK_GELU) v[e] = quick_gelu_f(v[e]);
+    else if (p.act == MB200_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
   }
   if (p.dact) {
-    float2 a;
-    if (two) a = bf16x2_to_f32(ldg32(p.aux_in + coff));
-    else a = make_float2(__bfloat162float(p.aux_in[coff]), 0.f);
-    if (p.dact == MB200_DACT_GELU_NEW) {
-      v0 *= gelu_new_grad_f(a.x);
-      v1 *= gelu_new_grad_f(a.y);
-    } else {
-      v0 = a.x > 0.f ? v0 : 0.f;
-      v1 = a.y > 0.f ? v1 : 0.f;
-    }
+    float a[4];
+    ld_bf16x4(p.aux_in + coff, n, a);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] = p.dact == MB200_DACT_GELU_NEW ? v[e] * gelu_new_grad_f(a[e]) : (a[e] > 0.f ? v[e] : 0.f);
   }
   const long long roff = boff + (long long)row * p.ld_res + col;
   if (p.res1) {
-    if (two) {
-      const float2 r = bf16x2_to_f32(ldg32(p.res1 + roff));
-      v0 += r.x;
-      v1 += r.y;
-    } else {
-      v0 += __bfloat162float(p.res1[roff]);
-    }
+    float r[4];
+    ld_bf16x4(p.res1 + roff, n, r);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] += r[e];
   }
   if (p.res2) {
-    if (two) {
-      const float2 r = bf16x2_to_f32(ldg32(p.res2 + roff));
-      v0 += r.x;
-      v1 += r.y;
-    } else {
-      v0 += __bfloat162float(p.res2[roff]);
-    }
+    float r[4];
+    ld_bf16x4(p.res2 + roff, n, r);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] += r[e];
   }
   if (p.act == MB200_ACT_RELU_POST) {
-    v0 = fmaxf(v0, 0.f);
-    v1 = fmaxf(v1, 0.f);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] = fmaxf(v[e], 0.f);
   }
-  if (p.c_f32) {
+  if (p.c_f32) {  // C is 16-byte aligned and ldc, the batch strides and col are multiples of 4
     float* dst = reinterpret_cast<float*>(p.C) + coff;
-    if (two) {
-      float2 o = make_float2(v0, v1);
+    if (n == 4) {
+      float4 o = make_float4(v[0], v[1], v[2], v[3]);
       if (p.accumulate) {
-        const float2 old = *reinterpret_cast<const float2*>(dst);
+        const float4 old = *reinterpret_cast<const float4*>(dst);
         o.x += old.x;
         o.y += old.y;
+        o.z += old.z;
+        o.w += old.w;
       }
-      *reinterpret_cast<float2*>(dst) = o;
+      *reinterpret_cast<float4*>(dst) = o;
     } else {
-      dst[0] = p.accumulate ? dst[0] + v0 : v0;
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (e < n) dst[e] = p.accumulate ? dst[e] + v[e] : v[e];
     }
   } else {
-    bf16* dst = reinterpret_cast<bf16*>(p.C) + coff;
-    if (two) *reinterpret_cast<uint32_t*>(dst) = f32x2_to_bf16(v0, v1);
-    else dst[0] = __float2bfloat16(v0);
+    st_bf16x4(reinterpret_cast<bf16*>(p.C) + coff, n, v);
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Epilogue of one consumer warpgroup's 64 x BN accumulator fragment (wgmma.cuh layout), 64 columns at a time. The
+// fragment chunk is written to the warpgroup's 64 x 64 fp32 slice of the staging buffer; after a barrier over the
+// warpgroup, a rolled loop hands each thread groups of 4 consecutive columns of a row (16 threads per row), so a warp's
+// global loads and stores cover two contiguous 128-byte (bf16) or 256-byte (fp32) row segments, and one copy of the
+// feature code serves every chunk. Staging layout: row-major, 16-byte chunk q of row r stored at q ^ 2 (r & 3). A
+// half-warp's 8-byte fragment writes (4 rows x 2 chunks) and a quarter-warp's 16-byte reads (8 chunks of one row) then
+// fall on distinct banks.
+// Split-K work items store alpha x the fp32 tile into their slice of the workspace instead (EK_SPLITK).
 // row0: first row (within the batch) of this warpgroup's 64-row slab; col0: first column of the tile
+// ---------------------------------------------------------------------------------------------
 template <int BN>
-__device__ __forceinline__ void epi_fragment(const GemmKernelParams& p, const float (&acc)[BN / 2], long long boff,
-                                             int row0, int col0, int ks) {
+__device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float (&acc)[BN / 2], float* stage,
+                                         int bar_id, long long boff, int row0, int col0, int ks) {
   const int wt = threadIdx.x & 127;
-  const int r = row0 + (wt >> 5) * 16 + ((wt & 31) >> 2);
-  const int c = col0 + 2 * (wt & 3);
+  const int fr = (wt >> 5) * 16 + ((wt & 31) >> 2);  // fragment rows fr, fr + 8; column pair 2 (wt % 4) of each 8
+  const int fq = wt & 3;
+  const int pr = wt >> 4, pc = wt & 15;  // processing: rows pr + 8 i, 16-byte chunk pc
+  const int nch = min(BN / kEpiCols, (p.N - col0 + kEpiCols - 1) / kEpiCols);
+#pragma unroll 1
+  for (int ch = 0; ch < nch; ++ch) {
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    if (col0 + 8 * j >= p.N) break;  // warp-uniform
-    epi_pair(p, boff, r, c + 8 * j, acc[4 * j], acc[4 * j + 1], ks);
-    epi_pair(p, boff, r + 8, c + 8 * j, acc[4 * j + 2], acc[4 * j + 3], ks);
+    for (int c = 0; c < BN / kEpiCols; ++c) {
+      if (c != ch) continue;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int j = c * 8 + jj;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = fr + 8 * h;
+          const int q = (2 * jj + (fq >> 1)) ^ ((r & 3) << 1);
+          *reinterpret_cast<float2*>(stage + r * kEpiCols + q * 4 + 2 * (fq & 1)) =
+              make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+      }
+    }
+    named_bar_sync(bar_id, 128);
+    const int col = col0 + ch * kEpiCols + pc * 4;
+#pragma unroll 1
+    for (int i = 0; i < 64 / 8; ++i) {
+      const int r = pr + 8 * i;
+      const int row = row0 + r;
+      if (row >= p.M || col >= p.N) continue;
+      const float4 s = *reinterpret_cast<const float4*>(stage + r * kEpiCols + ((pc ^ ((r & 3) << 1)) * 4));
+      float v[4] = {s.x * p.alpha, s.y * p.alpha, s.z * p.alpha, s.w * p.alpha};
+      if (p.epi_kind == EK_SPLITK) {  // ld_ws % 4 == 0: the padded columns of the group exist
+        *reinterpret_cast<float4*>(p.splitk_ws + ((long long)ks * p.M + row) * p.ld_ws + col) =
+            make_float4(v[0], v[1], v[2], v[3]);
+        continue;
+      }
+      epi_store4(p, boff, row, col, v);
+    }
+    named_bar_sync(bar_id, 128);  // the slice is rewritten by the next chunk
   }
 }
 

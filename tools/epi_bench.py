@@ -49,7 +49,7 @@ def main():
         return (torch.randn(*shape, device=dev) * scale).to(torch.bfloat16)
 
     def case(tag, M, N, K, *, bias=False, act=0, res=0, aux=False, a_mn=False, b_mn=False, f32=False, force_bn=0,
-             dact=0, check=True, use_ws=True, rope=0):
+             dact=0, check=True, use_ws=True, rope=0, cublas=False):
         nbuf = max(1, min(8, int(200e6 // (N * K * 2)) + 1)) if N * K * 2 > 30e6 else 1
         Bs = [rnd(K, N) if b_mn else rnd(N, K) for _ in range(nbuf)]
         A = rnd(K, M, scale=1.0) if a_mn else rnd(M, K, scale=1.0)
@@ -76,6 +76,13 @@ def main():
             kw["splitk_ws"] = torch.empty(32 << 20, device=dev, dtype=torch.float32)
         us = timed(lambda i: ops.gemm(A, Bs[i % nbuf], out=C, **kw), max(8, 2 * nbuf), s)
         tf = 2.0 * M * N * K / us / 1e6
+        ref = ""
+        if cublas:  # torch.matmul on the same operands (no epilogue): the rate this card reaches at this shape
+            Ct = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+            Af = A.t() if a_mn else A
+            us_ref = timed(lambda i: torch.matmul(Af, Bs[i % nbuf] if b_mn else Bs[i % nbuf].t(), out=Ct),
+                           max(8, 2 * nbuf), s)
+            ref = f"  cuBLAS {us_ref:8.1f} us {2.0 * M * N * K / us_ref / 1e6:7.1f} TFLOP/s"
         err = float("nan")
         if check:
             ops.gemm(A, Bs[0], out=C, **kw)
@@ -99,36 +106,37 @@ def main():
                 if res >= 2:
                     want = want + kw["res2"].float()
                 err = ((C.float() - want).norm() / want.norm()).item()
-        print(f"[EPI] {tag:34s} M={M:5d} N={N:5d} K={K:5d}  {us:8.1f} us  {tf:7.1f} TFLOP/s  rel_err={err:.1e}", flush=True)
+        print(f"[EPI] {tag:34s} M={M:5d} N={N:5d} K={K:5d}  {us:8.1f} us  {tf:7.1f} TFLOP/s  rel_err={err:.1e}{ref}",
+              flush=True)
         return us
 
     if "sweep" in only:
-        # fixed cost vs mainloop slope: 64 pair-tiles (one per cluster), plain / residual epilogues
+        # fixed cost vs mainloop slope: 128 tiles of 128 x 256 (one per CTA, one wave), plain / residual epilogues
         for K in (64, 256, 1024, 4096, 16384):
             case("sweep plain", 1024, 4096, K)
         for K in (64, 1024, 4096):
             case("sweep bias+res2", 1024, 4096, K, bias=True, res=2)
-        # epilogue pace: many tiles per cluster, one k-block each (time / tiles-per-cluster = epilogue time per tile)
+        # epilogue pace: 2048 tiles of 128 x 256, 15.5 per CTA, one or four k-blocks each (time / tiles-per-CTA =
+        # epilogue time per tile)
         for K in (64, 256):
-            case("pace plain   (13.8 tiles/cluster)", 8192, 8192, K)
-            case("pace gelu+aux(13.8 tiles/cluster)", 8192, 8192, K, bias=True, act=ops.ACT_GELU_NEW, aux=True)
-            case("pace res1    (13.8 tiles/cluster)", 8192, 8192, K, res=1)
+            case("pace plain   (15.5 tiles/CTA)", 8192, 8192, K)
+            case("pace gelu+aux(15.5 tiles/CTA)", 8192, 8192, K, bias=True, act=ops.ACT_GELU_NEW, aux=True)
+            case("pace res1    (15.5 tiles/CTA)", 8192, 8192, K, res=1)
     if "block" in only:
         M, d = 1024, 4096
-        case("qkv fwd", M, 3 * d, d)
-        case("qkv fwd (+rope epilogue)", M, 3 * d, d, rope=1)
-        case("out fwd (+res1)", M, d, d, res=1)
-        case("fc_in fwd (bias+gelu+aux)", M, 4 * d, d, bias=True, act=ops.ACT_GELU_NEW, aux=True)
-        case("fc_out fwd (+bias)", M, d, 4 * d, bias=True)
-        case("fc_out dgrad (dgelu)", M, 4 * d, d, b_mn=True, dact=ops.DACT_GELU_NEW)
-        case("fc_in dgrad", M, d, 4 * d, b_mn=True)
-        case("qkv dgrad (+res1)", M, d, 3 * d, b_mn=True, res=1)
-        case("lm_head", M, 50258 // 8 * 8, d, bias=True)
+        case("qkv fwd", M, 3 * d, d, cublas=True)
+        case("qkv fwd (+rope epilogue)", M, 3 * d, d, rope=1, cublas=True)
+        case("out fwd (+res1)", M, d, d, res=1, cublas=True)
+        case("fc_in fwd (bias+gelu+aux)", M, 4 * d, d, bias=True, act=ops.ACT_GELU_NEW, aux=True, cublas=True)
+        case("fc_out fwd (+bias)", M, d, 4 * d, bias=True, cublas=True)
+        case("fc_out dgrad (dgelu)", M, 4 * d, d, b_mn=True, dact=ops.DACT_GELU_NEW, cublas=True)
+        case("fc_in dgrad", M, d, 4 * d, b_mn=True, cublas=True)
+        case("qkv dgrad (+res1)", M, d, 3 * d, b_mn=True, res=1, cublas=True)
+        case("lm_head", M, 50258 // 8 * 8, d, bias=True, cublas=True)
     if "adapter" in only:
         M, d, r = 1024, 4096, 1024
         case("adapter down (bias+relu)", M, r, d, bias=True, act=ops.ACT_RELU)
         case("adapter down (no scratch: bn=64)", M, r, d, bias=True, act=ops.ACT_RELU, use_ws=False)
-        case("adapter down pair-forced", M, r, d, bias=True, act=ops.ACT_RELU, force_bn=512)
         case("adapter dgrad-up (no scratch)", M, r, d, b_mn=True, dact=ops.DACT_RELU, use_ws=False)
         case("adapter up (bias+res2)", M, d, r, bias=True, res=2)
         case("adapter dgrad-up (drelu)", M, r, d, b_mn=True, dact=ops.DACT_RELU)
