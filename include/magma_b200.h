@@ -117,7 +117,7 @@ typedef struct {
   void* aux_out;      /* bf16, same ld / batch strides as C, or NULL */
   const void* aux_in; /* bf16, same ld / batch strides as C, or NULL (required when dact != 0) */
   const void* res1;   /* bf16 [M,N], row stride ld_res, batch strides as C, or NULL */
-  const void* res2;   /* bf16 [M,N], row stride ld_res, or NULL */
+  const void* res2;   /* bf16 [M,N], row stride ld_res, batch strides as C, or NULL */
   int64_t ld_res;
   int32_t force_bn;   /* 0 = auto tile width (and split-K plan), else 64, 128 or 256 (no split-K) — testing / tuning */
   /* fused rotary embedding (rotate_every_two, hf:gptj/modeling_gptj.py:57-67) applied to adjacent column pairs after

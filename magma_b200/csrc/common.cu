@@ -43,7 +43,7 @@ int gemm_sms() {
     if (g_gemm_sm_limit < 0) g_gemm_sm_limit = 0;
   }
   const int n = num_sms();
-  return (g_gemm_sm_limit >= 2 && g_gemm_sm_limit < n) ? g_gemm_sm_limit : n;
+  return (g_gemm_sm_limit >= 1 && g_gemm_sm_limit < n) ? g_gemm_sm_limit : n;
 }
 void set_gemm_sm_limit(int n) { g_gemm_sm_limit = n < 0 ? 0 : n; }
 

@@ -74,8 +74,8 @@ struct Epi {
   int rope_mode = 0, rope_S = 0, rope_hd = 0, rope_rot = 0, rope_ncols = 0;
 };
 
-// scratch the training / ViT passes lend to the GEMM core (mb200_gemm_args.splitk_ws): 64 MB of stream-K flags and partial
-// tiles at its end, split-K slices in front (gemm.cu: kStreamKRegion)
+// scratch the training / ViT passes lend to the GEMM core (mb200_gemm_args.splitk_ws): the fp32 per-split partial slices of
+// the GEMMs gemm.cu splits along K (small-M, split_mid and split_few plans); the split count shrinks to what fits
 const size_t kGemmScratchBytes = (size_t)128 << 20;
 
 // split-K scratch of the pass being issued (small-M decode GEMMs stream their weights; see gemm.cu::plan_small_m)
@@ -167,7 +167,7 @@ struct Plan {
   int* n_valid;
   // backward temporaries
   bf16s *g0, *g1, *gs, *dt, *dzn, *dm, *dhact, *dh_mlp, *dattn_o, *dqkv, *dS, *dh, *da, *dhp;
-  void* gemm_ws;  // scratch lent to the GEMM core: stream-K partial tiles of the last wave, split-K slices
+  void* gemm_ws;  // scratch lent to the GEMM core: split-K slices
   size_t gemm_ws_bytes;
   size_t bytes;
 };

@@ -62,8 +62,8 @@ struct Epi {
   int accumulate = 0;
 };
 
-// scratch lent to the GEMM core while a pass is being issued (mb200_gemm_args.splitk_ws: stream-K partial tiles of the
-// last wave — the M = 2056 GEMMs of ViT-L/14 are 1.5 - 2.9 waves of 256 x 256 tiles — and split-K slices)
+// scratch lent to the GEMM core while a pass is being issued (mb200_gemm_args.splitk_ws: the fp32 per-split partial slices
+// of the GEMMs gemm.cu splits along K, e.g. the few-tile, long-K wgrads of the trainable encoder)
 const size_t kGemmScratchBytes = (size_t)128 << 20;
 thread_local void* t_gemm_ws = nullptr;
 thread_local long long t_gemm_ws_bytes = 0;

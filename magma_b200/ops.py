@@ -99,6 +99,13 @@ def gemm(
             if t.dtype != torch.bfloat16:
                 raise TypeError(f"gemm {name} must be bf16")
             setattr(g, name, t.data_ptr())
+    # The kernel gets raw pointers: bias is read as [N] with unit stride, aux and residual tensors at C's batch offsets
+    # (aux also at C's row stride), so any other layout would be read or written out of place.
+    if bias is not None and (tuple(bias.shape) != (N,) or (N > 1 and bias.stride(0) != 1)):
+        raise ValueError(f"gemm bias must be a contiguous [N={N}] vector, got shape {tuple(bias.shape)}")
+    for name, t in (("aux_out", aux_out), ("aux_in", aux_in), ("res1", res1), ("res2", res2)):
+        if t is not None and tuple(t.shape) != tuple(out.shape):
+            raise ValueError(f"gemm {name} shape {tuple(t.shape)} must equal out's {tuple(out.shape)}")
     for name, t in (("aux_out", aux_out), ("aux_in", aux_in)):
         if t is not None and _mat_meta(t, name)[2:] != (ldc, cnb0, cnb1, cbs0, cbs1):
             raise ValueError(f"gemm {name} must share out's strides")
@@ -106,6 +113,8 @@ def gemm(
     for name, t in (("res1", res1), ("res2", res2)):
         if t is not None:
             m = _mat_meta(t, name)
+            if (cnb0 > 1 and m[5] != cbs0) or (cnb1 > 1 and m[6] != cbs1):
+                raise ValueError(f"gemm {name} must share out's batch strides (its row stride may differ)")
             if ld_res and m[2] != ld_res:
                 raise ValueError("res1/res2 must share a row stride")
             ld_res = m[2]

@@ -5,7 +5,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("group", ["basic", "majors", "tails", "epilogue", "batched", "pair", "streamk", "splitk", "smallm"])
+@pytest.mark.parametrize("group", ["basic", "majors", "tails", "epilogue", "batched", "pair", "splitk", "smallm"])
 def test_gemm_group(group):
     import torch
 

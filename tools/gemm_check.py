@@ -12,7 +12,7 @@ import time
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
-GROUPS = ["basic", "majors", "tails", "epilogue", "batched", "pair", "streamk", "splitk", "smallm", "perf"]
+GROUPS = ["basic", "majors", "tails", "epilogue", "batched", "pair", "splitk", "smallm", "perf"]
 
 
 def ref_gemm(A, B, a_mn, b_mn):
@@ -295,94 +295,6 @@ def run_group(g):
         ob = torch.empty(Bsz, S_, H_, hd_, device=dev, dtype=torch.bfloat16)
         ops.gemm(pb, vb.permute(0, 2, 1, 3), out=ob.permute(0, 2, 1, 3), b_mn=True, force_bn=256)
         ok &= report("pair batched PV into [B,S,H,hd]", ob.permute(0, 2, 1, 3), pb.float() @ vb.permute(0, 2, 1, 3).float())
-        # perf vs 1-CTA
-        for (M, N, K, bmn) in ((1024, 4096, 4096, False), (1024, 16384, 4096, False), (1024, 4096, 16384, True), (8192, 8192, 8192, False)):
-            A, B = mk((M, K), False, dev), mk((N, K), bmn, dev)
-            C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-            for bn in (128, 256):
-                for _ in range(3):
-                    ops.gemm(A, B, out=C, b_mn=bmn, force_bn=bn)
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(20):
-                    ops.gemm(A, B, out=C, b_mn=bmn, force_bn=bn)
-                e1.record()
-                torch.cuda.synchronize()
-                ms = e0.elapsed_time(e1) / 20
-                print(f"[PERF] M={M} N={N} K={K} bmn={int(bmn)} {'pair' if bn == 512 else '1cta'}: {ms*1000:.1f} us {2.0*M*N*K/ms/1e9:.1f} TFLOP/s", flush=True)
-    elif g == "streamk":
-        # stream-K of the last wave on the CTA-pair kernel (scratch lent through splitk_ws): the shapes of the GPT-J block
-        # and of the ViT at the benchmark sizes, every epilogue family, bit-reproducible (fixed summation order)
-        import torch.nn.functional as F
-
-        ws = torch.full(((128 << 20) // 4,), float("nan"), device=dev, dtype=torch.float32)  # scratch needs no init
-        for (M, N, K, bmn, what) in ((1024, 4096, 4096, False, "64 tiles / 74 clusters: every tile split in two"),
-                                     (1024, 12288, 4096, False, "2 full waves + 44 tiles"),
-                                     (1024, 16384, 4096, True, "3 full waves + 34 tiles (up to 3 partials per tile)"),
-                                     (1024, 4096, 16384, True, "long K"),
-                                     (2056, 3072, 1024, False, "ViT qkv: ragged M, K = 1024"),
-                                     (1024, 50258, 4096, False, "LM head: ragged N")):
-            A, B = mk((M, K), False, dev, 0.5), mk((N, K), bmn, dev, 0.05)
-            ldc = (N + 7) // 8 * 8
-            C = torch.full((M, ldc), 7.0, device=dev, dtype=torch.bfloat16)
-            ops.gemm(A, B, out=C[:, :N], b_mn=bmn, splitk_ws=ws, force_bn=256)
-            want = ref_gemm(A, B, False, bmn)
-            ok &= report(f"streamk plain M={M} N={N} K={K} ({what})", C[:, :N], want)
-            if ldc > N:
-                ok &= untouched(f"streamk M={M} N={N} columns >= N", C[:, N:], 7.0)
-            C2 = torch.full((M, ldc), 7.0, device=dev, dtype=torch.bfloat16)
-            ops.gemm(A, B, out=C2[:, :N], b_mn=bmn, splitk_ws=ws, force_bn=256)
-            same = bool(torch.equal(C, C2))
-            print(f"[{'OK' if same else 'FAIL'}] streamk M={M} N={N} K={K}: second run bit-identical", flush=True)
-            ok &= same
-        M, N, K = 1024, 4096, 4096
-        A, B = mk((M, K), False, dev, 0.5), mk((N, K), False, dev, 0.05)
-        bias = torch.randn(N, device=dev).to(torch.bfloat16)
-        base = ref_gemm(A, B, False, False)
-        pre = base + bias.float()
-        r1, r2 = mk((M, N), False, dev), mk((M, N), False, dev)
-        C = ops.gemm(A, B, bias=bias, res1=r1, res2=r2, alpha=0.5, splitk_ws=ws, force_bn=256)
-        ok &= report("streamk alpha+bias+res1+res2", C, 0.5 * base + bias.float() + r1.float() + r2.float())
-        aux = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-        C = ops.gemm(A, B, bias=bias, act=ops.ACT_GELU_NEW, aux_out=aux, splitk_ws=ws, force_bn=256)
-        ok &= report("streamk bias+gelu_new+aux: C", C, F.gelu(pre, approximate="tanh"))
-        ok &= report("streamk bias+gelu_new+aux: aux", aux, pre)
-        x = mk((M, N), False, dev)
-        C = ops.gemm(A, B, aux_in=x, dact=ops.DACT_RELU, splitk_ws=ws, force_bn=256)
-        ok &= report("streamk dact relu", C, base * (x.float() > 0).float())
-        Cf = torch.ones(M, N, device=dev, dtype=torch.float32)
-        ops.gemm(A, B, out=Cf, accumulate=True, splitk_ws=ws, force_bn=256)
-        ok &= report("streamk f32 accumulate", Cf, base + 1.0, tol=5e-3)
-        Sx, H, hd, rot = 128, 16, 256, 64
-        A2, B2 = mk((8 * Sx, 4096), False, dev, 0.5), mk((3 * H * hd, 4096), False, dev, 0.05)
-        tab = ops.rope_table(Sx, rot, pos0=0, device=dev)
-        fused = ops.gemm(A2, B2, rope_tab=tab, rope_mode=1, rope_S=Sx, rope_hd=hd, rope_rot=rot, rope_ncols=2 * H * hd,
-                         splitk_ws=ws, force_bn=256)
-        plain = ops.gemm(A2, B2, out_dtype=torch.float32)
-        qq = plain.view(8, Sx, 3, H, hd).clone()
-        cs, sn = tab[None, :, None, None, :, 0], tab[None, :, None, None, :, 1]
-        x1, x2 = qq[:, :, :2, :, 0:rot:2].clone(), qq[:, :, :2, :, 1:rot:2].clone()
-        qq[:, :, :2, :, 0:rot:2] = x1 * cs - x2 * sn
-        qq[:, :, :2, :, 1:rot:2] = x2 * cs + x1 * sn
-        ok &= report("streamk qkv + fused rope (2 full waves + 44 tiles)", fused, qq.view(8 * Sx, -1))
-        for (M, N, K, bmn) in ((1024, 4096, 4096, False), (1024, 12288, 4096, False), (1024, 16384, 4096, False),
-                               (1024, 4096, 16384, True)):
-            A, B = mk((M, K), False, dev), mk((N, K), bmn, dev)
-            C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-            for tag, w in (("stream-K", ws), ("whole tiles", None)):
-                fb = 256 if w is not None else 0
-                for _ in range(3):
-                    ops.gemm(A, B, out=C, b_mn=bmn, splitk_ws=w, force_bn=fb)
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(20):
-                    ops.gemm(A, B, out=C, b_mn=bmn, splitk_ws=w, force_bn=fb)
-                e1.record()
-                torch.cuda.synchronize()
-                ms = e0.elapsed_time(e1) / 20
-                print(f"[PERF] M={M} N={N} K={K} bmn={int(bmn)} {tag}: {ms*1000:.1f} us {2.0*M*N*K/ms/1e9:.1f} TFLOP/s", flush=True)
     elif g == "splitk":
         import torch.nn.functional as F
 
@@ -411,23 +323,6 @@ def run_group(g):
         b = ops.gemm(A2, B2, **kw)
         torch.cuda.synchronize()
         ok &= report("splitk rope epilogue == single-pass rope epilogue", a, b.float())
-        for (M, N, K) in ((32, 12288, 4096), (32, 16384, 4096), (32, 4096, 16384), (32, 4096, 4096), (32, 1024, 4096), (32, 50258, 4096)):
-            A, B = mk((M, K), False, dev), mk((N, K), False, dev)
-            ldc = (N + 63) // 64 * 64
-            C = torch.empty(M, ldc, device=dev, dtype=torch.bfloat16)[:, :N]
-            for use in (False, True):
-                kw = dict(splitk_ws=ws) if use else {}
-                for _ in range(3):
-                    ops.gemm(A, B, out=C, **kw)
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(20):
-                    ops.gemm(A, B, out=C, **kw)
-                e1.record()
-                torch.cuda.synchronize()
-                ms = e0.elapsed_time(e1) / 20
-                print(f"[PERF] M={M} N={N} K={K} {'splitk' if use else 'single'}: {ms*1000:.1f} us  {N*K*2/ms/1e6:.0f} GB/s weights", flush=True)
     elif g == "smallm":
         # M <= 32: 32-row A ring (deeper pipeline). All tile widths, both B majors, fused epilogues, ragged N/K.
         import torch.nn.functional as F
@@ -447,20 +342,6 @@ def run_group(g):
         for bn in (64, 128, 256):
             A, B = mk((32, 512), False, dev), mk((512, 512), False, dev)
             ok &= report(f"smallm forced bn={bn}", ops.gemm(A, B, force_bn=bn), ref_gemm(A, B, False, False))
-        for (M, N, K) in ((32, 12288, 4096), (32, 16384, 4096), (32, 4096, 4096), (32, 1024, 4096), (32, 4096, 1024)):
-            A, B = mk((M, K), False, dev), mk((N, K), False, dev)
-            C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-            for _ in range(3):
-                ops.gemm(A, B, out=C)
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(20):
-                ops.gemm(A, B, out=C)
-            e1.record()
-            torch.cuda.synchronize()
-            ms = e0.elapsed_time(e1) / 20
-            print(f"[PERF] smallm M={M} N={N} K={K}: {ms*1000:.1f} us  {N*K*2/ms/1e6:.0f} GB/s weights", flush=True)
     elif g == "perf":
         shapes = [
             (1024, 4096, 4096, False, False, "out/qkv-like fwd"),
@@ -507,6 +388,39 @@ def run_group(g):
             ms = e0.elapsed_time(e1) / 20
             print(f"[PERF]   cuBLAS same shape: {ms*1000:.1f} us  {2.0*M*N*K/ms/1e9:.1f} TFLOP/s", flush=True)
             ok &= report(f"perf-shape correctness {name}", C, ref_gemm(A, B, a_mn, b_mn))
+        # split-K vs single pass and the small-M plan (weight-streaming GEMMs)
+        ws = torch.full((16 * 128 * 8192,), float("nan"), device=dev, dtype=torch.float32)
+        for (M, N, K) in ((32, 12288, 4096), (32, 16384, 4096), (32, 4096, 16384), (32, 4096, 4096), (32, 1024, 4096), (32, 50258, 4096)):
+            A, B = mk((M, K), False, dev), mk((N, K), False, dev)
+            ldc = (N + 63) // 64 * 64
+            C = torch.empty(M, ldc, device=dev, dtype=torch.bfloat16)[:, :N]
+            for use in (False, True):
+                kw = dict(splitk_ws=ws) if use else {}
+                for _ in range(3):
+                    ops.gemm(A, B, out=C, **kw)
+                torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(20):
+                    ops.gemm(A, B, out=C, **kw)
+                e1.record()
+                torch.cuda.synchronize()
+                ms = e0.elapsed_time(e1) / 20
+                print(f"[PERF] M={M} N={N} K={K} {'splitk' if use else 'single'}: {ms*1000:.1f} us  {N*K*2/ms/1e6:.0f} GB/s weights", flush=True)
+        for (M, N, K) in ((32, 12288, 4096), (32, 16384, 4096), (32, 4096, 4096), (32, 1024, 4096), (32, 4096, 1024)):
+            A, B = mk((M, K), False, dev), mk((N, K), False, dev)
+            C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+            for _ in range(3):
+                ops.gemm(A, B, out=C)
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(20):
+                ops.gemm(A, B, out=C)
+            e1.record()
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1) / 20
+            print(f"[PERF] smallm M={M} N={N} K={K}: {ms*1000:.1f} us  {N*K*2/ms/1e6:.0f} GB/s weights", flush=True)
     print(f"GROUP {g}: {'PASS' if ok else 'FAIL'}", flush=True)
     return 0 if ok else 1
 
