@@ -160,7 +160,8 @@ int mb200_rope(void* qkv, int64_t ld, int32_t rows, int32_t S, int32_t H, int32_
 /* (cos, sin) table fp32 [S][rot/2][2] for positions pos0 .. pos0+S-1 (create_sinusoidal_positions,
  * hf:gptj/modeling_gptj.py:47-50) consumed by the GEMM's fused rotary epilogue. */
 int mb200_rope_table(float* tab, int32_t S, int32_t rot, int32_t pos0, void* stream);
-/* softmax(scale*s [+ causal mask]) fp32 -> bf16 (GPTJAttention._attn, hf:gptj/modeling_gptj.py:136-147). */
+/* softmax(scale*s [+ causal mask]) fp32 -> bf16 (GPTJAttention._attn, hf:gptj/modeling_gptj.py:136-147). Writes
+ * columns [0, Sk) of each row (zeros beyond the causal limit); columns [Sk, ldp) are left as they are. */
 int mb200_softmax_fwd(const float* s, int64_t lds, int64_t s_bs, void* p, int64_t ldp, int64_t p_bs, int32_t nz,
                       int32_t Sq, int32_t Sk, float scale, int32_t causal, int32_t koff, void* stream);
 int mb200_softmax_bwd(const float* dp, int64_t lddp, int64_t dp_bs, const void* p, int64_t ldp, int64_t p_bs,
@@ -435,9 +436,10 @@ int mb200_scale_add(const void* u, const float* s, const void* r1, const void* r
 int mb200_dot(const void* a, const void* b, int64_t n, float* out, int32_t accumulate, void* stream);
 
 /* Fused causal self-attention for sequences that fit one tile (S <= 128, head_dim a multiple of 64, <= 256): one CTA
- * per (batch, head), S = QK^T / softmax / PV entirely on-chip (TMEM + smem). qkv is the fused, already-rotated
- * [B*S][3][H][hd] buffer; P (bf16 [B,H,S,ldP]) is saved for the backward pass; O is [B,S,H,hd] with row stride ldo.
- * GPTJAttention._attn, hf:gptj/modeling_gptj.py:136-149. */
+ * per (batch, head), S = QK^T / softmax / PV entirely on-chip (wgmma register accumulators + smem). qkv is the fused,
+ * already-rotated [B*S][3][H][hd] buffer; P (bf16 [B,H,S,ldP]) is saved for the backward pass: columns
+ * [0, min(ldP, 128)) of each row are written (zeros beyond S), columns from 128 on are left as they are. O is
+ * [B,S,H,hd] with row stride ldo. GPTJAttention._attn, hf:gptj/modeling_gptj.py:136-149. */
 int mb200_attn_fwd_tile(const void* qkv, int64_t ld_qkv, void* P, int64_t ldP, void* O, int64_t ldo, int32_t B,
                         int32_t S, int32_t H, int32_t hd, void* stream);
 /* Backward of the above: dqkv [B*S][3][H][hd] receives dQ, dK (inverse rotary applied through rope_tab, which may be
@@ -446,12 +448,13 @@ int mb200_attn_bwd_tile(const void* qkv, int64_t ld_qkv, const void* dO, int64_t
                         void* dqkv, int64_t ld_dqkv, const float* rope_tab, int32_t rot, int32_t B, int32_t S, int32_t H,
                         int32_t hd, void* stream);
 /* The forward attention for ANY sequence length (multi-tile): one CTA per (128-query tile, head, batch) sweeps the key
- * tiles twice (row max / sum, then bf16 probabilities and O += P V in TMEM), so no [B,H,S,S] fp32 score buffer exists
- * and the probabilities are rounded exactly where the materialised softmax rounds them. q / k / v point at head 0,
+ * tiles twice (row max / sum, then bf16 probabilities and O += P V in wgmma register accumulators), so no [B,H,S,S]
+ * fp32 score buffer exists and the probabilities are rounded to bf16 where the materialised softmax rounds them (the
+ * row sums are taken in a different order, so rare one-ulp differences remain). q / k / v point at head 0,
  * batch 0, row 0 with row stride ld*, head stride *_bsh and batch stride *_bsb in elements: the fused qkv buffer
  * (ld = 3d, bsh = hd, bsb = S * 3d) or a KV cache [B,H,Smax,hd] (ld = hd, bsh = Smax * hd, bsb = H * Smax * hd).
  * causal != 0: key j is visible to query i iff j <= i + (Sk - Sq) (prefill and its continuations). P (optional, bf16
- * [B,H,Sq,ldP], ldP >= Sk and % 8) is written for a materialised backward; stats (optional, [B,H,Sq][2]) receives the
+ * [B,H,Sq,ldP], ldP >= Sk and % 8) is written for a materialised backward, every column [0, ldP) (zeros from Sk on); stats (optional, [B,H,Sq][2]) receives the
  * row maximum of the scaled scores and 1 / sum. Replaces, for S > 128 and for the ViT (T = 257), the QK^T GEMM + softmax
  * kernel + PV GEMM of hf:gptj/modeling_gptj.py:136-149 / hf:clip/modeling_clip.py:282-330 (magma/magma.py:44: the
  * reference runs at seq_len 2048). */
@@ -461,7 +464,8 @@ int mb200_attn_fwd_flash(const void* q, int64_t ldq, int64_t q_bsh, int64_t q_bs
                          int32_t hd, int32_t causal, void* stream);
 
 /* Fused KV-cache attention for one decode step (Sq = 1): q/k/v come from the fused qkv row [B][3][H][hd] (already
- * rotated); k,v are appended to the cache at position `pos`, then softmax(q K^T / sqrt(hd)) V over [0, pos].
+ * rotated); k,v are appended to the cache at position `pos`, then softmax(q K^T / sqrt(hd)) V over [0, pos]. The
+ * scores live in shared memory, so pos < 51,168 (200 KB; the same limit applies to S_kv_max in mb200_attn_decode_dev).
  * Replaces the torch.cat cache growth + _attn of hf:gptj/modeling_gptj.py:209-214,136-149 per step. */
 int mb200_attn_decode(const void* qkv, int64_t ld_qkv, void* kcache, void* vcache, void* out, int64_t ld_out,
                       int32_t B, int32_t H, int32_t hd, int32_t S_kv_max, int32_t pos, void* stream);

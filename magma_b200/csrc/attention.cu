@@ -325,8 +325,10 @@ attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 // hf:clip/modeling_clip.py:282-330), obtained with two sweeps over the key tiles instead of an online rescale:
 //   sweep 1: S_j = Q K_j^T per 128-key tile, running row maximum m and sum l = sum exp(s - m)          (no V, no O)
 //   sweep 2: S_j again, p = bf16(exp(s - m) / l) exactly as the materialised path rounds it, O += P_j V_j in registers
-// so O never needs rescaling and P — when the caller wants it for the backward pass — is bit-identical to what
-// softmax_fwd_kernel would have written. QK^T is computed twice: +50 % of the attention FLOPs, which are < 1 % of the
+// so O never needs rescaling and P — when the caller wants it for the backward pass — is rounded where
+// softmax_fwd_kernel rounds it. The two sum exp(s - m) in different orders (per-tile quad sums with a running rescale
+// here, lane-strided warp sums there), so 1 / sum can differ in its last bits and a bf16 rounding can flip: rare
+// one-ulp differences (on an H100: 14 of 2.1 M probabilities at the ViT shape, 80 of 16.8 M at GPT-J S = 2048). QK^T is computed twice: +50 % of the attention FLOPs, which are < 1 % of the
 // step, in exchange for no [B,H,S,S] fp32 score buffer. K / V tiles are double-buffered (TMA of tile j+1 under the
 // softmax of tile j) when head_dim <= 128; at head_dim 256 one buffer each fits next to Q and P (224 KB) and the next
 // tile is prefetched into L2 instead.

@@ -110,6 +110,20 @@ attn_decode_kernel(const bf16* __restrict__ qkv, long long ld_qkv, bf16* __restr
   }
 }
 
+// Dynamic shared memory of a decode launch that scores n_keys keys ([n_keys] fp32 scores padded to 32, then the [32]
+// reduction scratch), checked against the 200 KB the kernel is opted in to — beyond the 48 KB default, so caches longer
+// than about 12,000 positions can be used.
+static int decode_smem(long long n_keys, size_t* smem) {
+  *smem = (((size_t)n_keys + 31) & ~(size_t)31) * 4 + 32 * 4;
+  MB_REQUIRE(*smem <= 200 * 1024, MB200_E_SHAPE, "attn_decode: %lld keys need %zu bytes of shared memory", n_keys, *smem);
+  static bool set = false;
+  if (!set) {
+    MB_CUDA(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    set = true;
+  }
+  return 0;
+}
+
 }  // namespace mb200
 
 using namespace mb200;
@@ -121,7 +135,8 @@ extern "C" int mb200_attn_decode(const void* qkv, int64_t ld_qkv, void* kcache, 
   if (rc) return rc;
   MB_REQUIRE(hd % 8 == 0 && pos >= 0 && pos < S_kv_max, MB200_E_SHAPE, "attn_decode: bad hd=%d pos=%d Smax=%d", hd, pos,
              S_kv_max);
-  const size_t smem = (((size_t)(pos + 1) + 31) & ~(size_t)31) * 4 + 32 * 4;
+  size_t smem;
+  if ((rc = decode_smem((long long)pos + 1, &smem))) return rc;
   attn_decode_kernel<<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>((const bf16*)qkv, ld_qkv, (bf16*)kcache,
                                                                          (bf16*)vcache, (bf16*)out, ld_out, H, hd,
                                                                          S_kv_max, pos, nullptr);
@@ -138,14 +153,8 @@ extern "C" int mb200_attn_decode_dev(const void* qkv, int64_t ld_qkv, void* kcac
   if (rc) return rc;
   MB_REQUIRE(hd % 8 == 0 && S_kv_max > 0 && pos_dev != nullptr, MB200_E_SHAPE, "attn_decode_dev: bad hd=%d Smax=%d", hd,
              S_kv_max);
-  const size_t smem = (((size_t)S_kv_max + 31) & ~(size_t)31) * 4 + 32 * 4;
-  MB_REQUIRE(smem <= 200 * 1024, MB200_E_SHAPE, "attn_decode_dev: cache length %d needs %zu bytes of shared memory", S_kv_max,
-             smem);
-  static bool set = false;
-  if (!set) {
-    MB_CUDA(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    set = true;
-  }
+  size_t smem;
+  if ((rc = decode_smem(S_kv_max, &smem))) return rc;
   attn_decode_kernel<<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>((const bf16*)qkv, ld_qkv, (bf16*)kcache,
                                                                          (bf16*)vcache, (bf16*)out, ld_out, H, hd,
                                                                          S_kv_max, 0, pos_dev);

@@ -200,20 +200,31 @@ def rope_table(S, rot, pos0=0, device=None):
     return tab
 
 
-def softmax_fwd(s, scale, causal, koff=0, ldp=None):
-    """s: fp32 [nz, Sq, Sk(ld)] -> bf16 probabilities with the same padded layout."""
+def softmax_fwd(s, scale, causal, koff=0, out=None):
+    """s: fp32 [nz, Sq, Sk(ld)] -> bf16 probabilities with the same padded layout, or into `out` (bf16 [nz, Sq, Sk] with
+    unit column stride, any row and batch strides). Columns [0, Sk) of each row are written."""
     nz, Sq, Sk = s.shape
     lds = s.stride(1)
-    p = torch.zeros(nz, Sq, lds, dtype=torch.bfloat16, device=s.device)[..., :Sk]
+    p = torch.zeros(nz, Sq, lds, dtype=torch.bfloat16, device=s.device)[..., :Sk] if out is None else out
+    _batched_out(p, "out", (nz, Sq, Sk))
     check(lib().mb200_softmax_fwd(_ptr(s), ctypes.c_int64(lds), ctypes.c_int64(s.stride(0)), _ptr(p),
                                   ctypes.c_int64(p.stride(1)), ctypes.c_int64(p.stride(0)), nz, Sq, Sk,
                                   ctypes.c_float(scale), int(causal), koff, _stream()))
     return p
 
 
-def softmax_bwd(dp, p, scale):
+def _batched_out(t, name, shape):
+    if t.dtype != torch.bfloat16 or tuple(t.shape) != shape or (shape[-1] > 1 and t.stride(-1) != 1):
+        raise ValueError(f"{name} must be a bf16 {list(shape)} view with unit column stride, got {t.dtype} "
+                         f"{tuple(t.shape)} strides {t.stride()}")
+
+
+def softmax_bwd(dp, p, scale, out=None):
+    """dS = P * (dP - rowsum(dP * P)) * scale: fp32 dp and bf16 p [nz, Sq, Sk] -> bf16, in the padded layout of p or
+    into `out` (bf16 [nz, Sq, Sk] with unit column stride)."""
     nz, Sq, Sk = dp.shape
-    ds = torch.zeros(nz, Sq, p.stride(1), dtype=torch.bfloat16, device=dp.device)[..., :Sk]
+    ds = torch.zeros(nz, Sq, p.stride(1), dtype=torch.bfloat16, device=dp.device)[..., :Sk] if out is None else out
+    _batched_out(ds, "out", (nz, Sq, Sk))
     check(lib().mb200_softmax_bwd(_ptr(dp), ctypes.c_int64(dp.stride(1)), ctypes.c_int64(dp.stride(0)), _ptr(p),
                                   ctypes.c_int64(p.stride(1)), ctypes.c_int64(p.stride(0)), _ptr(ds),
                                   ctypes.c_int64(ds.stride(1)), ctypes.c_int64(ds.stride(0)), nz, Sq, Sk,
@@ -450,28 +461,63 @@ def adamw_step(master, grad, m1, m2, shadow, lr, beta1, beta2, eps, wd, grad_sca
                                  int(zero_grad), _stream()))
 
 
-def attn_fwd_tile(qkv, B, S, H, hd):
+def _rows_out(t, name, rows, cols, dtype=torch.bfloat16):
+    """Row stride of a caller-supplied [rows, cols] output with unit column stride."""
+    if t.dtype != dtype or tuple(t.shape) != (rows, cols) or (cols > 1 and t.stride(1) != 1):
+        raise ValueError(f"{name} must be a {dtype} [{rows}, {cols}] view with unit column stride, got "
+                         f"{t.dtype} {tuple(t.shape)} strides {t.stride()}")
+    return t.stride(0) if rows > 1 else max(cols, t.stride(0))
+
+
+def _p_out(P, B, H, S, min_cols):
+    """Row stride ldP of a caller-supplied P [B, H, S, ldP]: the kernels address row (b, h, i) at ((b H + h) S + i) ldP,
+    so the view must be contiguous apart from its last dim, which may be cut short of the row stride."""
+    ldP = P.stride(2)
+    want = (H * S * ldP, S * ldP, ldP)
+    if (P.dtype != torch.bfloat16 or P.dim() != 4 or tuple(P.shape[:3]) != (B, H, S) or P.stride(3) != 1
+            or any(n > 1 and s != w for n, s, w in zip(P.shape[:3], P.stride()[:3], want)) or ldP % 8
+            or ldP < min_cols):
+        raise ValueError(f"P must be a bf16 [B={B}, H={H}, S={S}, >= {min_cols}] view of a [B, H, S, ldP] buffer "
+                         f"(ldP % 8 == 0), got shape {tuple(P.shape)} strides {P.stride()}")
+    return ldP
+
+
+def attn_fwd_tile(qkv, B, S, H, hd, O=None, P=None):
     """Fused single-tile causal attention (S <= 128). qkv: bf16 [B*S, 3*H*hd] already rotated.
-    Returns (O [B*S, H*hd], P [B, H, S, ldP])."""
-    ldP = (S + 7) // 8 * 8
-    P = torch.zeros(B, H, S, ldP, dtype=torch.bfloat16, device=qkv.device)
-    O = torch.empty(B * S, H * hd, dtype=torch.bfloat16, device=qkv.device)
+    Returns (O [B*S, H*hd], P [B, H, S, ldP]). O and P may be given with padded row strides; the kernel writes columns
+    [0, min(ldP, 128)) of every row of P."""
+    if P is None:
+        P = torch.zeros(B, H, S, (S + 7) // 8 * 8, dtype=torch.bfloat16, device=qkv.device)
+    ldP = _p_out(P, B, H, S, S)
+    if O is None:
+        O = torch.empty(B * S, H * hd, dtype=torch.bfloat16, device=qkv.device)
+    ldo = _rows_out(O, "O", B * S, H * hd)
     check(lib().mb200_attn_fwd_tile(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(P), ctypes.c_int64(ldP), _ptr(O),
-                                    ctypes.c_int64(H * hd), B, S, H, hd, _stream()))
+                                    ctypes.c_int64(ldo), B, S, H, hd, _stream()))
     return O, P
 
 
-def attn_fwd_flash(qkv, B, S, H, hd, causal=True, want_p=False, want_stats=False, kcache=None, vcache=None, pos0=0):
+def attn_fwd_flash(qkv, B, S, H, hd, causal=True, want_p=False, want_stats=False, kcache=None, vcache=None, pos0=0,
+                   O=None, P=None, stats=None):
     """Multi-tile attention forward for any sequence length (mb200_attn_fwd_flash). qkv: bf16 [B*S, 3*H*hd] (already
     rotated) supplies the queries and — without a cache — the keys / values. With kcache / vcache ([B, H, Smax, hd],
     positions [0, pos0 + S) valid) the keys / values come from the cache (prefill continuation: queries are the last S
-    of the pos0 + S positions). Returns O [B*S, H*hd] (+ P [B, H, S, ldP]) (+ stats [B, H, S, 2])."""
+    of the pos0 + S positions). Returns O [B*S, H*hd] (+ P [B, H, S, ldP]) (+ stats [B, H, S, 2]). O and P may be
+    given with padded row strides (P then need not be asked for with want_p; every column [0, ldP) is written), stats
+    as a contiguous fp32 [B, H, S, 2]."""
     d = H * hd
     Sk = pos0 + S if kcache is not None else S
-    O = torch.empty(B * S, d, dtype=torch.bfloat16, device=qkv.device)
-    ldP = (Sk + 7) // 8 * 8
-    P = torch.empty(B, H, S, ldP, dtype=torch.bfloat16, device=qkv.device) if want_p else None
-    stats = torch.empty(B, H, S, 2, dtype=torch.float32, device=qkv.device) if want_stats else None
+    if O is None:
+        O = torch.empty(B * S, d, dtype=torch.bfloat16, device=qkv.device)
+    ldo = _rows_out(O, "O", B * S, d)
+    if P is None and want_p:
+        P = torch.empty(B, H, S, (Sk + 7) // 8 * 8, dtype=torch.bfloat16, device=qkv.device)
+    ldP = _p_out(P, B, H, S, Sk) if P is not None else 0
+    if stats is None and want_stats:
+        stats = torch.empty(B, H, S, 2, dtype=torch.float32, device=qkv.device)
+    if stats is not None and (stats.dtype != torch.float32 or tuple(stats.shape) != (B, H, S, 2)
+                              or not stats.is_contiguous()):
+        raise ValueError(f"stats must be a contiguous fp32 [{B}, {H}, {S}, 2] tensor")
     ld = qkv.stride(0)
     if kcache is not None:
         Smax = kcache.shape[2]
@@ -480,7 +526,7 @@ def attn_fwd_flash(qkv, B, S, H, hd, causal=True, want_p=False, want_stats=False
         kk, vv, ldk, bsh, bsb = qkv.data_ptr() + 2 * d, qkv.data_ptr() + 4 * d, ld, hd, S * ld
     c64, vp = ctypes.c_int64, ctypes.c_void_p
     check(lib().mb200_attn_fwd_flash(_ptr(qkv), c64(ld), c64(hd), c64(S * ld), vp(kk), c64(ldk), c64(bsh), c64(bsb),
-                                     vp(vv), c64(ldk), c64(bsh), c64(bsb), _ptr(O), c64(d), _ptr(P), c64(ldP),
+                                     vp(vv), c64(ldk), c64(bsh), c64(bsb), _ptr(O), c64(ldo), _ptr(P), c64(ldP),
                                      _ptr(stats), B, S, Sk, H, hd, int(bool(causal)), _stream()))
     out = (O,)
     if want_p:
@@ -490,10 +536,42 @@ def attn_fwd_flash(qkv, B, S, H, hd, causal=True, want_p=False, want_stats=False
     return out if len(out) > 1 else O
 
 
-def attn_bwd_tile(qkv, dO, P, B, S, H, hd, rope_tab=None, rot=0):
-    """Backward of attn_fwd_tile -> dqkv [B*S, 3*H*hd] (inverse rotary applied to dq, dk when rope_tab is given)."""
-    dqkv = torch.empty_like(qkv)
+def attn_bwd_tile(qkv, dO, P, B, S, H, hd, rope_tab=None, rot=0, dqkv=None):
+    """Backward of attn_fwd_tile -> dqkv [B*S, 3*H*hd] (inverse rotary applied to dq, dk when rope_tab is given).
+    dqkv may be given with a padded row stride."""
+    if dqkv is None:
+        dqkv = torch.empty(B * S, 3 * H * hd, dtype=torch.bfloat16, device=qkv.device)
+    ld = _rows_out(dqkv, "dqkv", B * S, 3 * H * hd)
     check(lib().mb200_attn_bwd_tile(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(dO), ctypes.c_int64(dO.stride(0)),
-                                    _ptr(P), ctypes.c_int64(P.stride(2)), _ptr(dqkv), ctypes.c_int64(dqkv.stride(0)),
+                                    _ptr(P), ctypes.c_int64(_p_out(P, B, H, S, S)), _ptr(dqkv), ctypes.c_int64(ld),
                                     _ptr(rope_tab), int(rot), B, S, H, hd, _stream()))
     return dqkv
+
+
+def kv_append(qkv, kcache, vcache, B, S, H, hd, pos0):
+    """K / V of the fused qkv rows [B*S, 3*H*hd] (row stride qkv.stride(0)) into the caches [B, H, Smax, hd] at
+    positions [pos0, pos0 + S) (mb200_kv_append)."""
+    check(lib().mb200_kv_append(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(kcache), _ptr(vcache), B, S, H, hd,
+                                kcache.shape[2], pos0, _stream()))
+
+
+def attn_decode(qkv, kcache, vcache, B, H, hd, pos, out=None):
+    """One decode step (mb200_attn_decode): qkv [B, 3*H*hd] (one already-rotated row per batch, row stride
+    qkv.stride(0)) appends its k, v at cache position `pos` of kcache / vcache [B, H, Smax, hd], then attends over
+    [0, pos]. Returns out [B, H*hd] (may be given with a padded row stride)."""
+    if out is None:
+        out = torch.empty(B, H * hd, dtype=torch.bfloat16, device=qkv.device)
+    ldo = _rows_out(out, "out", B, H * hd)
+    check(lib().mb200_attn_decode(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(kcache), _ptr(vcache), _ptr(out),
+                                  ctypes.c_int64(ldo), B, H, hd, kcache.shape[2], int(pos), _stream()))
+    return out
+
+
+def attn_decode_dev(qkv, kcache, vcache, B, H, hd, pos_dev, out=None):
+    """attn_decode with the cache position read from device memory (int32 [1]; mb200_attn_decode_dev)."""
+    if out is None:
+        out = torch.empty(B, H * hd, dtype=torch.bfloat16, device=qkv.device)
+    ldo = _rows_out(out, "out", B, H * hd)
+    check(lib().mb200_attn_decode_dev(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(kcache), _ptr(vcache), _ptr(out),
+                                      ctypes.c_int64(ldo), B, H, hd, kcache.shape[2], _ptr(pos_dev), _stream()))
+    return out

@@ -688,7 +688,8 @@ int mb200_attn_fwd_tile(const void* qkv_, int64_t ld, void* P_, int64_t ldP, voi
         }
         for (int j = 0; j <= i; ++j) sum += expf(sc[j] - m);
         bf16_t* pr = P + ((b * H + h) * S + i) * ldP;
-        for (int j = 0; j < S; ++j) pr[j] = f2b(j <= i ? expf(sc[j] - m) / sum : 0.f);
+        // the kernel writes columns [0, min(ldP, 128)): zeros past the diagonal and past S
+        for (int j = 0; j < (ldP < 128 ? ldP : 128); ++j) pr[j] = f2b(j <= i ? expf(sc[j] - m) / sum : 0.f);
         bf16_t* o = O + (b * S + i) * ldo + (long long)h * hd;
         for (int c = 0; c < hd; ++c) {
           float acc = 0.f;

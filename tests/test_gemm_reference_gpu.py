@@ -22,63 +22,13 @@ import os
 
 import pytest
 
+from _refcheck import SENTINEL, ulp_bf16
+from _refcheck import Buf as _Buf, bits as _bits, dev as _dev, launches as _launches, rand as _rand
+
 pytestmark = pytest.mark.gpu
 
-SENTINEL = -1.5e38
 ACT = dict(none=0, gelu_new=1, quick_gelu=2, relu=3, relu_post=4)
 DACT = dict(none=0, gelu_new=1, relu=3)
-
-
-def _dev():
-    """cuda:0 — or the CPU when tests/test_gemm_reference_twin_cpu.py replays a test body on the emulated operator."""
-    import torch
-
-    return torch.device(os.environ.get("MB200_TEST_DEVICE", "cuda:0"))
-
-
-def _launches():
-    from magma_b200._lib import lib
-
-    return lib().mb200_launch_count()
-
-
-class _Buf:
-    """A [*lead, rows, cols] view into a flat storage filled with `fill`: row stride `ld` (default: cols rounded up to 8,
-    plus 8), 3 spare rows per batch and, unless given, batch strides that are not those of a contiguous tensor (the
-    outer batch dim has the smaller stride, and a gap of one batch follows)."""
-
-    def __init__(self, lead, rows, cols, dtype, dev, fill, ld=None, bstrides=None):
-        import torch
-
-        ld = ld or (cols + 7) // 8 * 8 + 8
-        plane = (rows + 3) * ld
-        if bstrides is None:
-            bstrides = (plane, (lead[0] + 1) * plane)[: len(lead)] if len(lead) == 2 else (2 * plane,) * len(lead)
-        size = sum((n - 1) * s for n, s in zip(lead, bstrides)) + plane + 8
-        self.shape, self.strides = (*lead, rows, cols), (*bstrides, ld, 1)
-        self.storage = torch.full((size,), fill, dtype=dtype, device=dev)
-        self.view = self.storage.as_strided(self.shape, self.strides)
-        inside = torch.zeros(size, dtype=torch.bool, device=dev)
-        inside.as_strided(self.shape, self.strides).fill_(True)
-        self.outside = ~inside
-        self.fill = torch.full((1,), fill, dtype=dtype, device=dev)
-
-    def overwritten(self):
-        return int((self.storage[self.outside] != self.fill).sum().item())
-
-
-def _rand(shape, gen, scale, dev, dtype=None):
-    import torch
-
-    t = torch.randn(*shape, generator=gen, dtype=torch.float64) * scale
-    return t.to(dtype or torch.bfloat16).to(dev)
-
-
-def _bits(t):
-    import torch
-
-    t = t.contiguous()
-    return t.view(torch.int16 if t.element_size() == 2 else torch.int32).clone()
 
 
 def _rope_params(M, N):
@@ -144,12 +94,7 @@ def _check(name, got, ref, bound_acc, f32, amb=None):
     """The element-wise criterion; prints the largest err / bound ratio, or fails with the worst element."""
     import torch
 
-    ref_abs = ref.abs()
-    if f32:
-        ulp = ref_abs * 2.0**-22
-    else:
-        _, e = torch.frexp(ref_abs.clamp(min=2.0**-126))  # |ref| in [2^(e-1), 2^e): bf16 ulp 2^(e-8)
-        ulp = torch.ldexp(torch.ones_like(ref), e - 8)
+    ulp = ref.abs() * 2.0**-22 if f32 else ulp_bf16(ref)
     bound = ulp + bound_acc
     err = (got.double() - ref).abs()
     ratio = torch.nan_to_num(err / bound, nan=math.inf)
