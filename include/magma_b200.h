@@ -381,7 +381,8 @@ typedef struct {
 } mb200_gptj_model_ex;
 
 /* bytes of caller-provided workspace for a [B,S] training pass (per-layer activations are kept: 122 MB per GPT-J-6B
- * layer at B = 8, S = 128; nothing is recomputed — the reference uses gradient checkpointing, language_model.py:23). */
+ * layer at B = 8, S = 128; nothing is recomputed — see mb200_gptj_sched_forward_recompute for the pass that
+ * recomputes, as the reference's gradient checkpointing does, language_model.py:23). */
 size_t mb200_gptj_sched_workspace_bytes(const mb200_gptj_model_ex* m, int32_t B, int32_t S);
 /* GPTJForCausalLM.forward(inputs_embeds=x, labels=labels) as called from magma/magma.py:270-274.
  * x bf16 [B,S,d]; labels int64 [B,S] or NULL; logits bf16 [B*S][ldv] or NULL (kept in the workspace then);
@@ -400,6 +401,22 @@ int mb200_gptj_sched_backward(const mb200_gptj_model_ex* m, void* dx, float loss
 int mb200_gptj_sched_backward_range(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t layer_hi,
                                     int32_t layer_lo, int32_t accumulate, int32_t B, int32_t S, void* ws,
                                     size_t ws_bytes, void* stream);
+
+/* The same training pass with activation recomputation, as the reference's get_gptj(gradient_checkpointing=True)
+ * (language_model.py:27-37): the workspace keeps each block's input only, and the backward reruns a block's forward
+ * (the same kernels in the same order, so bit-identical to what the stored path keeps) right before that block's
+ * backward. Loss, logits, dx and the weight gradients equal the stored path's bit for bit; the 1-D gradients (biases,
+ * LayerNorm parameters, adapter scale) are fp32 sums combined with atomics, whose last bits vary from run to run on
+ * either path. The price is one more forward of the blocks. At GPT-J-6B with MLP adapters, B = 8, S = 2048, the workspace is 13.6 GiB instead of 78.6 GiB.
+ * A recompute workspace pairs only with the recompute entry points: its layout differs from the stored one, and nothing
+ * in it records which forward filled it. Arguments are those of mb200_gptj_sched_forward / _backward_range. */
+size_t mb200_gptj_sched_recompute_workspace_bytes(const mb200_gptj_model_ex* m, int32_t B, int32_t S);
+int mb200_gptj_sched_forward_recompute(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels, void* logits,
+                                       int64_t ldv, float* loss, int32_t B, int32_t S, void* ws, size_t ws_bytes,
+                                       void* stream);
+int mb200_gptj_sched_backward_range_recompute(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t layer_hi,
+                                              int32_t layer_lo, int32_t accumulate, int32_t B, int32_t S, void* ws,
+                                              size_t ws_bytes, void* stream);
 /* Inference pass (no saved activations) — use_cache=True of magma/sampling.py:81-90: kcache / vcache bf16
  * [n_layer][B][H][S_kv_max][hd] or NULL; the K / V of this call are written at positions [pos0, pos0 + S) and attention
  * runs over [0, pos0 + S) (prefill S > 1 through mb200_attn_fwd_flash, decode S == 1 through mb200_attn_decode).

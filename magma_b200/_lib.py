@@ -169,6 +169,7 @@ def _setup_signatures(L):
     L.mb200_vit_train_workspace_bytes.restype = ctypes.c_size_t
     L.mb200_gptj_sched_workspace_bytes.restype = ctypes.c_size_t
     L.mb200_gptj_sched_infer_workspace_bytes.restype = ctypes.c_size_t
+    L.mb200_gptj_sched_recompute_workspace_bytes.restype = ctypes.c_size_t
     L.mb200_launch_count.restype = ctypes.c_longlong
 
 
@@ -190,5 +191,6 @@ EXPORTED_SYMBOLS = [
     "mb200_kv_append", "mb200_gptj_sched_infer_workspace_bytes", "mb200_gptj_sched_infer",
     "mb200_gptj_sched_backward_range", "mb200_bn_finalize_fwd", "mb200_bn_bwd_coeffs",
     "mb200_gptj_sched_decode_step", "mb200_decode_embed", "mb200_decode_advance", "mb200_rope_table_dev",
-    "mb200_attn_decode_dev",
+    "mb200_attn_decode_dev", "mb200_gptj_sched_recompute_workspace_bytes", "mb200_gptj_sched_forward_recompute",
+    "mb200_gptj_sched_backward_range_recompute",
 ]

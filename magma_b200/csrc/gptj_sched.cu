@@ -1,5 +1,6 @@
-// magma_b200 — GPT-J + adapters: THE language-model runtime (training forward with saved activations + backward,
-// full-sequence inference, KV-cache prefill and decode steps), host-only.
+// magma_b200 — GPT-J + adapters: THE language-model runtime (training forward with saved activations + backward, or
+// with only each block's input saved and the block recomputed in the backward; full-sequence inference, KV-cache
+// prefill and decode steps), host-only.
 //
 // One C call per pass instead of ~1000 Python-level op calls: this file carves the workspace and issues the kernels of a
 // pass on one stream. It schedules every adapter form of the reference — plain bottleneck in "normal" or "parallel"
@@ -212,7 +213,9 @@ void carve_adapter(Carver& c, AdapterActs& a, const mb200_adapter_ex& ad, int ki
   if (has_scale(ad)) a.u = c.take<bf16s>(M * d);
 }
 
-int make_plan(Plan& P, const mb200_gptj_model_ex* m, int B, int S, void* ws) {
+// recompute: every layer keeps only x_in; its other activations live in one scratch shared by all layers, which
+// the backward refills for each layer by rerunning that layer's forward (layer_fwd) from x_in
+int make_plan(Plan& P, const mb200_gptj_model_ex* m, int B, int S, void* ws, bool recompute = false) {
   MBS_REQUIRE(m && m->layers && m->n_layer > 0 && m->n_layer <= 64, MB200_E_SHAPE, "gptj_sched: n_layer out of range");
   MBS_REQUIRE(B > 0 && S > 0 && m->n_head > 0 && m->d % m->n_head == 0 && m->d % 8 == 0 && m->d_ff % 8 == 0,
               MB200_E_SHAPE, "gptj_sched: bad d / n_head / d_ff");
@@ -240,9 +243,24 @@ int make_plan(Plan& P, const mb200_gptj_model_ex* m, int B, int S, void* ws) {
   P.ldv = (long long)align_up(m->vocab, 64);
   const size_t M = P.M, d = P.d, dff = P.dff;
   const size_t nP = (size_t)B * P.H * S * P.ldP;
+  // the shared scratch of the recompute plan holds what any layer's adapters keep
+  mb200_adapter_ex um = m->layers[0].mlp_ad, ua = m->layers[0].attn_ad;
+  for (int l = 1; recompute && l < m->n_layer; ++l) {
+    const mb200_gptj_layer_ex& L = m->layers[l];
+    if (has_ln(L.mlp_ad)) um.ln_g = L.mlp_ad.ln_g;
+    if (has_scale(L.mlp_ad)) um.scale = L.mlp_ad.scale;
+    if (has_ln(L.attn_ad)) ua.ln_g = L.attn_ad.ln_g;
+    if (has_scale(L.attn_ad)) ua.scale = L.attn_ad.scale;
+  }
   for (int l = 0; l < m->n_layer; ++l) {
     LayerActs& a = P.acts[l];
     a.x_in = c.take<bf16s>(M * d);
+    if (recompute && l > 0) {
+      bf16s* x_in = a.x_in;
+      a = P.acts[0];
+      a.x_in = x_in;
+      continue;
+    }
     a.h = c.take<bf16s>(M * d);
     a.mean = c.take<float>(M);
     a.rstd = c.take<float>(M);
@@ -252,8 +270,9 @@ int make_plan(Plan& P, const mb200_gptj_model_ex* m, int B, int S, void* ws) {
     a.pre = c.take<bf16s>(M * dff);
     a.mlp_out = c.take<bf16s>(M * d);
     a.a_out = c.take<bf16s>(M * d);
-    carve_adapter(c, a.am, m->layers[l].mlp_ad, m->mlp_adapter, M, d, m->mlp_adapter_r, m->adapter_act);
-    carve_adapter(c, a.aa, m->layers[l].attn_ad, m->attn_adapter, M, d, m->attn_adapter_r, m->adapter_act);
+    carve_adapter(c, a.am, recompute ? um : m->layers[l].mlp_ad, m->mlp_adapter, M, d, m->mlp_adapter_r, m->adapter_act);
+    carve_adapter(c, a.aa, recompute ? ua : m->layers[l].attn_ad, m->attn_adapter, M, d, m->attn_adapter_r,
+                  m->adapter_act);
   }
   P.scores = c.take<float>(nP);
   P.hact = c.take<bf16s>(M * dff);
@@ -347,87 +366,93 @@ int adapter_bwd(void* st, const mb200_adapter_ex& ad, const AdapterActs& a, cons
   return mb200_layernorm_bwd(P.dzn, d, z, d, ad.ln_g, a.mean, a.rstd, res, d, dz_out, d, M, d, st);
 }
 
-int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels, bf16s* logits, long long ldv,
-            float* loss, int B, int S, void* ws, size_t ws_bytes, void* st) {
-  Plan P;
-  MBS_TRY(make_plan(P, m, B, S, ws));
-  MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_forward: workspace too small (%zu < %zu)",
-              ws_bytes, P.bytes);
-  const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd;
+// one block of the training forward: from P.acts[l].x_in to xout, keeping the activations the backward reads in
+// P.acts[l]. The forward pass and the recompute backward both issue it, so a recomputed layer is the stored one bit for bit.
+int layer_fwd(const mb200_gptj_model_ex* m, Plan& P, int l, bf16s* xout, void* st) {
+  const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd, B = P.B, S = P.S;
   const float scale = 1.0f / sqrtf((float)hd);
   const long long qb0 = hd, qb1 = (long long)S * 3 * d;
   const long long pb0 = (long long)S * P.ldP, pb1 = (long long)H * S * P.ldP;
+  const mb200_gptj_layer_ex& L = m->layers[l];
+  LayerActs& a = P.acts[l];
+  const bf16s* xin = a.x_in;
+  MBS_TRY(mb200_layernorm_fwd(xin, d, L.ln1_g, L.ln1_b, a.h, d, a.mean, a.rstd, M, d, m->ln_eps, st));
+  {  // fused q/k/v projection, rotary embedding applied to the q and k column ranges in the epilogue
+    Epi e;
+    e.rope_tab = P.rope_tab;
+    e.rope_mode = 1;
+    e.rope_S = S;
+    e.rope_hd = hd;
+    e.rope_rot = m->rotary_dim;
+    e.rope_ncols = 2 * d;
+    MBS_TRY(gemm(st, M, 3 * d, d, mat(a.h, d), wmat(L.w_qkv, d), a.qkv, 3 * d, 0, e));
+  }
+  if (tile_ok(S, hd)) {  // whole sequence in one tile: fused QK^T / softmax / PV, one CTA per (batch, head)
+    MBS_TRY(mb200_attn_fwd_tile(a.qkv, 3 * d, a.P, P.ldP, a.attn_o, d, B, S, H, hd, st));
+  } else if (flash_ok(hd)) {  // any S: fused multi-tile forward; P is written for the materialised backward
+    MBS_TRY(mb200_attn_fwd_flash(a.qkv, 3 * d, qb0, qb1, a.qkv + d, 3 * d, qb0, qb1, a.qkv + 2 * d, 3 * d, qb0, qb1,
+                                 a.attn_o, d, a.P, P.ldP, nullptr, B, S, S, H, hd, 1, st));
+  } else {
+    // scores = Q K^T (fp32), P = softmax(scores / sqrt(hd) + causal mask), O = P V
+    MBS_TRY(gemm(st, S, S, hd, mat(a.qkv, 3 * d, 0, qb0, qb1), mat(a.qkv + d, 3 * d, 0, qb0, qb1), P.scores, P.ldP, 1,
+                 Epi(), H, B, pb0, pb1));
+    MBS_TRY(mb200_softmax_fwd(P.scores, P.ldP, pb0, a.P, P.ldP, pb0, B * H, S, S, scale, 1, 0, st));
+    MBS_TRY(gemm(st, S, hd, S, mat(a.P, P.ldP, 0, pb0, pb1), mat(a.qkv + 2 * d, 3 * d, 1, qb0, qb1), a.attn_o, d, 0,
+                 Epi(), H, B, hd, (long long)S * d));
+  }
+  // out_proj; ax = attention branch + residual x
+  if (m->attn_adapter == MB200_ADAPTER_NONE) {
+    Epi e;
+    e.res1 = xin;
+    e.ld_res = d;
+    MBS_TRY(gemm(st, M, d, d, mat(a.attn_o, d), wmat(L.w_out, d), P.ax, d, 0, e));
+  } else if (m->attn_adapter == MB200_ADAPTER_NORMAL) {  // AdapterWrapper: A(attn_out) + attn_out
+    MBS_TRY(gemm(st, M, d, d, mat(a.attn_o, d), wmat(L.w_out, d), a.a_out, d, 0));
+    MBS_TRY(adapter_fwd(st, L.attn_ad, a.aa, M, d, m->attn_adapter_r, m->ln_eps, a.a_out, P.ax, a.a_out, xin, m->adapter_act));
+  } else {  // ParallelAdapterWrapper: attn(h) + s * A(h)
+    Epi e;
+    e.res1 = xin;
+    e.ld_res = d;
+    MBS_TRY(gemm(st, M, d, d, mat(a.attn_o, d), wmat(L.w_out, d), a.a_out, d, 0, e));
+    MBS_TRY(adapter_fwd(st, L.attn_ad, a.aa, M, d, m->attn_adapter_r, m->ln_eps, a.h, P.ax, a.a_out, nullptr, m->adapter_act));
+  }
+  {  // fc_in + bias + gelu_new, pre-activation kept
+    Epi e;
+    e.bias = L.b_fc_in;
+    e.act = MB200_ACT_GELU_NEW;
+    e.aux_out = a.pre;
+    MBS_TRY(gemm(st, M, dff, d, mat(a.h, d), wmat(L.w_fc_in, d), P.hact, dff, 0, e));
+  }
+  Epi eo;
+  eo.bias = L.b_fc_out;
+  if (m->mlp_adapter == MB200_ADAPTER_NONE) {
+    eo.res1 = P.ax;
+    eo.ld_res = d;
+    MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), xout, d, 0, eo));
+  } else if (m->mlp_adapter == MB200_ADAPTER_NORMAL) {  // Sequential(mlp, Adapter): A(mlp(h)) + mlp(h)
+    MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
+    MBS_TRY(adapter_fwd(st, L.mlp_ad, a.am, M, d, m->mlp_adapter_r, m->ln_eps, a.mlp_out, xout, a.mlp_out, P.ax, m->adapter_act));
+  } else {  // ParallelAdapter: mlp(h) + s * A(h)
+    eo.res1 = P.ax;
+    eo.ld_res = d;
+    MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
+    MBS_TRY(adapter_fwd(st, L.mlp_ad, a.am, M, d, m->mlp_adapter_r, m->ln_eps, a.h, xout, a.mlp_out, nullptr, m->adapter_act));
+  }
+  return 0;
+}
+
+int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels, bf16s* logits, long long ldv,
+            float* loss, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute) {
+  Plan P;
+  MBS_TRY(make_plan(P, m, B, S, ws, recompute));
+  MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_forward: workspace too small (%zu < %zu)",
+              ws_bytes, P.bytes);
+  const int M = P.M, d = P.d;
   ScratchScope scratch(P.gemm_ws, P.gemm_ws_bytes);
   MBS_TRY(mb200_rope_table(P.rope_tab, S, m->rotary_dim, 0, st));
   MBS_TRY(rt_copy(P.acts[0].x_in, x, (size_t)M * d * sizeof(bf16s), st));
-  for (int l = 0; l < m->n_layer; ++l) {
-    const mb200_gptj_layer_ex& L = m->layers[l];
-    LayerActs& a = P.acts[l];
-    const bf16s* xin = a.x_in;
-    bf16s* xout = l + 1 < m->n_layer ? P.acts[l + 1].x_in : P.x_final;
-    MBS_TRY(mb200_layernorm_fwd(xin, d, L.ln1_g, L.ln1_b, a.h, d, a.mean, a.rstd, M, d, m->ln_eps, st));
-    {  // fused q/k/v projection, rotary embedding applied to the q and k column ranges in the epilogue
-      Epi e;
-      e.rope_tab = P.rope_tab;
-      e.rope_mode = 1;
-      e.rope_S = S;
-      e.rope_hd = hd;
-      e.rope_rot = m->rotary_dim;
-      e.rope_ncols = 2 * d;
-      MBS_TRY(gemm(st, M, 3 * d, d, mat(a.h, d), wmat(L.w_qkv, d), a.qkv, 3 * d, 0, e));
-    }
-    if (tile_ok(S, hd)) {  // whole sequence in one tile: fused QK^T / softmax / PV, one CTA per (batch, head)
-      MBS_TRY(mb200_attn_fwd_tile(a.qkv, 3 * d, a.P, P.ldP, a.attn_o, d, B, S, H, hd, st));
-    } else if (flash_ok(hd)) {  // any S: fused multi-tile forward; P is written for the materialised backward
-      MBS_TRY(mb200_attn_fwd_flash(a.qkv, 3 * d, qb0, qb1, a.qkv + d, 3 * d, qb0, qb1, a.qkv + 2 * d, 3 * d, qb0, qb1,
-                                   a.attn_o, d, a.P, P.ldP, nullptr, B, S, S, H, hd, 1, st));
-    } else {
-      // scores = Q K^T (fp32), P = softmax(scores / sqrt(hd) + causal mask), O = P V
-      MBS_TRY(gemm(st, S, S, hd, mat(a.qkv, 3 * d, 0, qb0, qb1), mat(a.qkv + d, 3 * d, 0, qb0, qb1), P.scores, P.ldP, 1,
-                   Epi(), H, B, pb0, pb1));
-      MBS_TRY(mb200_softmax_fwd(P.scores, P.ldP, pb0, a.P, P.ldP, pb0, B * H, S, S, scale, 1, 0, st));
-      MBS_TRY(gemm(st, S, hd, S, mat(a.P, P.ldP, 0, pb0, pb1), mat(a.qkv + 2 * d, 3 * d, 1, qb0, qb1), a.attn_o, d, 0,
-                   Epi(), H, B, hd, (long long)S * d));
-    }
-    // out_proj; ax = attention branch + residual x
-    if (m->attn_adapter == MB200_ADAPTER_NONE) {
-      Epi e;
-      e.res1 = xin;
-      e.ld_res = d;
-      MBS_TRY(gemm(st, M, d, d, mat(a.attn_o, d), wmat(L.w_out, d), P.ax, d, 0, e));
-    } else if (m->attn_adapter == MB200_ADAPTER_NORMAL) {  // AdapterWrapper: A(attn_out) + attn_out
-      MBS_TRY(gemm(st, M, d, d, mat(a.attn_o, d), wmat(L.w_out, d), a.a_out, d, 0));
-      MBS_TRY(adapter_fwd(st, L.attn_ad, a.aa, M, d, m->attn_adapter_r, m->ln_eps, a.a_out, P.ax, a.a_out, xin, m->adapter_act));
-    } else {  // ParallelAdapterWrapper: attn(h) + s * A(h)
-      Epi e;
-      e.res1 = xin;
-      e.ld_res = d;
-      MBS_TRY(gemm(st, M, d, d, mat(a.attn_o, d), wmat(L.w_out, d), a.a_out, d, 0, e));
-      MBS_TRY(adapter_fwd(st, L.attn_ad, a.aa, M, d, m->attn_adapter_r, m->ln_eps, a.h, P.ax, a.a_out, nullptr, m->adapter_act));
-    }
-    {  // fc_in + bias + gelu_new, pre-activation kept
-      Epi e;
-      e.bias = L.b_fc_in;
-      e.act = MB200_ACT_GELU_NEW;
-      e.aux_out = a.pre;
-      MBS_TRY(gemm(st, M, dff, d, mat(a.h, d), wmat(L.w_fc_in, d), P.hact, dff, 0, e));
-    }
-    Epi eo;
-    eo.bias = L.b_fc_out;
-    if (m->mlp_adapter == MB200_ADAPTER_NONE) {
-      eo.res1 = P.ax;
-      eo.ld_res = d;
-      MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), xout, d, 0, eo));
-    } else if (m->mlp_adapter == MB200_ADAPTER_NORMAL) {  // Sequential(mlp, Adapter): A(mlp(h)) + mlp(h)
-      MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
-      MBS_TRY(adapter_fwd(st, L.mlp_ad, a.am, M, d, m->mlp_adapter_r, m->ln_eps, a.mlp_out, xout, a.mlp_out, P.ax, m->adapter_act));
-    } else {  // ParallelAdapter: mlp(h) + s * A(h)
-      eo.res1 = P.ax;
-      eo.ld_res = d;
-      MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
-      MBS_TRY(adapter_fwd(st, L.mlp_ad, a.am, M, d, m->mlp_adapter_r, m->ln_eps, a.h, xout, a.mlp_out, nullptr, m->adapter_act));
-    }
-  }
+  for (int l = 0; l < m->n_layer; ++l)
+    MBS_TRY(layer_fwd(m, P, l, l + 1 < m->n_layer ? P.acts[l + 1].x_in : P.x_final, st));
   // ln_f + LM head (+ shifted cross-entropy; the logits' gradient is written now, scaled in backward)
   MBS_TRY(mb200_layernorm_fwd(P.x_final, d, m->lnf_g, m->lnf_b, P.xf_ln, d, P.lnf_mean, P.lnf_rstd, M, d, m->ln_eps, st));
   bf16s* lg = logits ? logits : P.dlogits;
@@ -449,10 +474,13 @@ int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels,
 // Layers are processed from layer_hi-1 down to layer_lo; the LM-head / CE backward runs when layer_hi == n_layer. The
 // residual-stream gradient lives in the workspace between calls, so a caller can split the range and exchange the
 // gradients of finished layers while the rest runs (B200Engine.backward).
+// recompute: each layer's activations are rebuilt from its x_in first. The rebuilt block output goes to P.dh, which is
+// dead at that point, so x_in, x_final and everything else the forward left stay as they were and a second backward
+// gives the same result.
 int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int layer_hi, int layer_lo, int acc, int B, int S,
-             void* ws, size_t ws_bytes, void* st) {
+             void* ws, size_t ws_bytes, void* st, bool recompute) {
   Plan P;
-  MBS_TRY(make_plan(P, m, B, S, ws));
+  MBS_TRY(make_plan(P, m, B, S, ws, recompute));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_backward: workspace too small");
   MBS_REQUIRE(0 <= layer_lo && layer_lo <= layer_hi && layer_hi <= m->n_layer, MB200_E_ARG,
               "gptj_sched_backward: bad layer range [%d,%d)", layer_lo, layer_hi);
@@ -471,6 +499,7 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int laye
                                 M, d, st));
   }
   for (int l = layer_hi - 1; l >= layer_lo; --l) {
+    if (recompute) MBS_TRY(layer_fwd(m, P, l, P.dh, st));
     const mb200_gptj_layer_ex& L = m->layers[l];
     LayerActs& a = P.acts[l];
     const bf16s* g = gb[(l + 1) & 1];
@@ -757,14 +786,16 @@ extern "C" int mb200_gptj_sched_forward(const mb200_gptj_model_ex* m, const void
                                         void* stream) {
   int rc = mb200::rt_check_arch();
   if (rc) return rc;
-  return mb200::forward(m, (const mb200::bf16s*)x, labels, (mb200::bf16s*)logits, ldv, loss, B, S, ws, ws_bytes, stream);
+  return mb200::forward(m, (const mb200::bf16s*)x, labels, (mb200::bf16s*)logits, ldv, loss, B, S, ws, ws_bytes, stream,
+                        false);
 }
 
 extern "C" int mb200_gptj_sched_backward(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t accumulate,
                                          int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream) {
   int rc = mb200::rt_check_arch();
   if (rc) return rc;
-  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, m ? m->n_layer : 0, 0, accumulate, B, S, ws, ws_bytes, stream);
+  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, m ? m->n_layer : 0, 0, accumulate, B, S, ws, ws_bytes, stream,
+                         false);
 }
 
 extern "C" int mb200_gptj_sched_backward_range(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t layer_hi,
@@ -772,5 +803,30 @@ extern "C" int mb200_gptj_sched_backward_range(const mb200_gptj_model_ex* m, voi
                                                size_t ws_bytes, void* stream) {
   int rc = mb200::rt_check_arch();
   if (rc) return rc;
-  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes, stream);
+  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes, stream,
+                         false);
+}
+
+extern "C" size_t mb200_gptj_sched_recompute_workspace_bytes(const mb200_gptj_model_ex* m, int32_t B, int32_t S) {
+  mb200::Plan P;
+  if (mb200::make_plan(P, m, B, S, nullptr, true)) return 0;
+  return P.bytes;
+}
+
+extern "C" int mb200_gptj_sched_forward_recompute(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels,
+                                                  void* logits, int64_t ldv, float* loss, int32_t B, int32_t S, void* ws,
+                                                  size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::forward(m, (const mb200::bf16s*)x, labels, (mb200::bf16s*)logits, ldv, loss, B, S, ws, ws_bytes, stream,
+                        true);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_recompute(const mb200_gptj_model_ex* m, void* dx, float loss_scale,
+                                                         int32_t layer_hi, int32_t layer_lo, int32_t accumulate,
+                                                         int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes, stream,
+                         true);
 }

@@ -12,6 +12,7 @@ All frozen weights are bf16 tensors on the GPU; parameter names follow HF GPT-J 
 28-block forward and backward run inside libmagma_b200.so (csrc/gptj_sched.cu); this file only owns tensors and plumbing.
 """
 import ctypes
+import math
 import os
 from dataclasses import dataclass
 
@@ -40,7 +41,7 @@ class GPTJConfig:
     layer_norm_epsilon: float = 1e-5
     intermediate_size: int = None
     pad_token_id: int = None
-    gradient_checkpointing: bool = False  # accepted for API parity; 180 GB HBM holds all activations
+    gradient_checkpointing: bool = False  # accepted for API parity; the runtime decides (_use_recompute)
     use_cache: bool = True
 
     def __post_init__(self):
@@ -183,6 +184,22 @@ def _split_attn(attn):
     raise MB200Error(f"unsupported attention wrapper {type(attn).__name__}")
 
 
+def _use_recompute(stored_bytes, other_bytes, free_bytes):
+    """Whether a training pass recomputes block activations in its backward: yes when the stored-activation workspace
+    plus the pass's other allocations does not fit in the memory the process can still allocate. Both paths run the
+    same kernels on the same block inputs (the results agree bit for bit apart from the run-to-run last-bit variation
+    of the atomically reduced 1-D gradients), so this only trades time (one more forward of the blocks) for memory."""
+    return stored_bytes + other_bytes > free_bytes
+
+
+def _free_bytes(device):
+    """Memory a new allocation on `device` can use: free on the device plus what the caching allocator holds unused."""
+    if device.type != "cuda":
+        return math.inf  # the CPU emulation the host-side tests run on has no device memory to run out of
+    free, _ = torch.cuda.mem_get_info(device)
+    return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+
+
 class _LMTrainFn(torch.autograd.Function):
     """loss = LM(inputs_embeds, labels) with the backward pass of the C++ runtime (LM frozen: dgrad through every
     GEMM, wgrad only for adapters, written straight into the parameter arena's fp32 gradient buffer)."""
@@ -222,6 +239,7 @@ class B200GPTJForCausalLM(nn.Module):
         self._cmodel_ex_cache = None
         self._ws = {}
         self._generation = 0
+        self._generation_recompute = False  # whether the training forward of _generation recomputes in its backward
         self._loss_scale_hint = None
         self._bwd_chunks = None       # list of (layer_hi, layer_lo); None = single chunk
         self._after_chunk = None      # callback(layer_hi, layer_lo) for gradient all-reduce overlap
@@ -337,14 +355,20 @@ class B200GPTJForCausalLM(nn.Module):
         return self._cmodel_ex_cache
 
     def _workspace_ex(self, B, S):
+        """(training workspace for [B, S], whether its pass recomputes block activations). The path is chosen once,
+        when the workspace is allocated, and kept with it, so a run does not switch paths between steps."""
         key = ("ex", B, S)
         if key not in self._ws:
-            nbytes = lib().mb200_gptj_sched_workspace_bytes(ctypes.byref(self._cmodel_ex()[0]), B, S)
-            if nbytes == 0:
+            m = ctypes.byref(self._cmodel_ex()[0])
+            stored = lib().mb200_gptj_sched_workspace_bytes(m, B, S)
+            if stored == 0:
                 raise MB200Error(lib().mb200_last_error().decode())
             for k in [k for k in self._ws if isinstance(k, tuple) and k[0] == "ex"]:
                 del self._ws[k]
-            self._ws[key] = torch.empty(nbytes, dtype=torch.uint8, device=self._device)
+            other = B * S * (self.ldv + self.config.hidden_size) * 2  # the pass's bf16 logits and dx
+            recompute = _use_recompute(stored, other, _free_bytes(self._device))
+            nbytes = lib().mb200_gptj_sched_recompute_workspace_bytes(m, B, S) if recompute else stored
+            self._ws[key] = (torch.empty(nbytes, dtype=torch.uint8, device=self._device), recompute)
         return self._ws[key]
 
     def invalidate(self):
@@ -374,15 +398,16 @@ class B200GPTJForCausalLM(nn.Module):
         if labels is not None or training:
             if cache is not None or last_only or want_hidden:
                 raise MB200Error("a loss together with a KV cache / last-position logits / hidden states is not supported")
-            ws = self._workspace_ex(B, S)
+            ws, recompute = self._workspace_ex(B, S)
             logits = torch.empty(B * S, ldv, dtype=torch.bfloat16, device=x.device) if want_logits else None
             loss = torch.zeros(1, dtype=torch.float32, device=x.device) if labels is not None else None
             if labels is not None:
                 labels = labels.to(device=x.device, dtype=torch.int64).contiguous()
             self._generation += 1  # this pass records its activations in the workspace
-            check(lib().mb200_gptj_sched_forward(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits),
-                                                 ctypes.c_int64(ldv), ops._ptr(loss), B, S, ops._ptr(ws),
-                                                 ctypes.c_size_t(ws.numel()), ops._stream()))
+            self._generation_recompute = recompute
+            fwd = lib().mb200_gptj_sched_forward_recompute if recompute else lib().mb200_gptj_sched_forward
+            check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ctypes.c_int64(ldv),
+                      ops._ptr(loss), B, S, ops._ptr(ws), ctypes.c_size_t(ws.numel()), ops._stream()))
             self._last_hidden = None
             lg = logits.view(B, S, ldv)[..., :V] if logits is not None else None
             return (loss.squeeze(0) if loss is not None else None), lg
@@ -414,13 +439,15 @@ class B200GPTJForCausalLM(nn.Module):
         B, S, d = shape
         arena = self._arena
         dx = torch.empty(B, S, d, dtype=torch.bfloat16, device=self._device)
-        ws = self._workspace_ex(B, S)
+        ws, recompute = self._workspace_ex(B, S)
+        if recompute != self._generation_recompute:
+            raise MB200Error("backward called on a workspace of the other activation path (stored / recomputed) than "
+                             "its forward's")
+        bwd = lib().mb200_gptj_sched_backward_range_recompute if recompute else lib().mb200_gptj_sched_backward_range
         accumulate = int(arena.grads_live()) if arena is not None else 0
         for hi, lo in (self._bwd_chunks or [(len(self.transformer.h), 0)]):
-            check(lib().mb200_gptj_sched_backward_range(ctypes.byref(self._cmodel_ex()[0]),
-                                                        ops._ptr(dx) if lo == 0 else None, ctypes.c_float(loss_scale),
-                                                        hi, lo, accumulate, B, S, ops._ptr(ws),
-                                                        ctypes.c_size_t(ws.numel()), ops._stream()))
+            check(bwd(ctypes.byref(self._cmodel_ex()[0]), ops._ptr(dx) if lo == 0 else None, ctypes.c_float(loss_scale),
+                      hi, lo, accumulate, B, S, ops._ptr(ws), ctypes.c_size_t(ws.numel()), ops._stream()))
             if self._after_chunk is not None:
                 self._after_chunk(hi, lo)
         if arena is not None and self._own_arena:
@@ -494,7 +521,9 @@ def gptj_config():
 
 def get_gptj(gradient_checkpointing: bool = True, from_pretrained=False, config: GPTJConfig = None, device=None):
     """magma/language_model.py:27-45 — returns the (uninitialised-weights) LM. `gradient_checkpointing` is accepted
-    for signature parity and ignored: the runtime stores activations (3.4 GB at B=8,S=128) instead of recomputing."""
+    for signature parity and ignored: the runtime stores every block's activations when they fit in free device memory
+    (3.2 GiB at B=8, S=128) and otherwise keeps only each block's input and recomputes the block in the backward
+    (13.6 GiB instead of 78.6 GiB at B=8, S=2048). Both compute the same results."""
     if from_pretrained:
         raise NotImplementedError("GPTJ pretrained not implemented")  # same behaviour as the reference (:41-42)
     cfg = config or gptj_config()
