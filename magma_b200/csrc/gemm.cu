@@ -21,10 +21,20 @@
 
 namespace mb200 {
 
-template <int BN, bool A_MN, bool B_MN>
+// Tensor maps of the epilogue inputs staged by TMA (GemmKernelParams::epi_in of them, in its order), each a K-major
+// [M, N] operand with box (64 columns, BM rows). Kernels without staged inputs take an empty parameter and carry none
+// of the staging code: it would cost them instruction fetch in the epilogue loop.
+template <bool kOn>
+struct EpiMaps {
+  CUtensorMap m[3];
+};
+template <>
+struct EpiMaps<false> {};
+
+template <int BN, bool A_MN, bool B_MN, bool EPI_TMA>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ GemmKernelParams p) {
+                  const __grid_constant__ EpiMaps<EPI_TMA> tmE, const __grid_constant__ GemmKernelParams p) {
   using C_ = Cfg<BN>;
   constexpr int kStages = C_::kStages;
 
@@ -36,6 +46,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   float* epi_stage = reinterpret_cast<float*>(smem + kStages * C_::kStageBytes);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * C_::kStageBytes + kEpiBytes);
   uint64_t* empty_bar = full_bar + kStages;
+  const EpiRing ring{smem_a, smem_b, full_bar, empty_bar};
 
   const int wg = threadIdx.x >> 7;
   const int num_kb = (p.K + BK - 1) / BK;
@@ -45,6 +56,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if constexpr (EPI_TMA) {
+#pragma unroll 1
+      for (int i = 0; i < p.epi_in; ++i) tma_prefetch_desc(&tmE.m[i]);
+    }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
@@ -96,6 +111,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             phase ^= 1;
           }
         }
+        if constexpr (EPI_TMA) epi_queue_inputs<BN>(p, tmE.m, ring, stage, phase, m_blk * BM, n_blk * BN, z0, z1);
       }
     }
   } else {
@@ -147,7 +163,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>();
       if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
       const long long boff = (long long)z0 * p.c_bs0 + (long long)z1 * p.c_bs1;
-      epi_tile<BN>(p, acc, epi_stage + cw * 64 * kEpiCols, 1 + cw, boff, m_blk * BM + cw * 64, n_blk * BN, ks);
+      epi_tile<BN, EPI_TMA>(p, acc, epi_stage + cw * 64 * kEpiCols, 1 + cw, boff, m_blk * BM + cw * 64, n_blk * BN, ks, ring,
+                   stage, phase);
     }
   }
 }
@@ -171,7 +188,10 @@ __global__ void splitk_finalize_kernel(const GemmKernelParams p) {
       v[2] += w4.z;
       v[3] += w4.w;
     }
-    epi_store4(p, 0, row, col, v);
+    EpiIn in;
+    if (p.bias) ld_bf16x4(p.bias + col, min(4, p.N - col), in.bias);
+    epi_load_inputs(p, 0, row, col, in);
+    epi_store4(p, 0, row, col, v, in);
   }
 }
 
@@ -240,10 +260,10 @@ int make_operand_map(CUtensorMap* out, const mb200_operand& op, int rows, int K,
   return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmKernelParams& kp,
-                       cudaStream_t stream) {
-  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
+template <int BN, bool A_MN, bool B_MN, bool EPI_TMA>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiMaps<true>& tmE,
+                       const GemmKernelParams& kp, cudaStream_t stream) {
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI_TMA>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes));
@@ -256,29 +276,75 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
     const double flops = 2.0 * kp.M * (double)kp.N * kp.K * nb;
     const double bytes = nb * (2.0 * ((double)kp.M * kp.K + (double)kp.N * kp.K) + (kp.c_f32 ? 4.0 : 2.0) * kp.M * kp.N);
     GemmProfScope prof(stream, flops, bytes);
-    MB_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), Cfg<BN>::kSmemBytes, stream, tmA, tmB, kp));
+    if constexpr (EPI_TMA)
+      MB_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), Cfg<BN>::kSmemBytes, stream, tmA, tmB, tmE, kp));
+    else
+      MB_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), Cfg<BN>::kSmemBytes, stream, tmA, tmB, EpiMaps<false>{}, kp));
   }
   count_launch();
   MB_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <int BN>
+template <int BN, bool EPI_TMA>
 static int dispatch_major(bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                          const GemmKernelParams& kp, cudaStream_t s) {
-  if (!a_mn && !b_mn) return launch_gemm<BN, false, false>(tmA, tmB, kp, s);
-  if (!a_mn && b_mn) return launch_gemm<BN, false, true>(tmA, tmB, kp, s);
-  if (a_mn && !b_mn) return launch_gemm<BN, true, false>(tmA, tmB, kp, s);
-  return launch_gemm<BN, true, true>(tmA, tmB, kp, s);
+                          const EpiMaps<true>& tmE, const GemmKernelParams& kp, cudaStream_t s) {
+  if (!a_mn && !b_mn) return launch_gemm<BN, false, false, EPI_TMA>(tmA, tmB, tmE, kp, s);
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true, EPI_TMA>(tmA, tmB, tmE, kp, s);
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false, EPI_TMA>(tmA, tmB, tmE, kp, s);
+  return launch_gemm<BN, true, true, EPI_TMA>(tmA, tmB, tmE, kp, s);
 }
 
 static int dispatch_bn(int bn, bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                       const GemmKernelParams& kp, cudaStream_t s) {
+                       const EpiMaps<true>& tmE, const GemmKernelParams& kp, cudaStream_t s) {
+  const bool epi = kp.epi_in != 0;
   switch (bn) {
-    case 64: return dispatch_major<64>(a_mn, b_mn, tmA, tmB, kp, s);
-    case 128: return dispatch_major<128>(a_mn, b_mn, tmA, tmB, kp, s);
-    default: return dispatch_major<256>(a_mn, b_mn, tmA, tmB, kp, s);
+    case 64:
+      return epi ? dispatch_major<64, true>(a_mn, b_mn, tmA, tmB, tmE, kp, s)
+                 : dispatch_major<64, false>(a_mn, b_mn, tmA, tmB, tmE, kp, s);
+    case 128:
+      return epi ? dispatch_major<128, true>(a_mn, b_mn, tmA, tmB, tmE, kp, s)
+                 : dispatch_major<128, false>(a_mn, b_mn, tmA, tmB, tmE, kp, s);
+    default:
+      return epi ? dispatch_major<256, true>(a_mn, b_mn, tmA, tmB, tmE, kp, s)
+                 : dispatch_major<256, false>(a_mn, b_mn, tmA, tmB, tmE, kp, s);
   }
+}
+
+// Tensor maps for the epilogue's [M, N] inputs (aux_in when dact, res1, res2), fetched by the producer through the
+// operand ring. Used only when every input is TMA-addressable (16-byte base, row and batch strides multiples of 8
+// elements); otherwise kp->epi_in stays 0 and the epilogue reads all of them from global memory itself.
+static int make_epi_maps(EpiMaps<true>* maps, GemmKernelParams* kp, const mb200_gemm_args* a) {
+  const void* ptr[3];
+  long long ld[3];
+  int n = 0;
+  if (a->dact) {
+    ptr[n] = a->aux_in;
+    ld[n++] = a->ldc;
+  }
+  if (a->res1) {
+    ptr[n] = a->res1;
+    ld[n++] = a->ld_res;
+  }
+  if (a->res2) {
+    ptr[n] = a->res2;
+    ld[n++] = a->ld_res;
+  }
+  bool ok = (a->nb0 == 1 || a->c_bs0 % 8 == 0) && (a->nb1 == 1 || a->c_bs1 % 8 == 0);
+  for (int i = 0; i < n; ++i) ok = ok && (reinterpret_cast<uintptr_t>(ptr[i]) & 15) == 0 && ld[i] % 8 == 0;
+  if (n == 0 || !ok) return 0;
+  for (int i = 0; i < n; ++i) {
+    mb200_operand op;
+    memset(&op, 0, sizeof(op));
+    op.ptr = ptr[i];
+    op.ld = ld[i];
+    op.bs0 = a->c_bs0;
+    op.bs1 = a->c_bs1;
+    const int rc = make_operand_map(&maps->m[i], op, a->M, a->N, a->nb0, a->nb1, BM);
+    if (rc) return rc;
+  }
+  kp->epi_in = n;
+  return 0;
 }
 
 static int pick_bn(int M, int N, int batches) {
@@ -370,6 +436,8 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
   MB_REQUIRE(bn == 64 || bn == 128 || bn == 256, MB200_E_ARG, "gemm: force_bn must be 64, 128 or 256");
 
   CUtensorMap tmA, tmB;
+  EpiMaps<true> tmE;
+  memset(&tmE, 0, sizeof(tmE));
   // small-M problems (decode: M = batch <= 32) are planned for weight streaming (tile width + K split)
   const bool small_m = a->M <= 32 && a->A.mn_major == 0 && a->nb0 * a->nb1 == 1 && a->c_dtype == MB200_BF16;
   int plan_split = 1;
@@ -452,9 +520,9 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
       kp.kb_per_split = kb_per;
       kp.splitk_ws = reinterpret_cast<float*>(a->splitk_ws);
       kp.ld_ws = ld_ws;
-      GemmKernelParams kg = kp;  // the GEMM itself only writes partials (alpha applied)
+      GemmKernelParams kg = kp;  // the GEMM itself only writes partials (alpha applied); no epilogue inputs
       kg.epi_kind = EK_SPLITK;
-      rc = dispatch_bn(bn, amn, bmn, tmA, tmB, kg, stream);
+      rc = dispatch_bn(bn, amn, bmn, tmA, tmB, tmE, kg, stream);
       if (rc) return rc;
       const long long n4 = (long long)a->M * ((a->N + 3) / 4);
       const int fgrid = (int)((n4 + 255) / 256 > 2048 ? 2048 : (n4 + 255) / 256);
@@ -468,7 +536,9 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
   if (rc) return rc;
   kp.tiles_n = (a->N + bn - 1) / bn;
   kp.total_tiles = tiles_m * kp.tiles_n * a->nb0 * a->nb1;
-  return dispatch_bn(bn, amn, bmn, tmA, tmB, kp, stream);
+  rc = make_epi_maps(&tmE, &kp, a);
+  if (rc) return rc;
+  return dispatch_bn(bn, amn, bmn, tmA, tmB, tmE, kp, stream);
 }
 
 }  // namespace mb200

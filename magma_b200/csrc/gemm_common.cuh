@@ -11,6 +11,7 @@ static constexpr int WG_K = 16;       // wgmma K for 16-bit inputs
 static constexpr int kThreads = 384;  // warpgroup 0 = TMA producer, warpgroups 1, 2 = MMA + epilogue
 static constexpr int kEpiCols = 64;  // epilogue staging chunk: BM x 64 fp32, 64 rows per consumer warpgroup
 static constexpr int kEpiBytes = BM * kEpiCols * 4;
+static constexpr int kEpiBoxBytes = BM * kEpiCols * 2;  // one TMA box of an [M, N] epilogue input: BM x 64 bf16
 static constexpr int kSmemBudget = 192 * 1024;  // operand ring; + staging, alignment slack and barriers <= 227 KB
 
 template <int BN>
@@ -22,6 +23,12 @@ struct Cfg {
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
   static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
+  // Epilogue-input boxes one ring stage holds: the first fills the A slot, the others the B slot.
+  static constexpr int kEpiBoxesPerStage = 1 + kBBytes / kEpiBoxBytes;
+  static_assert(kABytes == kEpiBoxBytes && kEpiBoxesPerStage * kEpiBoxBytes <= kStageBytes, "epilogue box layout");
+  // A tile's three inputs fit in the ring at once, so the producer never waits on a slot the same tile's epilogue
+  // still has to release.
+  static_assert(3 * (BN / kEpiCols) <= kStages * kEpiBoxesPerStage, "epilogue inputs exceed the operand ring");
 };
 
 struct GemmKernelParams {
@@ -38,6 +45,9 @@ struct GemmKernelParams {
   const bf16* res1;
   const bf16* res2;
   long long ld_res;
+  // Number of [M, N] epilogue inputs (aux_in when dact, res1, res2, in that order) that the producer stages by TMA
+  // through the operand ring after each tile's last k-block; 0: the epilogue reads them from global memory.
+  int epi_in;
   // fused rotary embedding (rotate_every_two) on column pairs: applied when rope_mode != 0
   const float2* rope_tab;  // [rope_S][rope_rot/2] (cos, sin) of the position of row (row % rope_S)
   int rope_mode;           // +1 forward, -1 inverse (transpose rotation)
@@ -92,20 +102,44 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 
 enum { EK_GENERIC = 0, EK_SPLITK };
 
+// Epilogue inputs of one 4-column group: bias, aux_in, res1, res2. A field is filled only when its input is in use.
+struct EpiIn {
+  float bias[4], aux[4], res1[4], res2[4];
+};
+
+// aux_in / res1 / res2 of columns [col, col + 4) of one row, from global memory
+__device__ __forceinline__ void epi_load_inputs(const GemmKernelParams& p, long long boff, int row, int col,
+                                                EpiIn& in) {
+  const int n = min(4, p.N - col);
+  if (p.dact) ld_bf16x4(p.aux_in + boff + (long long)row * p.ldc + col, n, in.aux);
+  const long long roff = boff + (long long)row * p.ld_res + col;
+  if (p.res1) ld_bf16x4(p.res1 + roff, n, in.res1);
+  if (p.res2) ld_bf16x4(p.res2 + roff, n, in.res2);
+}
+
+// 4 bf16 of a TMA-staged epilogue box -> fp32 (8-byte aligned; columns past N were zero-filled by TMA)
+__device__ __forceinline__ void ld_smem_bf16x4(const uint8_t* src, float (&v)[4]) {
+  const uint2 u = *reinterpret_cast<const uint2*>(src);
+  const float2 a = bf16x2_to_f32(u.x), b = bf16x2_to_f32(u.y);
+  v[0] = a.x;
+  v[1] = a.y;
+  v[2] = b.x;
+  v[3] = b.y;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Fused epilogue of columns [col, col + 4) of one output row (col % 4 == 0, col < N, row < M); v holds alpha x the
-// accumulators (or the summed split-K partials). Applied in this order: bias, rotary, saved pre-activation (aux_out),
-// activation, activation derivative (aux_in), residuals, ReLU-post, store (bf16, fp32 or fp32 accumulate). rope_hd,
-// rope_rot and rope_ncols are multiples of 4, so both rotary pairs (col, col + 1), (col + 2, col + 3) of the group are
-// rotated or neither is. Every branch on p is uniform across the kernel.
+// accumulators (or the summed split-K partials), `in` the group's inputs. Applied in this order: bias, rotary, saved
+// pre-activation (aux_out), activation, activation derivative (aux_in), residuals, ReLU-post, store (bf16, fp32 or
+// fp32 accumulate). rope_hd, rope_rot and rope_ncols are multiples of 4, so both rotary pairs (col, col + 1),
+// (col + 2, col + 3) of the group are rotated or neither is. Every branch on p is uniform across the kernel.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long boff, int row, int col, float (&v)[4]) {
+__device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long boff, int row, int col, float (&v)[4],
+                                           const EpiIn& in) {
   const int n = min(4, p.N - col);
   if (p.bias) {
-    float b[4];
-    ld_bf16x4(p.bias + col, n, b);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) v[e] += b[e];
+    for (int e = 0; e < 4; ++e) v[e] += in.bias[e];
   }
   if (p.rope_mode != 0 && col < p.rope_ncols) {
     const int dim = col % p.rope_hd;
@@ -129,23 +163,17 @@ __device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long 
     else if (p.act == MB200_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
   }
   if (p.dact) {
-    float a[4];
-    ld_bf16x4(p.aux_in + coff, n, a);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) v[e] = p.dact == MB200_DACT_GELU_NEW ? v[e] * gelu_new_grad_f(a[e]) : (a[e] > 0.f ? v[e] : 0.f);
+    for (int e = 0; e < 4; ++e)
+      v[e] = p.dact == MB200_DACT_GELU_NEW ? v[e] * gelu_new_grad_f(in.aux[e]) : (in.aux[e] > 0.f ? v[e] : 0.f);
   }
-  const long long roff = boff + (long long)row * p.ld_res + col;
   if (p.res1) {
-    float r[4];
-    ld_bf16x4(p.res1 + roff, n, r);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) v[e] += r[e];
+    for (int e = 0; e < 4; ++e) v[e] += in.res1[e];
   }
   if (p.res2) {
-    float r[4];
-    ld_bf16x4(p.res2 + roff, n, r);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) v[e] += r[e];
+    for (int e = 0; e < 4; ++e) v[e] += in.res2[e];
   }
   if (p.act == MB200_ACT_RELU_POST) {
 #pragma unroll
@@ -182,16 +210,65 @@ __device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long 
 // half-warp's 8-byte fragment writes (4 rows x 2 chunks) and a quarter-warp's 16-byte reads (8 chunks of one row) then
 // fall on distinct banks.
 // Split-K work items store alpha x the fp32 tile into their slice of the workspace instead (EK_SPLITK).
-// row0: first row (within the batch) of this warpgroup's 64-row slab; col0: first column of the tile
+//
+// In the EPI_TMA kernels (p.epi_in != 0) the tile's [M, N] inputs arrive through the operand ring (epi_queue_inputs): box b holds chunk
+// b / epi_in of input b % epi_in, and ring item j (the j-th stage after the tile's last k-block) holds boxes
+// [j kEpiBoxesPerStage, (j + 1) kEpiBoxesPerStage). Each chunk waits for the items holding its boxes and releases the
+// items it has finished, so the producer refills them with the next tile's k-blocks while later chunks run.
+// row0: first row (within the batch) of this warpgroup's 64-row slab; col0: first column of the tile;
+// stage/phase: ring position of the first item, advanced past the tile's items
 // ---------------------------------------------------------------------------------------------
+
+// Operand ring as the epilogue sees it
+struct EpiRing {
+  uint8_t* a;  // A slots, Cfg::kABytes apart
+  uint8_t* b;  // B slots, Cfg::kBBytes apart
+  uint64_t* full;
+  uint64_t* empty;
+};
+
+// Column chunks of the tile starting at col0 that hold columns < N; the producer fetches inputs for these only.
 template <int BN>
+__device__ __forceinline__ int epi_chunks(const GemmKernelParams& p, int col0) {
+  return min(BN / kEpiCols, (p.N - col0 + kEpiCols - 1) / kEpiCols);
+}
+
+// Box k (< kEpiBoxesPerStage) of ring stage s
+template <int BN>
+__device__ __forceinline__ uint8_t* epi_box(const EpiRing& ring, int s, int k) {
+  return k == 0 ? ring.a + s * Cfg<BN>::kABytes : ring.b + s * Cfg<BN>::kBBytes + (k - 1) * kEpiBoxBytes;
+}
+
+template <int BN, bool EPI_TMA>
 __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float (&acc)[BN / 2], float* stage,
-                                         int bar_id, long long boff, int row0, int col0, int ks) {
+                                         int bar_id, long long boff, int row0, int col0, int ks, const EpiRing& ring,
+                                         int& ring_stage, uint32_t& ring_phase) {
+  constexpr int kStages = Cfg<BN>::kStages, kBps = Cfg<BN>::kEpiBoxesPerStage;
   const int wt = threadIdx.x & 127;
   const int fr = (wt >> 5) * 16 + ((wt & 31) >> 2);  // fragment rows fr, fr + 8; column pair 2 (wt % 4) of each 8
   const int fq = wt & 3;
   const int pr = wt >> 4, pc = wt & 15;  // processing: rows pr + 8 i, 16-byte chunk pc
-  const int nch = min(BN / kEpiCols, (p.N - col0 + kEpiCols - 1) / kEpiCols);
+  const int nch = epi_chunks<BN>(p, col0);
+  const int nin = EPI_TMA ? p.epi_in : 0;
+  // cursor over the staged boxes: the next one is slot bk of stage bs (phase bph); stages before rs are released
+  int bs = ring_stage, bk = 0, rs = ring_stage;
+  uint32_t bph = ring_phase;
+  auto next_box = [&]() {
+    if (bk == 0) mbar_wait(&ring.full[bs], bph);
+    const uint8_t* box = epi_box<BN>(ring, bs, bk);
+    if (++bk == kBps) {
+      bk = 0;
+      if (++bs == kStages) {
+        bs = 0;
+        bph ^= 1;
+      }
+    }
+    return box;
+  };
+  // Byte offset of this thread's 8 bytes (columns 4 pc .. 4 pc + 3) of row pr of its warpgroup's half of a box: in a
+  // SWIZZLE_128B box, 16-byte unit u of row r sits at u ^ (r & 7); rows pr + 8 i share r & 7 and lie 1024 B apart.
+  // A half-warp reads one 128-byte row: no bank conflicts.
+  const int box_off = ((row0 % BM) + pr) * 128 + (((pc >> 1) ^ pr) << 4) + ((pc & 1) << 3);
 #pragma unroll 1
   for (int ch = 0; ch < nch; ++ch) {
 #pragma unroll
@@ -211,6 +288,15 @@ __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float 
     }
     named_bar_sync(bar_id, 128);
     const int col = col0 + ch * kEpiCols + pc * 4;
+    // this chunk's input boxes, in epi_in order: aux_in (dact), res1, res2
+    const uint8_t *src_aux = nullptr, *src_res1 = nullptr, *src_res2 = nullptr;
+    if (nin) {
+      if (p.dact) src_aux = next_box() + box_off;
+      if (p.res1) src_res1 = next_box() + box_off;
+      if (p.res2) src_res2 = next_box() + box_off;
+    }
+    EpiIn in;
+    if (p.bias && col < p.N) ld_bf16x4(p.bias + col, min(4, p.N - col), in.bias);
 #pragma unroll 1
     for (int i = 0; i < 64 / 8; ++i) {
       const int r = pr + 8 * i;
@@ -223,9 +309,59 @@ __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float 
             make_float4(v[0], v[1], v[2], v[3]);
         continue;
       }
-      epi_store4(p, boff, row, col, v);
+      if (nin) {
+        if (p.dact) ld_smem_bf16x4(src_aux + i * 1024, in.aux);
+        if (p.res1) ld_smem_bf16x4(src_res1 + i * 1024, in.res1);
+        if (p.res2) ld_smem_bf16x4(src_res2 + i * 1024, in.res2);
+      } else {
+        epi_load_inputs(p, boff, row, col, in);
+      }
+      epi_store4(p, boff, row, col, v, in);
     }
-    named_bar_sync(bar_id, 128);  // the slice is rewritten by the next chunk
+    named_bar_sync(bar_id, 128);  // the slice is rewritten by the next chunk; the items read so far may be refilled
+    if (nin) {
+      if (ch + 1 == nch && bk != 0) {  // the tile's last item may be partly filled: it is done too
+        bk = 0;
+        if (++bs == kStages) {
+          bs = 0;
+          bph ^= 1;
+        }
+      }
+#pragma unroll 1
+      for (; rs != bs; rs = rs + 1 == kStages ? 0 : rs + 1)  // rs trails bs by fewer than kStages items
+        if (wt == 0) mbar_arrive(&ring.empty[rs]);
+    }
+  }
+  ring_stage = bs;
+  ring_phase = bph;
+}
+
+// Producer side: queues the tile's epilogue-input boxes (see epi_tile) as ring items after its last k-block.
+// maps: one tensor map per input, in epi_in order; m0: first row, col0: first column of the tile.
+template <int BN>
+__device__ __forceinline__ void epi_queue_inputs(const GemmKernelParams& p, const CUtensorMap* maps,
+                                                 const EpiRing& ring, int& stage, uint32_t& phase, int m0, int col0,
+                                                 int z0, int z1) {
+  constexpr int kStages = Cfg<BN>::kStages, kBps = Cfg<BN>::kEpiBoxesPerStage;
+  const int nbox = p.epi_in * epi_chunks<BN>(p, col0);
+  int col = col0, i = 0;  // box: input i, columns [col, col + 64)
+#pragma unroll 1
+  for (int b0 = 0; b0 < nbox; b0 += kBps) {
+    const int nb = min(kBps, nbox - b0);
+    mbar_wait(&ring.empty[stage], phase ^ 1);
+    mbar_expect_tx(&ring.full[stage], (uint32_t)(nb * kEpiBoxBytes));  // out-of-range parts are zero-filled
+#pragma unroll 1
+    for (int k = 0; k < nb; ++k) {
+      tma_load_4d(epi_box<BN>(ring, stage, k), &maps[i], &ring.full[stage], col, m0, z0, z1);
+      if (++i == p.epi_in) {
+        i = 0;
+        col += kEpiCols;
+      }
+    }
+    if (++stage == kStages) {
+      stage = 0;
+      phase ^= 1;
+    }
   }
 }
 

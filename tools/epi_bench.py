@@ -122,6 +122,7 @@ def main():
             case("pace plain   (15.5 tiles/CTA)", 8192, 8192, K)
             case("pace gelu+aux(15.5 tiles/CTA)", 8192, 8192, K, bias=True, act=ops.ACT_GELU_NEW, aux=True)
             case("pace res1    (15.5 tiles/CTA)", 8192, 8192, K, res=1)
+            case("pace dact    (15.5 tiles/CTA)", 8192, 8192, K, dact=ops.DACT_GELU_NEW)
     if "block" in only:
         M, d = 1024, 4096
         case("qkv fwd", M, 3 * d, d, cublas=True)
@@ -130,6 +131,7 @@ def main():
         case("fc_in fwd (bias+gelu+aux)", M, 4 * d, d, bias=True, act=ops.ACT_GELU_NEW, aux=True, cublas=True)
         case("fc_out fwd (+bias)", M, d, 4 * d, bias=True, cublas=True)
         case("fc_out dgrad (dgelu)", M, 4 * d, d, b_mn=True, dact=ops.DACT_GELU_NEW, cublas=True)
+        case("fc_out dgrad shape, plain", M, 4 * d, d, b_mn=True)  # the floor for the dgelu epilogue above
         case("fc_in dgrad", M, d, 4 * d, b_mn=True, cublas=True)
         case("qkv dgrad (+res1)", M, d, 3 * d, b_mn=True, res=1, cublas=True)
         case("lm_head", M, 50258 // 8 * 8, d, bias=True, cublas=True)
