@@ -176,9 +176,11 @@ int mb200_embed_assemble(const int64_t* captions, int64_t ldc, const void* wte, 
 /* word_embedding(ids) (magma/magma.py:205; sampling.py:88-90 input_ids path). */
 int mb200_embed_gather(const int64_t* ids, const void* wte, void* out, int32_t n, int32_t d, int32_t vocab,
                        void* stream);
-/* ForCausalLMLoss (hf:loss/loss_utils.py:28-67): shifted CE over bf16 logits [B*S][ldv], ignore -100, mean.
+/* ForCausalLMLoss (hf:loss/loss_utils.py:28-67): shifted CE over bf16 logits [B*S][ldv], mean over the valid targets.
+ * A target is valid when it lies in [0, V); every other label (-100, any other negative value, V..ldv-1 and beyond)
+ * is ignored: its row gets zero loss and zero gradient and does not count in n_valid.
  * row_loss fp32 [B*S], n_valid int32 [1], loss fp32 [1] are device scratch/outputs. When dlogits != NULL it
- * receives grad_scale * dloss/dlogits (may alias logits). */
+ * receives grad_scale * dloss/dlogits (may alias logits). logits and dlogits must be 16-byte aligned. */
 int mb200_cross_entropy(const void* logits, int64_t ldv, const int64_t* labels, int32_t B, int32_t S, int32_t V,
                         float* row_loss, int32_t* n_valid, float* loss, void* dlogits, float grad_scale,
                         void* stream);

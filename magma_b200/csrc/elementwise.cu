@@ -32,6 +32,12 @@ static void co_resident_kernels_init() {
   prefer_max_smem_carveout(cast_f32_bf16_kernel);
 }
 
+// True when every pointer (null counts as aligned) is a multiple of `bytes`, the width of the kernel's vector accesses.
+template <typename... Ptr>
+static inline bool aligned_to(uintptr_t bytes, const Ptr*... p) {
+  return ((reinterpret_cast<uintptr_t>(p) | ... | uintptr_t{0}) & (bytes - 1)) == 0;
+}
+
 static int g_opt_grid = 0;  // mb200_set_optimizer_grid
 static inline int opt_grid(int grid) { return (g_opt_grid > 0 && grid > g_opt_grid) ? g_opt_grid : grid; }
 
@@ -66,6 +72,7 @@ extern "C" int mb200_layernorm_fwd(const void* x, int64_t ldx, const void* gamma
   MB_REQUIRE(rows > 0 && d > 0 && d % 8 == 0 && d <= kLnThreads * kLnMaxVec * 8, MB200_E_SHAPE,
              "layernorm: d=%d must be a multiple of 8 and <= %d", d, kLnThreads * kLnMaxVec * 8);
   MB_REQUIRE(ldx % 8 == 0 && ldy % 8 == 0, MB200_E_ALIGN, "layernorm: row strides must be multiples of 8");
+  MB_REQUIRE(aligned_to(16, x, gamma, beta, y), MB200_E_ALIGN, "layernorm: x, gamma, beta, y must be 16-byte aligned");
   MB_CUDA(launch_pdl(layernorm_fwd_kernel, dim3(rows), dim3(kLnThreads), 0, ST(stream), (const bf16*)x, (long long)ldx,
                      (const bf16*)gamma, (const bf16*)beta, (bf16*)y, (long long)ldy, mean, rstd, (int)d, eps));
   MB_LAUNCH_CHECK();
@@ -80,6 +87,8 @@ extern "C" int mb200_layernorm_bwd(const void* dy, int64_t lddy, const void* x, 
              "layernorm_bwd: bad d=%d", d);
   MB_REQUIRE(lddy % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!res || ldres % 8 == 0), MB200_E_ALIGN,
              "layernorm_bwd: row strides must be multiples of 8");
+  MB_REQUIRE(aligned_to(16, dy, x, gamma, res, dx), MB200_E_ALIGN,
+             "layernorm_bwd: dy, x, gamma, res, dx must be 16-byte aligned");
   MB_CUDA(launch_pdl(layernorm_bwd_kernel, dim3(rows), dim3(kLnThreads), 0, ST(stream), (const bf16*)dy,
                      (long long)lddy, (const bf16*)x, (long long)ldx, (const bf16*)gamma, mean, rstd, (const bf16*)res,
                      (long long)ldres, (bf16*)dx, (long long)lddx, (int)d));
@@ -103,6 +112,7 @@ extern "C" int mb200_layernorm_param_grad_rows(const void* dy, int64_t lddy, con
   MB_ENTER();
   MB_REQUIRE(rows > 0 && d > 0 && d % 2 == 0 && lddy % 2 == 0 && ldx % 2 == 0, MB200_E_ALIGN,
              "layernorm_param_grad_rows: d and row strides must be even");
+  MB_REQUIRE(aligned_to(4, dy, x), MB200_E_ALIGN, "layernorm_param_grad_rows: dy, x must be 4-byte aligned");
   {
     // many rows: 2-D decomposition with one atomic per (column, row chunk)
     if (!accumulate) {
@@ -122,6 +132,7 @@ extern "C" int mb200_col_moments(const void* u, int64_t ldu, const void* v, int6
   MB_ENTER();
   MB_REQUIRE(rows > 0 && cols > 0 && cols % 2 == 0 && ldu % 2 == 0 && ldv % 2 == 0 && (!mask || ldm % 2 == 0),
              MB200_E_ALIGN, "col_moments: cols and row strides must be even");
+  MB_REQUIRE(aligned_to(4, u, v, mask), MB200_E_ALIGN, "col_moments: u, v, mask must be 4-byte aligned");
   MB_CUDA(cudaMemsetAsync(out1, 0, (size_t)cols * sizeof(float), ST(stream)));
   MB_CUDA(cudaMemsetAsync(out2, 0, (size_t)cols * sizeof(float), ST(stream)));
   dim3 grid((cols + 63) / 64, (rows + kMomRows - 1) / kMomRows);
@@ -151,6 +162,7 @@ extern "C" int mb200_col2im3x3(const void* dcols, void* dx, int32_t B, int32_t H
   MB_ENTER();
   MB_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && (stride == 1 || stride == 2), MB200_E_SHAPE,
              "col2im3x3: B=%d H=%d W=%d C=%d (multiple of 8) stride=%d (1 or 2)", B, H, W, C, stride);
+  MB_REQUIRE(aligned_to(16, dcols, dx), MB200_E_ALIGN, "col2im3x3: dcols, dx must be 16-byte aligned");
   const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
   col2im3x3_kernel<<<grid_for((long long)B * H * W * (C / 8), 256), 256, 0, ST(stream)>>>((const bf16*)dcols, (bf16*)dx, B,
                                                                                           H, W, C, stride, Ho, Wo);
@@ -163,6 +175,7 @@ extern "C" int mb200_avgpool_nhwc_bwd(const void* dy, void* dx, int32_t B, int32
   MB_ENTER();
   MB_REQUIRE(B > 0 && k >= 1 && H >= k && W >= k && C > 0 && C % 8 == 0, MB200_E_SHAPE,
              "avgpool_nhwc_bwd: B=%d H=%d W=%d C=%d k=%d", B, H, W, C, k);
+  MB_REQUIRE(aligned_to(16, dy, dx), MB200_E_ALIGN, "avgpool_nhwc_bwd: dy, dx must be 16-byte aligned");
   avgpool_nhwc_bwd_kernel<<<grid_for((long long)B * H * W * (C / 8), 256), 256, 0, ST(stream)>>>((const bf16*)dy, (bf16*)dx,
                                                                                                 B, H, W, C, k);
   MB_LAUNCH_CHECK();
@@ -288,6 +301,7 @@ extern "C" int mb200_embed_assemble(const int64_t* captions, int64_t ldc, const 
                                     void* stream) {
   MB_ENTER();
   MB_REQUIRE(d % 8 == 0 && L >= 0 && L <= S, MB200_E_SHAPE, "embed_assemble: bad d=%d L=%d S=%d", d, L, S);
+  MB_REQUIRE(aligned_to(16, wte, prefix, x), MB200_E_ALIGN, "embed_assemble: wte, prefix, x must be 16-byte aligned");
   embed_assemble_kernel<<<B * S, 256, 0, ST(stream)>>>((const long long*)captions, ldc, (const bf16*)wte,
                                                        (const bf16*)prefix, L, (bf16*)x, B, S, d, vocab);
   MB_LAUNCH_CHECK();
@@ -298,6 +312,7 @@ extern "C" int mb200_embed_gather(const int64_t* ids, const void* wte, void* out
                                   int32_t vocab, void* stream) {
   MB_ENTER();
   MB_REQUIRE(d % 8 == 0 && n > 0, MB200_E_SHAPE, "embed_gather: bad n=%d d=%d", n, d);
+  MB_REQUIRE(aligned_to(16, wte, out), MB200_E_ALIGN, "embed_gather: wte, out must be 16-byte aligned");
   embed_gather_kernel<<<n, 256, 0, ST(stream)>>>((const long long*)ids, (const bf16*)wte, (bf16*)out, d, vocab);
   MB_LAUNCH_CHECK();
   return 0;
@@ -309,7 +324,8 @@ extern "C" int mb200_cross_entropy(const void* logits, int64_t ldv, const int64_
   MB_ENTER();
   MB_REQUIRE(ldv % 8 == 0 && V <= ldv, MB200_E_ALIGN, "cross_entropy: ldv=%lld must be a multiple of 8 and >= V",
              (long long)ldv);
-  ce_count_kernel<<<1, 1024, 0, ST(stream)>>>((const long long*)labels, B, S, n_valid);
+  MB_REQUIRE(aligned_to(16, logits, dlogits), MB200_E_ALIGN, "cross_entropy: logits, dlogits must be 16-byte aligned");
+  ce_count_kernel<<<1, 1024, 0, ST(stream)>>>((const long long*)labels, B, S, V, n_valid);
   ce_row_kernel<<<B * S, kCeThreads, 0, ST(stream)>>>((const bf16*)logits, ldv, (const long long*)labels, S, V,
                                                       n_valid, row_loss, (bf16*)dlogits, grad_scale);
   ce_reduce_kernel<<<1, 1024, 0, ST(stream)>>>(row_loss, B * S, n_valid, loss);
@@ -322,6 +338,7 @@ extern "C" int mb200_colsum(const void* x, int64_t ldx, int32_t rows, int32_t co
                             void* stream) {
   MB_ENTER();
   MB_REQUIRE(cols % 2 == 0 && ldx % 2 == 0, MB200_E_ALIGN, "colsum: cols and ldx must be even");
+  MB_REQUIRE(aligned_to(4, x), MB200_E_ALIGN, "colsum: x must be 4-byte aligned");
   if (!accumulate) MB_CUDA(cudaMemsetAsync(out, 0, (size_t)cols * sizeof(float), ST(stream)));
   dim3 grid((cols + 63) / 64, (rows + kColsumRows - 1) / kColsumRows);
   MB_CUDA(launch_pdl(colsum_kernel, grid, dim3(256), 0, ST(stream), (const bf16*)x, (long long)ldx, (int)rows, (int)cols,
@@ -369,6 +386,7 @@ extern "C" int mb200_nchw_to_nhwc8(const void* src, void* dst, int32_t B, int32_
                                    void* stream) {
   MB_ENTER();
   MB_REQUIRE(C >= 1 && C <= 8 && B > 0 && H > 0 && W > 0, MB200_E_SHAPE, "nchw_to_nhwc8: B=%d C=%d H=%d W=%d", B, C, H, W);
+  MB_REQUIRE(aligned_to(16, dst), MB200_E_ALIGN, "nchw_to_nhwc8: dst must be 16-byte aligned");
   nchw_to_nhwc8_kernel<<<grid_for((long long)B * H * W, 256), 256, 0, ST(stream)>>>((const bf16*)src, (bf16*)dst, B, C,
                                                                                    H, W);
   MB_LAUNCH_CHECK();
@@ -380,6 +398,7 @@ extern "C" int mb200_im2col3x3(const void* src, void* dst, int32_t B, int32_t H,
   MB_ENTER();
   MB_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && (stride == 1 || stride == 2), MB200_E_SHAPE,
              "im2col3x3: B=%d H=%d W=%d C=%d (multiple of 8) stride=%d (1 or 2)", B, H, W, C, stride);
+  MB_REQUIRE(aligned_to(16, src, dst), MB200_E_ALIGN, "im2col3x3: src, dst must be 16-byte aligned");
   const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
   const long long nvec = (long long)B * Ho * Wo * 9 * (C / 8);
   if (nvec < (1LL << 31) - (1LL << 24))  // headroom for the grid-stride increment
@@ -397,6 +416,7 @@ extern "C" int mb200_avgpool_nhwc(const void* src, void* dst, int32_t B, int32_t
   MB_ENTER();
   MB_REQUIRE(B > 0 && k >= 1 && H >= k && W >= k && C > 0 && C % 8 == 0, MB200_E_SHAPE,
              "avgpool_nhwc: B=%d H=%d W=%d C=%d (multiple of 8) k=%d", B, H, W, C, k);
+  MB_REQUIRE(aligned_to(16, src, dst), MB200_E_ALIGN, "avgpool_nhwc: src, dst must be 16-byte aligned");
   avgpool_nhwc_kernel<<<grid_for((long long)B * (H / k) * (W / k) * (C / 8), 256), 256, 0, ST(stream)>>>(
       (const bf16*)src, (bf16*)dst, B, H, W, C, k);
   MB_LAUNCH_CHECK();
@@ -405,6 +425,8 @@ extern "C" int mb200_avgpool_nhwc(const void* src, void* dst, int32_t B, int32_t
 
 extern "C" int mb200_argmax(const void* x, int64_t ldx, int32_t rows, int32_t V, int64_t* out, void* stream) {
   MB_ENTER();
+  MB_REQUIRE(rows > 0 && V > 0 && V <= ldx, MB200_E_SHAPE, "argmax: need rows=%d > 0 and 0 < V=%d <= ldx=%lld", rows, V,
+             (long long)ldx);
   argmax_kernel<<<rows, 512, 0, ST(stream)>>>((const bf16*)x, ldx, V, (long long*)out);
   MB_LAUNCH_CHECK();
   return 0;
@@ -413,6 +435,7 @@ extern "C" int mb200_argmax(const void* x, int64_t ldx, int32_t rows, int32_t V,
 extern "C" int mb200_add(const void* a, const void* b, const void* c, void* y, int64_t n, void* stream) {
   MB_ENTER();
   MB_REQUIRE(n % 8 == 0, MB200_E_ALIGN, "add: n must be a multiple of 8");
+  MB_REQUIRE(aligned_to(16, a, b, c, y), MB200_E_ALIGN, "add: a, b, c, y must be 16-byte aligned");
   add_kernel<<<grid_for(n / 8, 256), 256, 0, ST(stream)>>>((const bf16*)a, (const bf16*)b, (const bf16*)c, (bf16*)y,
                                                            n / 8);
   MB_LAUNCH_CHECK();
@@ -457,6 +480,8 @@ extern "C" int mb200_adamw_step(float* master, float* grad, float* exp_avg, floa
   MB_REQUIRE(step >= 1, MB200_E_ARG, "adamw: step must be >= 1");
   const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
   MB_REQUIRE(n % 4 == 0, MB200_E_ALIGN, "adamw: n must be a multiple of 4 (the arena pads every tensor to 64)");
+  MB_REQUIRE(aligned_to(16, master, grad, exp_avg, exp_avg_sq) && aligned_to(8, shadow_bf16), MB200_E_ALIGN,
+             "adamw: master, grad, moments must be 16-byte aligned, the bf16 shadow 8-byte aligned");
   co_resident_kernels_init();
   adamw_kernel<<<opt_grid(grid_for(n / 4, 256)), 256, 0, ST(stream)>>>(master, grad, exp_avg, exp_avg_sq, (bf16*)shadow_bf16, n / 4, lr,
                                                          beta1, beta2, eps, weight_decay, grad_scale, gnorm_sq,
@@ -539,6 +564,7 @@ extern "C" int mb200_decode_embed(const int64_t* tokens, int64_t ld_tok, const i
                                   int32_t B, int32_t d, int32_t vocab, void* stream) {
   MB_ENTER();
   MB_REQUIRE(d % 8 == 0 && B > 0 && tokens && pos_dev, MB200_E_SHAPE, "decode_embed: bad B=%d d=%d", B, d);
+  MB_REQUIRE(aligned_to(16, wte, x), MB200_E_ALIGN, "decode_embed: wte, x must be 16-byte aligned");
   mb200::decode_embed_kernel<<<B, 256, 0, ST(stream)>>>((const long long*)tokens, ld_tok, pos_dev, (const bf16*)wte,
                                                          (bf16*)x, d, vocab);
   MB_LAUNCH_CHECK();

@@ -287,16 +287,17 @@ __global__ void embed_gather_kernel(const long long* __restrict__ ids, const bf1
 
 // ---------------------------------------------------------------------------------------------
 // Shifted cross-entropy over bf16 logits [M = B*S][ldv] (ForCausalLMLoss, loss_utils.py:28-67):
-// target of row (b, s) is labels[b, s+1]; the last position and label -100 are ignored; mean over valid.
+// target of row (b, s) is labels[b, s+1]; the last position and every target outside [0, V) (-100 among them) are
+// ignored; mean over valid. Both passes below apply that one rule, so an ignored row never enters n_valid.
 // Pass 1 (ce_count): n_valid. Pass 2 (ce_row): per-row loss + in-place dlogits = (softmax - onehot)/n_valid.
 // Pass 3 (ce_reduce): deterministic tree sum of row losses -> mean.
 // ---------------------------------------------------------------------------------------------
-__global__ void ce_count_kernel(const long long* __restrict__ labels, int B, int S, int* __restrict__ n_valid) {
+__global__ void ce_count_kernel(const long long* __restrict__ labels, int B, int S, int V, int* __restrict__ n_valid) {
   __shared__ float red[32];
   float c = 0.f;
   for (int i = threadIdx.x; i < B * S; i += blockDim.x) {
     const int s = i % S;
-    if (s + 1 < S && labels[i + 1] != -100) c += 1.f;
+    if (s + 1 < S && labels[i + 1] >= 0 && labels[i + 1] < V) c += 1.f;
   }
   const float t = block_sum<1024>(c, red);
   if (threadIdx.x == 0) *n_valid = (int)(t + 0.5f);
@@ -313,7 +314,7 @@ ce_row_kernel(const bf16* logits, long long ldv, const long long* __restrict__ l
   const bf16* lr = logits + (long long)row * ldv;
   bf16* dr = dlogits ? dlogits + (long long)row * ldv : nullptr;
   const int nvec = V >> 3;
-  if (tgt == -100 || tgt < 0 || tgt >= V) {
+  if (tgt < 0 || tgt >= V) {  // the validity rule of ce_count_kernel
     if (threadIdx.x == 0) row_loss[row] = 0.f;
     if (dr) {
       const uint4 z = make_uint4(0, 0, 0, 0);

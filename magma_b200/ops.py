@@ -156,12 +156,13 @@ def layernorm_fwd(x, gamma, beta, eps=1e-5, save_stats=True, out=None):
     return y, mean, rstd
 
 
-def layernorm_bwd(dy, x, gamma, mean, rstd, res=None):
+def layernorm_bwd(dy, x, gamma, mean, rstd, res=None, out=None):
+    """dx of LayerNorm (+ res); into `out` (any row stride) when given."""
     rows, d, ldx = _rows(x)
-    dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if out is None else out
     check(lib().mb200_layernorm_bwd(_ptr(dy), ctypes.c_int64(_rows(dy)[2]), _ptr(x), ctypes.c_int64(ldx), _ptr(gamma),
                                     _ptr(mean), _ptr(rstd), _ptr(res), ctypes.c_int64(_rows(res)[2] if res is not None else 0),
-                                    _ptr(dx), ctypes.c_int64(d), rows, d, _stream()))
+                                    _ptr(dx), ctypes.c_int64(_rows(dx)[2]), rows, d, _stream()))
     return dx
 
 
@@ -243,33 +244,37 @@ def build_labels(captions, prefix_len, eos_token):
     return labels
 
 
-def embed_assemble(captions, wte, prefix, S=None):
+def embed_assemble(captions, wte, prefix, S=None, out=None):
     B, Sc = captions.shape
     S = Sc if S is None else S
     L = 0 if prefix is None else prefix.shape[1]
     V, d = wte.shape
-    x = torch.empty(B, S, d, dtype=torch.bfloat16, device=wte.device)
+    x = torch.empty(B, S, d, dtype=torch.bfloat16, device=wte.device) if out is None else out
     check(lib().mb200_embed_assemble(_ptr(captions), ctypes.c_int64(captions.stride(0)), _ptr(wte), _ptr(prefix), L,
                                      _ptr(x), B, S, d, V, _stream()))
     return x
 
 
-def embed_gather(ids, wte):
+def embed_gather(ids, wte, out=None):
     V, d = wte.shape
     flat = ids.reshape(-1).contiguous()
-    out = torch.empty(*ids.shape, d, dtype=torch.bfloat16, device=wte.device)
+    out = torch.empty(*ids.shape, d, dtype=torch.bfloat16, device=wte.device) if out is None else out
     check(lib().mb200_embed_gather(_ptr(flat), _ptr(wte), _ptr(out), flat.numel(), d, V, _stream()))
     return out
 
 
-def cross_entropy(logits, labels, V, write_grad=False, grad_scale=1.0):
-    """logits bf16 [B,S,ldv]; returns (loss fp32 [1], dlogits or None)."""
+def cross_entropy(logits, labels, V, write_grad=False, grad_scale=1.0, dlogits=None, row_loss=None):
+    """logits bf16 [B,S,ldv]; returns (loss fp32 [1], dlogits or None). `dlogits` (same strides as logits; may be
+    logits itself) receives the gradient instead of a new buffer; `row_loss` (fp32 [B*S]) the per-row losses."""
     B, S = labels.shape
     ldv = logits.stride(-2)
-    row_loss = torch.empty(B * S, dtype=torch.float32, device=logits.device)
+    if row_loss is None:
+        row_loss = torch.empty(B * S, dtype=torch.float32, device=logits.device)
     n_valid = torch.zeros(4, dtype=torch.int32, device=logits.device)
     loss = torch.empty(1, dtype=torch.float32, device=logits.device)
-    dl = torch.zeros_like(logits) if write_grad else None
+    if dlogits is not None and dlogits.stride() != logits.stride():
+        raise ValueError("cross_entropy: dlogits must share the strides of logits")
+    dl = dlogits if dlogits is not None else (torch.zeros_like(logits) if write_grad else None)
     check(lib().mb200_cross_entropy(_ptr(logits), ctypes.c_int64(ldv), _ptr(labels), B, S, V, _ptr(row_loss),
                                     _ptr(n_valid), _ptr(loss), _ptr(dl), ctypes.c_float(grad_scale), _stream()))
     return loss, dl
@@ -283,16 +288,16 @@ def colsum(x, out=None, accumulate=False):
     return out
 
 
-def dropout_fwd(x, p, seed):
-    y = torch.empty_like(x)
+def dropout_fwd(x, p, seed, out=None):
+    y = torch.empty_like(x) if out is None else out
     mask = torch.empty(x.numel(), dtype=torch.uint8, device=x.device)
     check(lib().mb200_dropout_fwd(_ptr(x), _ptr(y), _ptr(mask), ctypes.c_int64(x.numel()), ctypes.c_float(p),
                                   ctypes.c_uint64(seed), _stream()))
     return y, mask
 
 
-def dropout_apply(x, mask, p):
-    y = torch.empty_like(x)
+def dropout_apply(x, mask, p, out=None):
+    y = torch.empty_like(x) if out is None else out
     check(lib().mb200_dropout_apply(_ptr(x), _ptr(mask), _ptr(y), ctypes.c_int64(x.numel()), ctypes.c_float(p), _stream()))
     return y
 
@@ -322,30 +327,30 @@ def decode_advance(next_tokens, tokens, pos_dev, eos, flags, s0):
                                      flags.numel() if flags is not None else 0, tokens.shape[0], _stream()))
 
 
-def nchw_to_nhwc8(x):
+def nchw_to_nhwc8(x, out=None):
     """[B, C<=8, H, W] bf16 -> [B, H, W, 8] bf16 with zero-padded channels (conv-trunk stem input)."""
     assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.ndim == 4
     B, C, H, W = x.shape
-    y = torch.empty(B, H, W, 8, dtype=torch.bfloat16, device=x.device)
+    y = torch.empty(B, H, W, 8, dtype=torch.bfloat16, device=x.device) if out is None else out
     check(lib().mb200_nchw_to_nhwc8(_ptr(x), _ptr(y), B, C, H, W, _stream()))
     return y
 
 
-def im2col3x3(x, stride=1):
+def im2col3x3(x, stride=1, out=None):
     """NHWC [B,H,W,C] bf16 -> [B*Ho*Wo, 9*C] bf16 (3x3, padding 1), columns ordered (kh, kw, c)."""
     assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.ndim == 4
     B, H, W, C = x.shape
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    y = torch.empty(B * Ho * Wo, 9 * C, dtype=torch.bfloat16, device=x.device)
+    y = torch.empty(B * Ho * Wo, 9 * C, dtype=torch.bfloat16, device=x.device) if out is None else out
     check(lib().mb200_im2col3x3(_ptr(x), _ptr(y), B, H, W, C, stride, _stream()))
     return y, Ho, Wo
 
 
-def avgpool_nhwc(x, k):
+def avgpool_nhwc(x, k, out=None):
     """nn.AvgPool2d(k) on NHWC bf16: [B,H,W,C] -> [B,H//k,W//k,C]."""
     assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.ndim == 4
     B, H, W, C = x.shape
-    y = torch.empty(B, H // k, W // k, C, dtype=torch.bfloat16, device=x.device)
+    y = torch.empty(B, H // k, W // k, C, dtype=torch.bfloat16, device=x.device) if out is None else out
     check(lib().mb200_avgpool_nhwc(_ptr(x), _ptr(y), B, H, W, C, k, _stream()))
     return y
 
@@ -362,7 +367,7 @@ def col_moments(u, v, mask=None):
     return o1, o2
 
 
-def channel_affine(x1, a1, x2=None, a2=None, c0=None, mask=None, res=None, relu=False):
+def channel_affine(x1, a1, x2=None, a2=None, c0=None, mask=None, res=None, relu=False, out=None):
     """y = relu?(a1[c] * x1 * 1[mask > 0] + a2[c] * x2 + c0[c] + res) over contiguous [rows, C] bf16 tensors with fp32
     per-channel coefficients (BatchNorm forward / backward, ReLU backward)."""
     rows, C = x1.shape
@@ -370,7 +375,7 @@ def channel_affine(x1, a1, x2=None, a2=None, c0=None, mask=None, res=None, relu=
         assert t is None or (t.dtype == torch.bfloat16 and t.is_contiguous() and t.shape == x1.shape)
     for t in (a1, a2, c0):
         assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.numel() == C)
-    y = torch.empty_like(x1)
+    y = torch.empty_like(x1) if out is None else out
     check(lib().mb200_channel_affine(_ptr(x1), _ptr(a1), _ptr(x2), _ptr(a2), _ptr(c0), _ptr(mask), _ptr(res), int(relu),
                                      _ptr(y), ctypes.c_int64(rows), C, _stream()))
     return y
@@ -401,19 +406,19 @@ def bn_bwd_coeffs(s1, t, mean, rstd, gamma, rows, dgamma, dbeta, accumulate=Fals
     return out[0], out[1], out[2]
 
 
-def col2im3x3(dcols, B, H, W, C, stride=1):
+def col2im3x3(dcols, B, H, W, C, stride=1, out=None):
     """Adjoint of im2col3x3: [B*Ho*Wo, 9*C] bf16 -> [B, H, W, C] bf16."""
     assert dcols.dtype == torch.bfloat16 and dcols.is_contiguous() and dcols.shape[1] == 9 * C
-    dx = torch.empty(B, H, W, C, dtype=torch.bfloat16, device=dcols.device)
+    dx = torch.empty(B, H, W, C, dtype=torch.bfloat16, device=dcols.device) if out is None else out
     check(lib().mb200_col2im3x3(_ptr(dcols), _ptr(dx), B, H, W, C, stride, _stream()))
     return dx
 
 
-def avgpool_nhwc_bwd(dy, H, W, k):
+def avgpool_nhwc_bwd(dy, H, W, k, out=None):
     """Adjoint of avgpool_nhwc: [B, H//k, W//k, C] -> [B, H, W, C]."""
     assert dy.dtype == torch.bfloat16 and dy.is_contiguous() and dy.ndim == 4
     B, _, _, C = dy.shape
-    dx = torch.empty(B, H, W, C, dtype=torch.bfloat16, device=dy.device)
+    dx = torch.empty(B, H, W, C, dtype=torch.bfloat16, device=dy.device) if out is None else out
     check(lib().mb200_avgpool_nhwc_bwd(_ptr(dy), _ptr(dx), B, H, W, C, k, _stream()))
     return dx
 
@@ -431,8 +436,8 @@ def sample(logits, temperature, top_k=0, top_p=0.0, seed=0, offset=0, return_mas
     return (out, mask) if return_mask else out
 
 
-def add(a, b, c=None):
-    y = torch.empty_like(a)
+def add(a, b, c=None, out=None):
+    y = torch.empty_like(a) if out is None else out
     check(lib().mb200_add(_ptr(a), _ptr(b), _ptr(c), _ptr(y), ctypes.c_int64(a.numel()), _stream()))
     return y
 
@@ -446,6 +451,49 @@ def peer_reduce_bcast(buffer_ptrs, offset, n, max_blocks=0):
 
 def cast_f32_to_bf16(src, dst):
     check(lib().mb200_cast_f32_to_bf16(_ptr(src), _ptr(dst), ctypes.c_int64(src.numel()), _stream()))
+
+
+def cast_bf16_to_f32(src, dst):
+    check(lib().mb200_cast_bf16_to_f32(_ptr(src), _ptr(dst), ctypes.c_int64(src.numel()), _stream()))
+
+
+def patchify(img, P, out):
+    """images bf16 [B, 3, R, R] -> out [B * (R/P)^2, >= 3 P P] (row stride out.stride(0)), columns ordered (c, py, px)."""
+    B, _, R, _ = img.shape
+    check(lib().mb200_patchify(_ptr(img), _ptr(out), ctypes.c_int64(out.stride(0)), B, R, P, _stream()))
+    return out
+
+
+def vit_assemble(x, pe, cls, pos):
+    """x [B, T, w] = [cls; pe] + pos with pe [B, T-1, w], cls [w], pos [T, w] (all contiguous bf16)."""
+    B, T, w = x.shape
+    check(lib().mb200_vit_assemble(_ptr(x), _ptr(pe), _ptr(cls), _ptr(pos), B, T, w, _stream()))
+    return x
+
+
+def scale_add(u, s=None, r1=None, r2=None, out=None):
+    """out = s[0] * u + r1 + r2 (s: device fp32 scalar or None for 1; r1 / r2 optional), bf16."""
+    out = torch.empty_like(u) if out is None else out
+    check(lib().mb200_scale_add(_ptr(u), _ptr(s), _ptr(r1), _ptr(r2), _ptr(out), ctypes.c_int64(u.numel()), _stream()))
+    return out
+
+
+def dot(a, b, out, accumulate=False):
+    """out[0] (+)= sum a * b over bf16 vectors, fp32."""
+    check(lib().mb200_dot(_ptr(a), _ptr(b), ctypes.c_int64(a.numel()), _ptr(out), int(accumulate), _stream()))
+    return out
+
+
+def rope_table_dev(S, rot, pos0_dev, out=None):
+    """rope_table with the first position read from device memory (int32 [1])."""
+    tab = torch.empty(S, rot // 2, 2, dtype=torch.float32, device=pos0_dev.device) if out is None else out
+    check(lib().mb200_rope_table_dev(_ptr(tab), S, rot, _ptr(pos0_dev), _stream()))
+    return tab
+
+
+def set_optimizer_grid(n_blocks):
+    """Cap the grid of the optimizer kernels (sumsq, adamw) at n_blocks (0: no cap). Returns the cap in force."""
+    return lib().mb200_set_optimizer_grid(int(n_blocks))
 
 
 def sumsq(x, out):

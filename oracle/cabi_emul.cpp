@@ -398,7 +398,7 @@ int mb200_cross_entropy(const void* logits_, int64_t ldv, const int64_t* labels,
   bf16_t* dlogits = (bf16_t*)dlogits_;
   int nv = 0;
   for (int i = 0; i < B * S; ++i)
-    if (i % S + 1 < S && labels[i + 1] != -100) ++nv;
+    if (i % S + 1 < S && labels[i + 1] >= 0 && labels[i + 1] < V) ++nv;
   *n_valid = nv;
   const float gs = grad_scale / (float)(nv > 0 ? nv : 1);
   double total = 0.0;
@@ -408,7 +408,7 @@ int mb200_cross_entropy(const void* logits_, int64_t ldv, const int64_t* labels,
     const long long tgt = s + 1 < S ? labels[row + 1] : -100;
     const bf16_t* lr = logits + (long long)row * ldv;
     bf16_t* dr = dlogits ? dlogits + (long long)row * ldv : nullptr;
-    if (tgt == -100 || tgt < 0 || tgt >= V) {
+    if (tgt < 0 || tgt >= V) {
       row_loss[row] = 0.f;
       if (dr)
         for (int j = 0; j < V; ++j) dr[j] = f2b(0.f);

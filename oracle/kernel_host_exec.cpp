@@ -311,7 +311,7 @@ int mb200_embed_gather(const int64_t* ids, const void* wte, void* out, int32_t n
 }
 int mb200_cross_entropy(const void* logits, int64_t ldv, const int64_t* labels, int32_t B, int32_t S, int32_t V,
                         float* row_loss, int32_t* n_valid, float* loss, void* dlogits, float grad_scale, void*) {
-  run_grid(Dim3{1, 1, 1}, 1024, [&] { ce_count_kernel((const long long*)labels, B, S, n_valid); });
+  run_grid(Dim3{1, 1, 1}, 1024, [&] { ce_count_kernel((const long long*)labels, B, S, V, n_valid); });
   run_grid(Dim3{(unsigned)(B * S), 1, 1}, kCeThreads, [&] {
     ce_row_kernel((const bf16*)logits, ldv, (const long long*)labels, S, V, n_valid, row_loss, (bf16*)dlogits, grad_scale);
   });

@@ -1,7 +1,10 @@
 """Shared pieces of the element-wise float64 reference tests (tests/test_gemm_reference_gpu.py,
-tests/test_attention_reference_gpu.py): sentinel-filled output buffers, bit snapshots of inputs, bf16 ulps and
-round-to-nearest-even from float64, the device under test and the launch counter."""
+tests/test_attention_reference_gpu.py, tests/test_elementwise_reference_gpu.py): sentinel-filled output buffers, bit
+snapshots of inputs, bf16 ulps and round-to-nearest-even from float64, the rounding rule for bf16 outputs, the device
+under test and the launch counter."""
 import os
+
+import pytest
 
 SENTINEL = -1.5e38
 
@@ -72,3 +75,39 @@ def bf16_rne(x):
 
     u = ulp_bf16(x)
     return torch.round(x / u) * u  # torch.round rounds half to even; x / u is exact (u is a power of two)
+
+
+def roundings(ref, delta, band=None):
+    """bf16 roundings of the interval ends (the lower end is 0 in the flush band)."""
+    import torch
+
+    lo = ref - delta
+    if band is not None:
+        lo = torch.where(band, torch.zeros_like(lo), lo)
+    return bf16_rne(lo), bf16_rne(ref + delta)
+
+
+def check_rounded(name, got, ref, delta, keep, band=None, limit=0.001):
+    """The rounding rule: a bf16 output whose float computation is within `delta` of the float64 `ref` must equal the
+    reference rounding unless [ref - delta, ref + delta] holds a rounding midpoint; then it may take either rounding of
+    the interval ends. At most `limit` of the kept elements (plus 8) may be ambiguous. Returns the width
+    (upper - lower rounding) of every element that may take either value."""
+    import torch
+
+    keep = keep.expand(ref.shape)
+    rlo, rhi = roundings(ref, delta, band)
+    g = got.double()
+    bad = ~((g >= rlo) & (g <= rhi)) & keep
+    either = (rlo != rhi) & keep
+    n_flush = int((either & band).sum().item()) if band is not None else 0
+    n_amb = int(either.sum().item()) - n_flush
+    n = int(keep.sum().item())
+    if int(bad.sum().item()):
+        i = int(bad.reshape(-1).nonzero()[0].item())
+        idx = tuple(int(t) for t in torch.unravel_index(torch.tensor(i), ref.shape))
+        pytest.fail(f"{name}: {int(bad.sum().item())} of {n} elements break the rounding rule; first at {idx}: got "
+                    f"{g.reshape(-1)[i].item():.9g}, reference {ref.reshape(-1)[i].item():.9g} rounds to "
+                    f"[{rlo.reshape(-1)[i].item():.9g}, {rhi.reshape(-1)[i].item():.9g}]")
+    assert n_amb <= limit * n + 8, f"{name}: {n_amb} of {n} elements ambiguous (limit {limit:.1%})"
+    print(f"[ambiguous] {name}: {n_amb} of {n} ({n_flush} more in the flush band)")
+    return torch.where(either, rhi - rlo, torch.zeros_like(ref))

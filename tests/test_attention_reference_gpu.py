@@ -73,7 +73,8 @@ import zlib
 
 import pytest
 
-from _refcheck import SENTINEL, Buf, bf16_rne, bits, dev as _dev, launches, ulp_bf16
+from _refcheck import SENTINEL, Buf, bf16_rne, bits, check_rounded, dev as _dev, launches, ulp_bf16
+from _refcheck import roundings as _roundings
 
 pytestmark = pytest.mark.gpu
 
@@ -207,38 +208,9 @@ def _probs(s, ds, vis, depth, rescales=0):
     return p, E, flush
 
 
-def _roundings(ref, delta, band=None):
-    """bf16 roundings of the interval ends (the lower end is 0 in the flush band)."""
-    import torch
-
-    lo = ref - delta
-    if band is not None:
-        lo = torch.where(band, torch.zeros_like(lo), lo)
-    return bf16_rne(lo), bf16_rne(ref + delta)
-
-
 def _check_rounded(name, got, ref, delta, keep, band=None, dist="std2"):
-    """The rounding rule. Returns the width (upper - lower rounding) of every element that may take either value."""
-    import torch
-
-    keep = keep.expand(ref.shape)
-    rlo, rhi = _roundings(ref, delta, band)
-    g = got.double()
-    bad = ~((g >= rlo) & (g <= rhi)) & keep
-    either = (rlo != rhi) & keep
-    n_flush = int((either & band).sum().item()) if band is not None else 0
-    n_amb = int(either.sum().item()) - n_flush
-    n = int(keep.sum().item())
-    if int(bad.sum().item()):
-        i = int(bad.reshape(-1).nonzero()[0].item())
-        idx = tuple(int(t) for t in torch.unravel_index(torch.tensor(i), ref.shape))
-        pytest.fail(f"{name}: {int(bad.sum().item())} of {n} elements break the rounding rule; first at {idx}: got "
-                    f"{g.reshape(-1)[i].item():.9g}, reference {ref.reshape(-1)[i].item():.9g} rounds to "
-                    f"[{rlo.reshape(-1)[i].item():.9g}, {rhi.reshape(-1)[i].item():.9g}]")
-    limit = AMBIGUOUS_MAX.get(dist, AMBIGUOUS_MAX["std2"])
-    assert n_amb <= limit * n + 8, f"{name}: {n_amb} of {n} elements ambiguous (limit {limit:.0%})"
-    print(f"[ambiguous] {name}: {n_amb} of {n} ({n_flush} more in the flush band)")
-    return torch.where(either, rhi - rlo, torch.zeros_like(ref))
+    """The rounding rule (tests/_refcheck.py) with this file's ambiguous-share cap for the score distribution."""
+    return check_rounded(name, got, ref, delta, keep, band, AMBIGUOUS_MAX.get(dist, AMBIGUOUS_MAX["std2"]))
 
 
 def _check_bound(name, got, ref, extra):
