@@ -20,119 +20,16 @@
 // batched GEMMs + softmax kernels for head dims the fused kernels do not take. The LM is frozen: dgrad through every
 // GEMM, wgrad only for adapters.
 //
-// No kernels and no CUDA calls here (sched_rt.h): tests/test_sched_emul_cpu.py compiles this file as plain C++ against
+// No kernels and no CUDA calls here (sched_rt.h, which also holds the GEMM helpers and the materialised attention this
+// file shares with vit_sched.cu): tests/test_sched_emul_cpu.py compiles this file as plain C++ against
 // oracle/cabi_emul.cpp and checks every adapter form against torch autograd of the oracle on the CPU; on the GPU it is
 // the path every LM test and the benchmark run.
 #include "sched_rt.h"
 
-#include <math.h>
 #include <stdlib.h>
-#include <string.h>
 
 namespace mb200 {
 namespace {
-
-typedef uint16_t bf16s;
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-struct Carver {
-  uint8_t* base;
-  size_t off;
-  explicit Carver(void* b) : base(reinterpret_cast<uint8_t*>(b)), off(0) {}
-  template <typename T>
-  T* take(size_t n) {
-    off = align_up(off, 256);
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * sizeof(T);
-    return p;
-  }
-};
-
-struct Mat {
-  const void* p;
-  long long ld, bs0, bs1;
-  int mn, frozen;
-};
-inline Mat mat(const void* p, long long ld, int mn = 0, long long bs0 = 0, long long bs1 = 0) {
-  return Mat{p, ld, bs0, bs1, mn, 0};
-}
-// a frozen weight matrix (never written by a kernel of the stream): the GEMM may fetch its first tiles ahead of the
-// programmatic dependency on the previous kernel (mb200_operand.static_data)
-inline Mat wmat(const void* p, long long ld, int mn = 0) { return Mat{p, ld, 0, 0, mn, 1}; }
-struct Epi {
-  float alpha = 1.f;
-  const void* bias = nullptr;
-  int act = 0;
-  void* aux_out = nullptr;
-  const void* aux_in = nullptr;
-  int dact = 0;
-  const void* res1 = nullptr;
-  const void* res2 = nullptr;
-  long long ld_res = 0;
-  int accumulate = 0;
-  const float* rope_tab = nullptr;
-  int rope_mode = 0, rope_S = 0, rope_hd = 0, rope_rot = 0, rope_ncols = 0;
-};
-
-// scratch the training / ViT passes lend to the GEMM core (mb200_gemm_args.splitk_ws): the fp32 per-split partial slices of
-// the GEMMs gemm.cu splits along K (small-M, split_mid and split_few plans); the split count shrinks to what fits
-const size_t kGemmScratchBytes = (size_t)128 << 20;
-
-// split-K scratch of the pass being issued (small-M decode GEMMs stream their weights; see gemm.cu::plan_small_m)
-thread_local void* t_splitk_ws = nullptr;
-thread_local long long t_splitk_bytes = 0;
-
-struct ScratchScope {  // the scratch is only valid while the pass that owns the workspace is being issued
-  ScratchScope(void* w, size_t b) { t_splitk_ws = w; t_splitk_bytes = (long long)b; }
-  ~ScratchScope() { t_splitk_ws = nullptr; t_splitk_bytes = 0; }
-};
-
-int gemm(void* st, int M, int N, int K, Mat A, Mat B, void* C, long long ldc, int c_f32, const Epi& e = Epi(),
-         int nb0 = 1, int nb1 = 1, long long c_bs0 = 0, long long c_bs1 = 0) {
-  mb200_gemm_args g;
-  memset(&g, 0, sizeof(g));
-  g.M = M;
-  g.N = N;
-  g.K = K;
-  g.nb0 = nb0;
-  g.nb1 = nb1;
-  g.c_dtype = c_f32 ? MB200_F32 : MB200_BF16;
-  g.A.ptr = A.p;
-  g.A.ld = A.ld;
-  g.A.bs0 = A.bs0;
-  g.A.bs1 = A.bs1;
-  g.A.mn_major = A.mn;
-  g.B.ptr = B.p;
-  g.B.ld = B.ld;
-  g.B.bs0 = B.bs0;
-  g.B.bs1 = B.bs1;
-  g.B.mn_major = B.mn;
-  g.B.static_data = B.frozen;
-  g.C = C;
-  g.ldc = ldc;
-  g.c_bs0 = c_bs0;
-  g.c_bs1 = c_bs1;
-  g.alpha = e.alpha;
-  g.act = e.act;
-  g.dact = e.dact;
-  g.accumulate = e.accumulate;
-  g.bias = e.bias;
-  g.aux_out = e.aux_out;
-  g.aux_in = e.aux_in;
-  g.res1 = e.res1;
-  g.res2 = e.res2;
-  g.ld_res = e.ld_res;
-  g.rope_tab = e.rope_tab;
-  g.rope_mode = e.rope_mode;
-  g.rope_S = e.rope_S;
-  g.rope_hd = e.rope_hd;
-  g.rope_rot = e.rope_rot;
-  g.rope_ncols = e.rope_ncols;
-  g.splitk_ws = t_splitk_ws;
-  g.splitk_ws_bytes = t_splitk_bytes;
-  return mb200_gemm(&g, st);
-}
 
 // what one adapter keeps from forward to backward
 struct AdapterActs {
@@ -184,14 +81,17 @@ inline bool tile_ok(int S, int hd) {
   return on != 0 && S >= 1 && S <= 128 && hd >= 64 && hd <= 256 && hd % 64 == 0;
 }
 
-// the fused multi-tile forward takes any sequence length at those head dims; MB200_ATTN_FLASH=0 forces batched GEMMs
-inline bool flash_ok(int hd) {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("MB200_ATTN_FLASH");
-    on = e ? atoi(e) : 1;
-  }
-  return on != 0 && hd >= 64 && hd <= 256 && hd % 64 == 0;
+// the GEMM epilogue that rotates (mode 1) or inversely rotates (mode -1) the first rot dims of each hd-wide head in
+// columns [0, ncols), with the positions of row % S in the rotary table tab
+inline Epi rope_epi(const float* tab, int mode, int S, int hd, int rot, int ncols) {
+  Epi e;
+  e.rope_tab = tab;
+  e.rope_mode = mode;
+  e.rope_S = S;
+  e.rope_hd = hd;
+  e.rope_rot = rot;
+  e.rope_ncols = ncols;
+  return e;
 }
 
 inline bool has_ln(const mb200_adapter_ex& a) { return a.ln_g != nullptr; }
@@ -347,11 +247,9 @@ int adapter_bwd(void* st, const mb200_adapter_ex& ad, const AdapterActs& a, cons
   e1.aux_in = act ? a.pre : a.t;
   MBS_TRY(gemm(st, M, r, d, mat(gu, d), mat(ad.wu, r, 1), P.dt, r, 0, e1));  // dt = (gu Wu) * act'(pre)   (ReLU: 1[t > 0])
   if (ad.g_wd) {
-    Epi ew;
-    ew.accumulate = acc;
-    MBS_TRY(gemm(st, d, r, M, mat(gu, d, 1), mat(a.t, r, 1), ad.g_wu, r, 1, ew));    // dWu[d,r] = gu^T t
+    MBS_TRY(wgrad(st, d, r, M, gu, d, a.t, r, ad.g_wu, r, acc));    // dWu[d,r] = gu^T t
     MBS_TRY(mb200_colsum(gu, d, M, d, ad.g_bu, acc, st));
-    MBS_TRY(gemm(st, r, d, M, mat(P.dt, r, 1), mat(zin, d, 1), ad.g_wd, d, 1, ew));  // dWd[r,d] = dt^T zin
+    MBS_TRY(wgrad(st, r, d, M, P.dt, r, zin, d, ad.g_wd, d, acc));  // dWd[r,d] = dt^T zin
     MBS_TRY(mb200_colsum(P.dt, r, M, r, ad.g_bd, acc, st));
   }
   if (!has_ln(ad)) {
@@ -370,35 +268,22 @@ int adapter_bwd(void* st, const mb200_adapter_ex& ad, const AdapterActs& a, cons
 // P.acts[l]. The forward pass and the recompute backward both issue it, so a recomputed layer is the stored one bit for bit.
 int layer_fwd(const mb200_gptj_model_ex* m, Plan& P, int l, bf16s* xout, void* st) {
   const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd, B = P.B, S = P.S;
-  const float scale = 1.0f / sqrtf((float)hd);
   const long long qb0 = hd, qb1 = (long long)S * 3 * d;
-  const long long pb0 = (long long)S * P.ldP, pb1 = (long long)H * S * P.ldP;
   const mb200_gptj_layer_ex& L = m->layers[l];
   LayerActs& a = P.acts[l];
   const bf16s* xin = a.x_in;
   MBS_TRY(mb200_layernorm_fwd(xin, d, L.ln1_g, L.ln1_b, a.h, d, a.mean, a.rstd, M, d, m->ln_eps, st));
-  {  // fused q/k/v projection, rotary embedding applied to the q and k column ranges in the epilogue
-    Epi e;
-    e.rope_tab = P.rope_tab;
-    e.rope_mode = 1;
-    e.rope_S = S;
-    e.rope_hd = hd;
-    e.rope_rot = m->rotary_dim;
-    e.rope_ncols = 2 * d;
-    MBS_TRY(gemm(st, M, 3 * d, d, mat(a.h, d), wmat(L.w_qkv, d), a.qkv, 3 * d, 0, e));
-  }
+  // fused q/k/v projection, rotary embedding applied to the q and k column ranges in the epilogue
+  MBS_TRY(gemm(st, M, 3 * d, d, mat(a.h, d), wmat(L.w_qkv, d), a.qkv, 3 * d, 0,
+               rope_epi(P.rope_tab, 1, S, hd, m->rotary_dim, 2 * d)));
   if (tile_ok(S, hd)) {  // whole sequence in one tile: fused QK^T / softmax / PV, one CTA per (batch, head)
     MBS_TRY(mb200_attn_fwd_tile(a.qkv, 3 * d, a.P, P.ldP, a.attn_o, d, B, S, H, hd, st));
   } else if (flash_ok(hd)) {  // any S: fused multi-tile forward; P is written for the materialised backward
     MBS_TRY(mb200_attn_fwd_flash(a.qkv, 3 * d, qb0, qb1, a.qkv + d, 3 * d, qb0, qb1, a.qkv + 2 * d, 3 * d, qb0, qb1,
                                  a.attn_o, d, a.P, P.ldP, nullptr, B, S, S, H, hd, 1, st));
   } else {
-    // scores = Q K^T (fp32), P = softmax(scores / sqrt(hd) + causal mask), O = P V
-    MBS_TRY(gemm(st, S, S, hd, mat(a.qkv, 3 * d, 0, qb0, qb1), mat(a.qkv + d, 3 * d, 0, qb0, qb1), P.scores, P.ldP, 1,
-                 Epi(), H, B, pb0, pb1));
-    MBS_TRY(mb200_softmax_fwd(P.scores, P.ldP, pb0, a.P, P.ldP, pb0, B * H, S, S, scale, 1, 0, st));
-    MBS_TRY(gemm(st, S, hd, S, mat(a.P, P.ldP, 0, pb0, pb1), mat(a.qkv + 2 * d, 3 * d, 1, qb0, qb1), a.attn_o, d, 0,
-                 Epi(), H, B, hd, (long long)S * d));
+    MBS_TRY(attn_fwd_gemm(st, mat(a.qkv, 3 * d, 0, qb0, qb1), mat(a.qkv + d, 3 * d, 0, qb0, qb1),
+                          mat(a.qkv + 2 * d, 3 * d, 1, qb0, qb1), S, S, H, B, hd, P.scores, a.P, P.ldP, a.attn_o, d, 1, 0));
   }
   // out_proj; ax = attention branch + residual x
   if (m->attn_adapter == MB200_ADAPTER_NONE) {
@@ -485,9 +370,6 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int laye
   MBS_REQUIRE(0 <= layer_lo && layer_lo <= layer_hi && layer_hi <= m->n_layer, MB200_E_ARG,
               "gptj_sched_backward: bad layer range [%d,%d)", layer_lo, layer_hi);
   const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd;
-  const float scale = 1.0f / sqrtf((float)hd);
-  const long long qb0 = hd, qb1 = (long long)S * 3 * d;
-  const long long pb0 = (long long)S * P.ldP, pb1 = (long long)H * S * P.ldP;
   ScratchScope scratch(P.gemm_ws, P.gemm_ws_bytes);
   // gradient w.r.t. the residual stream entering layer l lives in g[(l) & 1]
   bf16s* gb[2] = {P.g0, P.g1};
@@ -538,23 +420,9 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int laye
     if (tile_ok(S, hd)) {
       MBS_TRY(mb200_attn_bwd_tile(a.qkv, 3 * d, P.dattn_o, d, a.P, P.ldP, P.dqkv, 3 * d, P.rope_tab, m->rotary_dim, B, S, H,
                                   hd, st));
-    } else {
-      Mat dO = mat(P.dattn_o, d, 0, hd, (long long)S * d);
-      Mat dO_mn = mat(P.dattn_o, d, 1, hd, (long long)S * d);
-      MBS_TRY(gemm(st, S, S, hd, dO, mat(a.qkv + 2 * d, 3 * d, 0, qb0, qb1), P.scores, P.ldP, 1, Epi(), H, B, pb0, pb1));
-      MBS_TRY(gemm(st, S, hd, S, mat(a.P, P.ldP, 1, pb0, pb1), dO_mn, P.dqkv + 2 * d, 3 * d, 0, Epi(), H, B, qb0, qb1));
-      MBS_TRY(mb200_softmax_bwd(P.scores, P.ldP, pb0, a.P, P.ldP, pb0, P.dS, P.ldP, pb0, B * H, S, S, scale, st));
-      Epi er;  // dQ, dK w.r.t. the rotated q, k: inverse rotation in the epilogue
-      er.rope_tab = P.rope_tab;
-      er.rope_mode = -1;
-      er.rope_S = S;
-      er.rope_hd = hd;
-      er.rope_rot = m->rotary_dim;
-      er.rope_ncols = hd;
-      MBS_TRY(gemm(st, S, hd, S, mat(P.dS, P.ldP, 0, pb0, pb1), mat(a.qkv + d, 3 * d, 1, qb0, qb1), P.dqkv, 3 * d, 0, er, H,
-                   B, qb0, qb1));
-      MBS_TRY(gemm(st, S, hd, S, mat(P.dS, P.ldP, 1, pb0, pb1), mat(a.qkv, 3 * d, 1, qb0, qb1), P.dqkv + d, 3 * d, 0, er, H,
-                   B, qb0, qb1));
+    } else {  // dQ, dK w.r.t. the rotated q, k: inverse rotation in the epilogue
+      MBS_TRY(attn_bwd_gemm(st, a.qkv, a.P, P.dattn_o, P.dqkv, P.scores, P.dS, P.ldP, S, H, B, hd,
+                            rope_epi(P.rope_tab, -1, S, hd, m->rotary_dim, hd)));
     }
     {
       Epi e;
@@ -636,12 +504,8 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
                 MB200_E_ARG, "gptj_sched_infer: every layer must carry the same adapter options");
   const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd;
   const int Sk = kcache ? pos0 + S : S;
-  const float scale = 1.0f / sqrtf((float)hd);
   const size_t cache_layer = (size_t)B * H * Smax * hd;
-  struct SplitScope {
-    SplitScope(void* w, size_t b) { t_splitk_ws = w; t_splitk_bytes = (long long)b; }
-    ~SplitScope() { t_splitk_ws = nullptr; t_splitk_bytes = 0; }
-  } split_scope(P.splitk, P.splitk_bytes);
+  ScratchScope scratch(P.splitk, P.splitk_bytes);
   if (pos_dev) MBS_TRY(mb200_rope_table_dev(P.rope_tab, S, m->rotary_dim, pos_dev, st));
   else MBS_TRY(mb200_rope_table(P.rope_tab, S, m->rotary_dim, pos0, st));
   const bf16s* xin = x;
@@ -649,16 +513,8 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
     const mb200_gptj_layer_ex& L = m->layers[l];
     bf16s* xout = (l & 1) ? P.xb : P.xa;
     MBS_TRY(mb200_layernorm_fwd(xin, d, L.ln1_g, L.ln1_b, P.h, d, nullptr, nullptr, M, d, m->ln_eps, st));
-    {
-      Epi e;
-      e.rope_tab = P.rope_tab;
-      e.rope_mode = 1;
-      e.rope_S = S;
-      e.rope_hd = hd;
-      e.rope_rot = m->rotary_dim;
-      e.rope_ncols = 2 * d;
-      MBS_TRY(gemm(st, M, 3 * d, d, mat(P.h, d), wmat(L.w_qkv, d), P.qkv, 3 * d, 0, e));
-    }
+    MBS_TRY(gemm(st, M, 3 * d, d, mat(P.h, d), wmat(L.w_qkv, d), P.qkv, 3 * d, 0,
+                 rope_epi(P.rope_tab, 1, S, hd, m->rotary_dim, 2 * d)));
     bf16s* kc = kcache ? kcache + (size_t)l * cache_layer : nullptr;
     bf16s* vc = vcache ? vcache + (size_t)l * cache_layer : nullptr;
     if (kcache && S == 1 && pos_dev) {
@@ -686,10 +542,7 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
         Kk = mat(P.qkv + d, 3 * d, 0, hd, (long long)S * 3 * d);
         Vv = mat(P.qkv + 2 * d, 3 * d, 1, hd, (long long)S * 3 * d);
       }
-      const long long pb0 = (long long)S * P.ldS, pb1 = (long long)H * S * P.ldS;
-      MBS_TRY(gemm(st, S, Sk, hd, Q, Kk, P.scores, P.ldS, 1, Epi(), H, B, pb0, pb1));
-      MBS_TRY(mb200_softmax_fwd(P.scores, P.ldS, pb0, P.P, P.ldS, pb0, B * H, S, Sk, scale, 1, Sk - S, st));
-      MBS_TRY(gemm(st, S, hd, Sk, mat(P.P, P.ldS, 0, pb0, pb1), Vv, P.attn_o, d, 0, Epi(), H, B, hd, (long long)S * d));
+      MBS_TRY(attn_fwd_gemm(st, Q, Kk, Vv, S, Sk, H, B, hd, P.scores, P.P, P.ldS, P.attn_o, d, 1, Sk - S));
     }
     if (m->attn_adapter == MB200_ADAPTER_NONE) {
       Epi e;

@@ -15,107 +15,12 @@
 // This file contains no kernels and no CUDA calls (see sched_rt.h): tests/ dry-run it on the CPU against
 // oracle/cabi_emul.cpp. Attention (T = 257 for ViT-L/14, head_dim 64, no mask) runs in the fused multi-tile kernel
 // (mb200_attn_fwd_flash) whenever head_dim is a multiple of 64 — the training forward asks it for the probabilities
-// the materialised backward consumes — and as batched GEMMs + softmax otherwise.
+// the materialised backward consumes — and as batched GEMMs + softmax otherwise. The GEMM helpers and that
+// materialised attention are shared with gptj_sched.cu through sched_rt.h.
 #include "sched_rt.h"
-
-#include <math.h>
-#include <stdlib.h>
-#include <string.h>
 
 namespace mb200 {
 namespace {
-
-typedef uint16_t bf16s;  // bf16 storage; this file only does pointer arithmetic on it
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-struct Carver {
-  uint8_t* base;
-  size_t off;
-  explicit Carver(void* b) : base(reinterpret_cast<uint8_t*>(b)), off(0) {}
-  template <typename T>
-  T* take(size_t n) {
-    off = align_up(off, 256);
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * sizeof(T);
-    return p;
-  }
-};
-
-struct Mat {
-  const void* p;
-  long long ld, bs0, bs1;
-  int mn, frozen;
-};
-inline Mat mat(const void* p, long long ld, int mn = 0, long long bs0 = 0, long long bs1 = 0) {
-  return Mat{p, ld, bs0, bs1, mn, 0};
-}
-// a frozen weight matrix (never written by a kernel of the stream): the GEMM may fetch its first tiles ahead of the
-// programmatic dependency on the previous kernel (mb200_operand.static_data)
-inline Mat wmat(const void* p, long long ld, int mn = 0) { return Mat{p, ld, 0, 0, mn, 1}; }
-struct Epi {
-  const void* bias = nullptr;
-  int act = 0;
-  void* aux_out = nullptr;
-  const void* res1 = nullptr;
-  long long ld_res = 0;
-  int accumulate = 0;
-};
-
-// scratch lent to the GEMM core while a pass is being issued (mb200_gemm_args.splitk_ws: the fp32 per-split partial slices
-// of the GEMMs gemm.cu splits along K, e.g. the few-tile, long-K wgrads of the trainable encoder)
-const size_t kGemmScratchBytes = (size_t)128 << 20;
-thread_local void* t_gemm_ws = nullptr;
-thread_local long long t_gemm_ws_bytes = 0;
-struct ScratchScope {
-  ScratchScope(void* w, size_t b) { t_gemm_ws = w; t_gemm_ws_bytes = (long long)b; }
-  ~ScratchScope() { t_gemm_ws = nullptr; t_gemm_ws_bytes = 0; }
-};
-
-int gemm(void* st, int M, int N, int K, Mat A, Mat B, void* C, long long ldc, int c_f32, const Epi& e = Epi(),
-         int nb0 = 1, int nb1 = 1, long long c_bs0 = 0, long long c_bs1 = 0) {
-  mb200_gemm_args g;
-  memset(&g, 0, sizeof(g));
-  g.splitk_ws = t_gemm_ws;
-  g.splitk_ws_bytes = t_gemm_ws_bytes;
-  g.M = M;
-  g.N = N;
-  g.K = K;
-  g.nb0 = nb0;
-  g.nb1 = nb1;
-  g.c_dtype = c_f32 ? MB200_F32 : MB200_BF16;
-  g.A.ptr = A.p;
-  g.A.ld = A.ld;
-  g.A.bs0 = A.bs0;
-  g.A.bs1 = A.bs1;
-  g.A.mn_major = A.mn;
-  g.B.ptr = B.p;
-  g.B.ld = B.ld;
-  g.B.bs0 = B.bs0;
-  g.B.bs1 = B.bs1;
-  g.B.mn_major = B.mn;
-  g.B.static_data = B.frozen;
-  g.C = C;
-  g.ldc = ldc;
-  g.c_bs0 = c_bs0;
-  g.c_bs1 = c_bs1;
-  g.alpha = 1.f;
-  g.act = e.act;
-  g.accumulate = e.accumulate;
-  g.bias = e.bias;
-  g.aux_out = e.aux_out;
-  g.res1 = e.res1;
-  g.ld_res = e.ld_res;
-  return mb200_gemm(&g, st);
-}
-
-// wgrad of a linear y = x W^T: dW[out, in] (+)= dy^T x, both operands read MN-major from their [rows, features] storage
-int wgrad(void* st, int out, int in, int rows, const bf16s* dy, long long lddy, const bf16s* x, long long ldx, float* dW,
-          long long ldw, int accumulate) {
-  Epi e;
-  e.accumulate = accumulate;
-  return gemm(st, out, in, rows, mat(dy, lddy, 1), mat(x, ldx, 1), dW, ldw, 1, e);
-}
 
 struct LayerActs {
   bf16s* x_in;    // [M,w] residual stream entering the block
@@ -201,16 +106,6 @@ int make_plan(Plan& P, const mb200_vit_model* m, int B, void* ws) {
 
 const float kEps = 1e-5f;  // CLIP LayerNorm eps
 
-// head dims the fused multi-tile attention kernel takes (csrc/attention.cu); MB200_ATTN_FLASH=0 forces the GEMM path
-inline bool flash_ok(int hd) {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("MB200_ATTN_FLASH");
-    on = e ? atoi(e) : 1;
-  }
-  return on != 0 && hd >= 64 && hd <= 256 && hd % 64 == 0;
-}
-
 // ---------------------------------------------------------------------------------------------
 // inference forward (the image encoder is frozen on the measured path, magma/magma.py:98-100): one set of activation
 // buffers reused by every layer. Arithmetic: hf:clip/modeling_clip.py:138-219 (patch + class + position embeddings),
@@ -258,7 +153,6 @@ int forward_infer(const mb200_vit_model* m, const bf16s* images, bf16s* feats, i
               P.bytes);
   const int w = m->width, H = m->n_head, hd = w / H, T = P.T, M = P.M, g = m->image / m->patch;
   const int Kp = 3 * m->patch * m->patch;
-  const float scale = 1.0f / sqrtf((float)hd);
   ScratchScope scratch(P.gemm_ws, kGemmScratchBytes);
   // conv1 as im2col + GEMM (patch embeddings staged in h), then [cls; patches] + positional embedding
   MBS_TRY(rt_zero(P.patches, (size_t)B * g * g * P.ldpatch * sizeof(bf16s), st));
@@ -268,7 +162,6 @@ int forward_infer(const mb200_vit_model* m, const bf16s* images, bf16s* feats, i
   // ln_pre (in place: each row is cached in registers before it is rewritten)
   MBS_TRY(mb200_layernorm_fwd(P.x, w, m->ln_pre_g, m->ln_pre_b, P.x, w, nullptr, nullptr, M, w, kEps, st));
   const long long qb0 = hd, qb1 = (long long)T * 3 * w;
-  const long long pb0 = (long long)T * P.ldS, pb1 = (long long)H * T * P.ldS;
   for (int l = 0; l < m->n_layer; ++l) {
     const mb200_vit_layer& L = m->layers[l];
     MBS_TRY(mb200_layernorm_fwd(P.x, w, L.ln1_g, L.ln1_b, P.h, w, nullptr, nullptr, M, w, kEps, st));
@@ -281,11 +174,9 @@ int forward_infer(const mb200_vit_model* m, const bf16s* images, bf16s* feats, i
       MBS_TRY(mb200_attn_fwd_flash(P.qkv, 3 * w, qb0, qb1, P.qkv + w, 3 * w, qb0, qb1, P.qkv + 2 * w, 3 * w, qb0, qb1,
                                    P.attn_o, w, nullptr, 0, nullptr, B, T, T, H, hd, 0, st));
     } else {
-      MBS_TRY(gemm(st, T, T, hd, mat(P.qkv, 3 * w, 0, qb0, qb1), mat(P.qkv + w, 3 * w, 0, qb0, qb1), P.scores, P.ldS, 1,
-                   Epi(), H, B, pb0, pb1));
-      MBS_TRY(mb200_softmax_fwd(P.scores, P.ldS, pb0, P.P, P.ldS, pb0, B * H, T, T, scale, 0, 0, st));
-      MBS_TRY(gemm(st, T, hd, T, mat(P.P, P.ldS, 0, pb0, pb1), mat(P.qkv + 2 * w, 3 * w, 1, qb0, qb1), P.attn_o, w, 0,
-                   Epi(), H, B, hd, (long long)T * w));
+      MBS_TRY(attn_fwd_gemm(st, mat(P.qkv, 3 * w, 0, qb0, qb1), mat(P.qkv + w, 3 * w, 0, qb0, qb1),
+                            mat(P.qkv + 2 * w, 3 * w, 1, qb0, qb1), T, T, H, B, hd, P.scores, P.P, P.ldS, P.attn_o, w, 0,
+                            0));
     }
     {
       Epi e;
@@ -322,7 +213,6 @@ int forward_train(const mb200_vit_model* m, const bf16s* images, bf16s* feats, i
   ScratchScope scratch(P.gemm_ws, kGemmScratchBytes);
   MBS_REQUIRE(m->ld_conv % 8 == 0 && m->ld_conv >= P.Kp, MB200_E_ALIGN, "vit_forward_train: bad ld_conv");
   const int w = m->width, H = m->n_head, hd = w / H, T = P.T, M = P.M, np = B * P.g * P.g;
-  const float scale = 1.0f / sqrtf((float)hd);
   // conv1 as im2col + GEMM, then [cls; patches] + positional embedding, then ln_pre (input xa kept for its backward)
   MBS_TRY(rt_zero(P.patches, (size_t)np * P.ldpatch * sizeof(bf16s), st));
   MBS_TRY(mb200_patchify(images, P.patches, P.ldpatch, B, m->image, m->patch, st));
@@ -330,7 +220,6 @@ int forward_train(const mb200_vit_model* m, const bf16s* images, bf16s* feats, i
   MBS_TRY(mb200_vit_assemble(P.xa, P.pe, m->cls, m->pos, B, T, w, st));
   MBS_TRY(mb200_layernorm_fwd(P.xa, w, m->ln_pre_g, m->ln_pre_b, P.acts[0].x_in, w, P.mean0, P.rstd0, M, w, kEps, st));
   const long long qb0 = hd, qb1 = (long long)T * 3 * w;
-  const long long pb0 = (long long)T * P.ldS, pb1 = (long long)H * T * P.ldS;
   for (int l = 0; l < m->n_layer; ++l) {
     const mb200_vit_layer& L = m->layers[l];
     LayerActs& a = P.acts[l];
@@ -346,11 +235,9 @@ int forward_train(const mb200_vit_model* m, const bf16s* images, bf16s* feats, i
       MBS_TRY(mb200_attn_fwd_flash(a.qkv, 3 * w, qb0, qb1, a.qkv + w, 3 * w, qb0, qb1, a.qkv + 2 * w, 3 * w, qb0, qb1,
                                    a.attn_o, w, a.P, P.ldS, nullptr, B, T, T, H, hd, 0, st));
     } else {
-      MBS_TRY(gemm(st, T, T, hd, mat(a.qkv, 3 * w, 0, qb0, qb1), mat(a.qkv + w, 3 * w, 0, qb0, qb1), P.scores, P.ldS, 1,
-                   Epi(), H, B, pb0, pb1));
-      MBS_TRY(mb200_softmax_fwd(P.scores, P.ldS, pb0, a.P, P.ldS, pb0, B * H, T, T, scale, 0, 0, st));
-      MBS_TRY(gemm(st, T, hd, T, mat(a.P, P.ldS, 0, pb0, pb1), mat(a.qkv + 2 * w, 3 * w, 1, qb0, qb1), a.attn_o, w, 0,
-                   Epi(), H, B, hd, (long long)T * w));
+      MBS_TRY(attn_fwd_gemm(st, mat(a.qkv, 3 * w, 0, qb0, qb1), mat(a.qkv + w, 3 * w, 0, qb0, qb1),
+                            mat(a.qkv + 2 * w, 3 * w, 1, qb0, qb1), T, T, H, B, hd, P.scores, a.P, P.ldS, a.attn_o, w, 0,
+                            0));
     }
     {
       Epi e;
@@ -388,9 +275,6 @@ int backward(const mb200_vit_model* m, const mb200_vit_grads* G, const bf16s* df
   MBS_REQUIRE(G && G->layers && dfeats, MB200_E_ARG, "vit_backward: null gradient table / dfeats");
   ScratchScope scratch(P.gemm_ws, kGemmScratchBytes);
   const int w = m->width, H = m->n_head, hd = w / H, T = P.T, M = P.M, np = B * P.g * P.g, mlp = m->mlp;
-  const float scale = 1.0f / sqrtf((float)hd);
-  const long long qb0 = hd, qb1 = (long long)T * 3 * w;
-  const long long pb0 = (long long)T * P.ldS, pb1 = (long long)H * T * P.ldS;
 
   // ---- head: feats = ln_post(x_out[:, 0]) @ proj ----
   // dproj[w, out] (+)= pooled^T dfeats
@@ -424,21 +308,7 @@ int backward(const mb200_vit_model* m, const mb200_vit_grads* G, const bf16s* df
     MBS_TRY(wgrad(st, w, w, M, P.gmid, w, a.attn_o, w, GL.w_out, w, acc));
     MBS_TRY(mb200_colsum(P.gmid, w, M, w, GL.b_out, acc, st));
     MBS_TRY(gemm(st, M, w, w, mat(P.gmid, w), mat(L.w_out, w, 1), P.dattn_o, w, 0));  // d(attn_o) = gmid Wout
-    {
-      Mat dO = mat(P.dattn_o, w, 0, hd, (long long)T * w);
-      Mat dO_mn = mat(P.dattn_o, w, 1, hd, (long long)T * w);
-      // dP = dO V^T (fp32)
-      MBS_TRY(gemm(st, T, T, hd, dO, mat(a.qkv + 2 * w, 3 * w, 0, qb0, qb1), P.scores, P.ldS, 1, Epi(), H, B, pb0, pb1));
-      // dV = P^T dO
-      MBS_TRY(gemm(st, T, hd, T, mat(a.P, P.ldS, 1, pb0, pb1), dO_mn, P.dqkv + 2 * w, 3 * w, 0, Epi(), H, B, qb0, qb1));
-      // dS = P * (dP - rowsum(dP * P)) / sqrt(hd)
-      MBS_TRY(mb200_softmax_bwd(P.scores, P.ldS, pb0, a.P, P.ldS, pb0, P.dS, P.ldS, pb0, B * H, T, T, scale, st));
-      // dQ = dS K ; dK = dS^T Q
-      MBS_TRY(gemm(st, T, hd, T, mat(P.dS, P.ldS, 0, pb0, pb1), mat(a.qkv + w, 3 * w, 1, qb0, qb1), P.dqkv, 3 * w, 0,
-                   Epi(), H, B, qb0, qb1));
-      MBS_TRY(gemm(st, T, hd, T, mat(P.dS, P.ldS, 1, pb0, pb1), mat(a.qkv, 3 * w, 1, qb0, qb1), P.dqkv + w, 3 * w, 0,
-                   Epi(), H, B, qb0, qb1));
-    }
+    MBS_TRY(attn_bwd_gemm(st, a.qkv, a.P, P.dattn_o, P.dqkv, P.scores, P.dS, P.ldS, T, H, B, hd, Epi()));
     MBS_TRY(wgrad(st, 3 * w, w, M, P.dqkv, 3 * w, a.h1, w, GL.w_qkv, w, acc));
     MBS_TRY(mb200_colsum(P.dqkv, 3 * w, M, 3 * w, GL.b_qkv, acc, st));
     MBS_TRY(gemm(st, M, w, 3 * w, mat(P.dqkv, 3 * w), mat(L.w_qkv, w, 1), P.dh, w, 0));  // dh1 = dqkv Wqkv
