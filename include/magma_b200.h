@@ -233,7 +233,10 @@ int mb200_argmax(const void* x, int64_t ldx, int32_t rows, int32_t V, int64_t* o
 /* One sampled token per row for temperature > 0 (magma/sampling.py:97-105): top_k_filter (:22-30, off when top_k == 0),
  * top_p_filter including its inverted-nucleus comparison (:7-19, off when top_p == 0; ties ordered by index = a stable
  * sort), softmax(logits / temperature) and one multinomial draw from Philox(seed, row, offset). logits bf16 or f32
- * [rows, V] with row stride ld; keep_mask (optional, [rows, V] bytes) receives 1 where a token survives both filters. */
+ * [rows, V] with row stride ld; keep_mask (optional, [rows, V] bytes) receives 1 where a token survives both filters.
+ * -0 and +0 are equal to the order (a tie, resolved by index). NaN of either sign is read as -inf (the reference's
+ * torch.multinomial rejects such rows). A row with no finite entry in the top-k set has no distribution: its token is
+ * rank 0 of the order (the lowest index), and keep_mask is the top-k set when top_p == 0, rank 0 alone otherwise. */
 int mb200_sample(const void* logits, int32_t dtype, int64_t ld, int32_t rows, int32_t V, float temperature,
                  int32_t top_k, float top_p, uint64_t seed, uint64_t offset, int64_t* tokens, uint8_t* keep_mask,
                  void* stream);

@@ -38,7 +38,8 @@ def build(force=False):
 KX_OUT = os.path.join(OUT_DIR, "libkernel_host_exec.so")
 KX_SRC = os.path.join(ROOT, "oracle", "kernel_host_exec.cpp")
 KX_DEPS = [KX_SRC] + [os.path.join(ROOT, "magma_b200", "csrc", f) for f in ("warp_helpers.cuh", "elt_helpers.cuh",
-                                                                          "elt_kernels.cuh", "train_kernels.cuh")]
+                                                                          "elt_kernels.cuh", "train_kernels.cuh",
+                                                                          "samp_kernels.cuh")]
 
 
 def build_kernel_exec(force=False):

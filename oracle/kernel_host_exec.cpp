@@ -14,6 +14,13 @@
 #define _GNU_SOURCE  // sincosf
 #endif
 #include <cuda_bf16.h>
+// Philox4x32-10 of mb200_sample is plain arithmetic and compiles as host C++; the MTGP32 part of the header declares the
+// built-in thread indices, which this file defines itself
+#define threadIdx curand_unused_threadIdx
+#define blockDim curand_unused_blockDim
+#include <curand_kernel.h>
+#undef threadIdx
+#undef blockDim
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
@@ -99,6 +106,28 @@ static inline int __shfl_xor_sync(unsigned, int v, int o) {
   g_warp_barrier[w]->wait();
   return r;
 }
+template <typename T>
+static inline T shfl_up(T v, int o) {  // lanes below o get their own value back, as on the GPU
+  static T x[1024];
+  const int t = (int)threadIdx.x, w = t >> 5;
+  x[t] = v;
+  g_warp_barrier[w]->wait();
+  const T r = (t & 31) >= o ? x[t - o] : v;
+  g_warp_barrier[w]->wait();
+  return r;
+}
+static inline int __shfl_up_sync(unsigned, int v, int o) { return shfl_up(v, o); }
+static inline double __shfl_up_sync(unsigned, double v, int o) { return shfl_up(v, o); }
+static inline unsigned __float_as_uint(float x) {
+  unsigned u;
+  memcpy(&u, &x, 4);
+  return u;
+}
+static inline float __uint_as_float(unsigned u) {
+  float x;
+  memcpy(&x, &u, 4);
+  return x;
+}
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 template <typename T> static inline T __ldcs(const T* p) { return *p; }             // cache-streaming hints: plain accesses
 template <typename T> static inline void __stcs(T* p, const T& v) { *p = v; }
@@ -114,6 +143,18 @@ static inline unsigned int atomicAdd(unsigned int* p, unsigned int v) {
   std::lock_guard<std::mutex> lk(g_atomic);
   const unsigned int old = *p;
   *p = old + v;
+  return old;
+}
+static inline double atomicAdd(double* p, double v) {
+  std::lock_guard<std::mutex> lk(g_atomic);
+  const double old = *p;
+  *p = old + v;
+  return old;
+}
+static inline int atomicMin(int* p, int v) {
+  std::lock_guard<std::mutex> lk(g_atomic);
+  const int old = *p;
+  if (v < old) *p = v;
   return old;
 }
 static inline void __threadfence() {}  // blocks run one after another here, threads of a block meet at barriers
@@ -159,6 +200,7 @@ typedef __nv_bfloat16 bf16;
 #include "../magma_b200/csrc/elt_helpers.cuh"
 #include "../magma_b200/csrc/elt_kernels.cuh"
 #include "../magma_b200/csrc/train_kernels.cuh"
+#include "../magma_b200/csrc/samp_kernels.cuh"
 }  // namespace mb200
 
 using namespace mb200;
@@ -439,6 +481,34 @@ int mb200_bn_bwd_coeffs(const float* s1, const float* t, const float* mean, cons
   run_grid(Dim3{(unsigned)((C + 127) / 128), 1, 1}, 128, [&] {
     bn_bwd_coeffs_kernel(s1, t, mean, rstd, gamma, (float)(1.0 / (double)rows), dgamma, dbeta, accumulate, A, Bc, Cc, C);
   });
+  return 0;
+}
+// curand_uniform after curand_init(seed, subsequence, offset), for the Python restatement of the draw in the tests
+float hx_curand_uniform(unsigned long long seed, unsigned long long subsequence, unsigned long long offset) {
+  curandStatePhilox4_32_10_t st;
+  curand_init(seed, subsequence, offset, &st);
+  return curand_uniform(&st);
+}
+// sampling.cu and the gradient exchange: the kernels only, without the argument checks of the host wrappers
+int mb200_sample(const void* logits, int32_t dtype, int64_t ld, int32_t rows, int32_t V, float temperature, int32_t top_k,
+                 float top_p, uint64_t seed, uint64_t offset, int64_t* tokens, uint8_t* keep_mask, void*) {
+  run_grid(Dim3{(unsigned)rows, 1, 1}, kSampThreads, [&] {
+    if (dtype == 1)
+      sample_kernel<float>((const float*)logits, ld, V, 1.f / temperature, top_k, top_p, seed, offset, (long long*)tokens,
+                           keep_mask);
+    else
+      sample_kernel<bf16>((const bf16*)logits, ld, V, 1.f / temperature, top_k, top_p, seed, offset, (long long*)tokens,
+                          keep_mask);
+  });
+  return 0;
+}
+int mb200_peer_reduce_bcast(void* const* bufs, int32_t world, int64_t offset, int64_t n, int32_t max_blocks, void*) {
+  if (n == 0) return 0;
+  PeerBufs pb;
+  for (int r = 0; r < 16; ++r) pb.p[r] = r < world ? reinterpret_cast<float*>(bufs[r]) : nullptr;
+  int grid = grid_for(n / 4, 256);
+  if (max_blocks > 0 && grid > max_blocks) grid = max_blocks;
+  run_grid(Dim3{(unsigned)grid, 1, 1}, 256, [&] { peer_reduce_bcast_kernel(pb, world, offset / 4, n / 4); });
   return 0;
 }
 const char* mb200_last_error(void) { return ""; }
