@@ -120,6 +120,7 @@ typedef struct {
   const void* res2;   /* bf16 [M,N], row stride ld_res, batch strides as C, or NULL */
   int64_t ld_res;
   int32_t force_bn;   /* 0 = auto tile width (and split-K plan), else 64, 128 or 256 (no split-K) — testing / tuning */
+  int32_t generic_epilogue; /* non-zero: run the runtime epilogue form even when a compiled form matches — testing */
   /* fused rotary embedding (rotate_every_two, hf:gptj/modeling_gptj.py:57-67) applied to adjacent column pairs after
    * the bias: for columns c < rope_ncols with (c % rope_hd) < rope_rot, using (cos, sin) = rope_tab[row % rope_S]
    * [(c % rope_hd)/2] (fp32 pairs, mb200_rope_table). rope_mode +1 = forward, -1 = inverse; rope_tab NULL = off. */

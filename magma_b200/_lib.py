@@ -52,6 +52,7 @@ class GemmArgs(ctypes.Structure):
         ("res2", ctypes.c_void_p),
         ("ld_res", ctypes.c_int64),
         ("force_bn", ctypes.c_int32),
+        ("generic_epilogue", ctypes.c_int32),
         ("rope_mode", ctypes.c_int32),
         ("rope_tab", ctypes.c_void_p),
         ("rope_S", ctypes.c_int32),

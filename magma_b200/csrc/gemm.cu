@@ -9,7 +9,8 @@
 //   * warp-specialised: warpgroup 0 = TMA producer (one lane, registers handed to the consumers with setmaxnreg),
 //     warpgroups 1 and 2 = consumers, each owning 64 rows of the 128-row tile: wgmma.mma_async m64nBNk16 with fp32
 //     accumulators in registers, then the fused epilogue, staged through shared memory 64 columns at a time so that
-//     one rolled copy of its code reads and writes global memory in contiguous row segments (gemm_common.cuh);
+//     one copy of its code, compiled per epilogue form, reads and writes global memory in contiguous row segments
+//     (gemm_common.cuh);
 //   * operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a multi-stage smem ring,
 //     completion tracked with mbarriers; a consumer releases a slot once the wgmma reading it has retired;
 //   * both operand majors (K-major and MN-major) are supported through the wgmma shared-memory descriptors and the
@@ -31,7 +32,8 @@ struct EpiMaps {
 template <>
 struct EpiMaps<false> {};
 
-template <int BN, bool A_MN, bool B_MN, bool EPI_TMA>
+// FORM: the epilogue form (gemm_common.cuh) the kernel is compiled for.
+template <int BN, bool A_MN, bool B_MN, bool EPI_TMA, uint32_t FORM = EF_RUNTIME>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ EpiMaps<EPI_TMA> tmE, const __grid_constant__ GemmKernelParams p) {
@@ -39,8 +41,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr int kStages = C_::kStages;
 
   extern __shared__ uint8_t smem_raw[];
-  // SWIZZLE_128B atoms need 1024-byte alignment
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // SWIZZLE_128B atoms need 1024-byte alignment. An offset on the array, not a rounded integer address: the compiler
+  // then still knows everything derived from it is shared memory (LDS / STS for the epilogue staging, not generic).
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * C_::kABytes;
   float* epi_stage = reinterpret_cast<float*>(smem + kStages * C_::kStageBytes);
@@ -163,8 +166,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>();
       if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
       const long long boff = (long long)z0 * p.c_bs0 + (long long)z1 * p.c_bs1;
-      epi_tile<BN, EPI_TMA>(p, acc, epi_stage + cw * 64 * kEpiCols, 1 + cw, boff, m_blk * BM + cw * 64, n_blk * BN, ks, ring,
-                   stage, phase);
+      epi_tile<BN, EPI_TMA, EpiForm<FORM>>(p, acc, epi_stage + cw * 64 * kEpiCols, 1 + cw, boff, m_blk * BM + cw * 64,
+                                           n_blk * BN, ks, ring, stage, phase);
     }
   }
 }
@@ -188,10 +191,12 @@ __global__ void splitk_finalize_kernel(const GemmKernelParams p) {
       v[2] += w4.z;
       v[3] += w4.w;
     }
+    using Form = EpiForm<EF_RUNTIME>;
+    float bias[4];
     EpiIn in;
-    if (p.bias) ld_bf16x4(p.bias + col, min(4, p.N - col), in.bias);
-    epi_load_inputs(p, 0, row, col, in);
-    epi_store4(p, 0, row, col, v, in);
+    if (p.bias) ld_bf16x4(p.bias + col, min(4, p.N - col), bias);
+    epi_load_inputs<Form>(p, 0, row, col, in);
+    epi_store4<Form>(p, 0, row, col, v, bias, in);
   }
 }
 
@@ -260,10 +265,10 @@ int make_operand_map(CUtensorMap* out, const mb200_operand& op, int rows, int K,
   return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, bool EPI_TMA>
+template <int BN, bool A_MN, bool B_MN, bool EPI_TMA, uint32_t FORM = EF_RUNTIME>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiMaps<true>& tmE,
                        const GemmKernelParams& kp, cudaStream_t stream) {
-  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI_TMA>;
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI_TMA, FORM>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes));
@@ -309,6 +314,46 @@ static int dispatch_bn(int bn, bool a_mn, bool b_mn, const CUtensorMap& tmA, con
       return epi ? dispatch_major<256, true>(a_mn, b_mn, tmA, tmB, tmE, kp, s)
                  : dispatch_major<256, false>(a_mn, b_mn, tmA, tmB, tmE, kp, s);
   }
+}
+
+// The compiled epilogue forms: the feature sets the GEMMs of a GPT-J training step with MLP adapters launch at the
+// 256-wide tile, each for the operand majors it is launched with. Returns false when (form, majors) is not one of them.
+template <uint32_t F, bool A_MN, bool B_MN>
+static bool launch_form(uint32_t form, bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                        const EpiMaps<true>& tmE, const GemmKernelParams& kp, cudaStream_t s, int* rc) {
+  if (form != F || a_mn != A_MN || b_mn != B_MN) return false;
+  *rc = launch_gemm<256, A_MN, B_MN, EpiForm<F>::kInputs != 0, F>(tmA, tmB, tmE, kp, s);
+  return true;
+}
+static bool dispatch_form(uint32_t form, bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                          const EpiMaps<true>& tmE, const GemmKernelParams& kp, cudaStream_t s, int* rc) {
+#define MB_FORM(F, A_MN, B_MN) launch_form<(F), A_MN, B_MN>(form, a_mn, b_mn, tmA, tmB, tmE, kp, s, rc)
+  return MB_FORM(EF_ROPE, false, false) ||                           // qkv forward
+         MB_FORM(EF_RES1, false, false) ||                           // attention out forward
+         MB_FORM(EF_BIAS | EF_GELU | EF_AUX_OUT, false, false) ||    // fc_in forward
+         MB_FORM(EF_BIAS, false, false) ||                           // fc_out forward, LM head
+         MB_FORM(EF_BIAS | EF_RES1 | EF_RES2, false, false) ||       // adapter up
+         MB_FORM(EF_DGELU, false, true) ||                           // fc_out dgrad
+         MB_FORM(0u, false, true) ||                                 // fc_in, attention out and LM-head dgrad
+         MB_FORM(EF_RES1, false, true) ||                            // qkv dgrad, adapter dgrad-down
+         MB_FORM(EF_F32, true, true);                                // adapter wgrads
+#undef MB_FORM
+}
+
+// The compiled form a launch qualifies for, or EF_RUNTIME: its features must all be ones a form can express, every
+// [M, N] input staged by TMA (kp.epi_in), and bias and aux_out 8-byte aligned, which with the alignment gemm_impl
+// requires of C, ldc and the batch strides makes every 4-column access of a compiled form a vector.
+static uint32_t epi_form(const mb200_gemm_args* a, const GemmKernelParams& kp, int bn) {
+  if (a->generic_epilogue || bn != 256) return EF_RUNTIME;
+  if ((a->act != MB200_ACT_NONE && a->act != MB200_ACT_GELU_NEW) ||
+      (a->dact != MB200_DACT_NONE && a->dact != MB200_DACT_GELU_NEW))
+    return EF_RUNTIME;
+  if (((reinterpret_cast<uintptr_t>(a->bias) | reinterpret_cast<uintptr_t>(a->aux_out)) & 7) != 0) return EF_RUNTIME;
+  const uint32_t f = (a->bias ? EF_BIAS : 0u) | (kp.rope_mode ? EF_ROPE : 0u) | (a->aux_out ? EF_AUX_OUT : 0u) |
+                     (a->act ? EF_GELU : 0u) | (a->dact ? EF_DGELU : 0u) | (a->res1 ? EF_RES1 : 0u) |
+                     (a->res2 ? EF_RES2 : 0u) | (kp.c_f32 ? EF_F32 : 0u);
+  const int inputs = (a->dact != 0) + (a->res1 != nullptr) + (a->res2 != nullptr);
+  return kp.epi_in == inputs ? f : EF_RUNTIME;
 }
 
 // Tensor maps for the epilogue's [M, N] inputs (aux_in when dact, res1, res2), fetched by the producer through the
@@ -538,6 +583,7 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
   kp.total_tiles = tiles_m * kp.tiles_n * a->nb0 * a->nb1;
   rc = make_epi_maps(&tmE, &kp, a);
   if (rc) return rc;
+  if (dispatch_form(epi_form(a, kp, bn), amn, bmn, tmA, tmB, tmE, kp, stream, &rc)) return rc;
   return dispatch_bn(bn, amn, bmn, tmA, tmB, tmE, kp, stream);
 }
 

@@ -1,6 +1,8 @@
 // magma_b200 — pieces shared by the GEMM core (gemm.cu) and the fused attention kernels (attention.cu): tile
 // configuration, kernel parameter block and the fused epilogue applied to wgmma accumulator fragments.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace mb200 {
@@ -71,9 +73,11 @@ __device__ __forceinline__ uint32_t f32x2_to_bf16(float a, float b) {
 }
 
 // n (<= 4) consecutive bf16 -> fp32 (missing elements read as 0): one 8-byte read-only load when all four are in range
-// and 8-byte aligned (operand pointers other than C carry no alignment guarantee beyond the element).
+// and 8-byte aligned (operand pointers other than C carry no alignment guarantee beyond the element). kVec: the caller
+// knows both hold, and only the vector access is compiled.
+template <bool kVec = false>
 __device__ __forceinline__ void ld_bf16x4(const bf16* src, int n, float (&v)[4]) {
-  if (n == 4 && (reinterpret_cast<uintptr_t>(src) & 7) == 0) {
+  if (kVec || (n == 4 && (reinterpret_cast<uintptr_t>(src) & 7) == 0)) {
     uint32_t u0, u1;
     asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(u0), "=r"(u1) : "l"(src));
     const float2 a = bf16x2_to_f32(u0), b = bf16x2_to_f32(u1);
@@ -86,8 +90,9 @@ __device__ __forceinline__ void ld_bf16x4(const bf16* src, int n, float (&v)[4])
     for (int e = 0; e < 4; ++e) v[e] = e < n ? __bfloat162float(src[e]) : 0.f;
   }
 }
+template <bool kVec = false>
 __device__ __forceinline__ void st_bf16x4(bf16* dst, int n, const float (&v)[4]) {
-  if (n == 4 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+  if (kVec || (n == 4 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0)) {
     *reinterpret_cast<uint2*>(dst) = make_uint2(f32x2_to_bf16(v[0], v[1]), f32x2_to_bf16(v[2], v[3]));
   } else {
 #pragma unroll
@@ -102,19 +107,67 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 
 enum { EK_GENERIC = 0, EK_SPLITK };
 
-// Epilogue inputs of one 4-column group: bias, aux_in, res1, res2. A field is filled only when its input is in use.
+// ---------------------------------------------------------------------------------------------
+// Epilogue form: which features the epilogue of a kernel instantiation is compiled for. The epilogue code below asks
+// the form, not GemmKernelParams, whether a feature is in use. EF_RUNTIME answers every question from the parameters
+// (any feature set, any alignment; also what the split-K kernels run). Any other form is a fixed set of EF_ bits and
+// answers from constants, so the code of the features it lacks is not generated, every access is a vector (the host
+// checks the alignments, epi_form in gemm.cu) and the row loop can be unrolled. Values (alpha, the rotary direction,
+// whether an fp32 store accumulates) stay parameters in every form.
+// ---------------------------------------------------------------------------------------------
+enum : uint32_t {
+  EF_BIAS = 1,
+  EF_ROPE = 2,
+  EF_AUX_OUT = 4,
+  EF_GELU = 8,    // act == MB200_ACT_GELU_NEW
+  EF_DGELU = 16,  // dact == MB200_DACT_GELU_NEW
+  EF_RES1 = 32,
+  EF_RES2 = 64,
+  EF_F32 = 128,
+  EF_RUNTIME = 1u << 31
+};
+
+template <uint32_t F>
+struct EpiForm {
+  static constexpr bool kRuntime = F == EF_RUNTIME;
+  // [M, N] inputs (aux_in, res1, res2) of a compiled form; all of them are staged by TMA
+  static constexpr int kInputs = kRuntime ? 0 : ((F & EF_DGELU) != 0) + ((F & EF_RES1) != 0) + ((F & EF_RES2) != 0);
+  // Rows of a chunk in flight per thread: the accumulators (BN / 2 registers) are live until the last chunk is staged,
+  // which leaves room for 8 rows of fp32 values and their inputs at BN = 256.
+  static constexpr int kRows = kRuntime ? 1 : 8;
+  using P = GemmKernelParams;
+  static __device__ __forceinline__ bool bias(const P& p) { return kRuntime ? p.bias != nullptr : (F & EF_BIAS) != 0; }
+  static __device__ __forceinline__ bool rope(const P& p) { return kRuntime ? p.rope_mode != 0 : (F & EF_ROPE) != 0; }
+  static __device__ __forceinline__ bool aux_out(const P& p) {
+    return kRuntime ? p.aux_out != nullptr : (F & EF_AUX_OUT) != 0;
+  }
+  static __device__ __forceinline__ int act(const P& p) {
+    return kRuntime ? p.act : (F & EF_GELU) ? MB200_ACT_GELU_NEW : MB200_ACT_NONE;
+  }
+  static __device__ __forceinline__ int dact(const P& p) {
+    return kRuntime ? p.dact : (F & EF_DGELU) ? MB200_DACT_GELU_NEW : MB200_DACT_NONE;
+  }
+  static __device__ __forceinline__ bool res1(const P& p) { return kRuntime ? p.res1 != nullptr : (F & EF_RES1) != 0; }
+  static __device__ __forceinline__ bool res2(const P& p) { return kRuntime ? p.res2 != nullptr : (F & EF_RES2) != 0; }
+  static __device__ __forceinline__ bool c_f32(const P& p) { return kRuntime ? p.c_f32 != 0 : (F & EF_F32) != 0; }
+  static __device__ __forceinline__ bool accumulate(const P& p) { return (kRuntime || (F & EF_F32)) && p.accumulate; }
+  static __device__ __forceinline__ bool splitk(const P& p) { return kRuntime && p.epi_kind == EK_SPLITK; }
+};
+
+// [M, N] epilogue inputs of one 4-column group: aux_in, res1, res2. A field is filled only when its input is in use.
 struct EpiIn {
-  float bias[4], aux[4], res1[4], res2[4];
+  float aux[4], res1[4], res2[4];
 };
 
 // aux_in / res1 / res2 of columns [col, col + 4) of one row, from global memory
+template <class Form>
 __device__ __forceinline__ void epi_load_inputs(const GemmKernelParams& p, long long boff, int row, int col,
                                                 EpiIn& in) {
   const int n = min(4, p.N - col);
-  if (p.dact) ld_bf16x4(p.aux_in + boff + (long long)row * p.ldc + col, n, in.aux);
+  if (Form::dact(p)) ld_bf16x4(p.aux_in + boff + (long long)row * p.ldc + col, n, in.aux);
   const long long roff = boff + (long long)row * p.ld_res + col;
-  if (p.res1) ld_bf16x4(p.res1 + roff, n, in.res1);
-  if (p.res2) ld_bf16x4(p.res2 + roff, n, in.res2);
+  if (Form::res1(p)) ld_bf16x4(p.res1 + roff, n, in.res1);
+  if (Form::res2(p)) ld_bf16x4(p.res2 + roff, n, in.res2);
 }
 
 // 4 bf16 of a TMA-staged epilogue box -> fp32 (8-byte aligned; columns past N were zero-filled by TMA)
@@ -129,19 +182,21 @@ __device__ __forceinline__ void ld_smem_bf16x4(const uint8_t* src, float (&v)[4]
 
 // ---------------------------------------------------------------------------------------------
 // Fused epilogue of columns [col, col + 4) of one output row (col % 4 == 0, col < N, row < M); v holds alpha x the
-// accumulators (or the summed split-K partials), `in` the group's inputs. Applied in this order: bias, rotary, saved
-// pre-activation (aux_out), activation, activation derivative (aux_in), residuals, ReLU-post, store (bf16, fp32 or
+// accumulators (or the summed split-K partials), `bias` and `in` the group's inputs. Applied in this order: bias, rotary,
+// saved pre-activation (aux_out), activation, activation derivative (aux_in), residuals, ReLU-post, store (bf16, fp32 or
 // fp32 accumulate). rope_hd, rope_rot and rope_ncols are multiples of 4, so both rotary pairs (col, col + 1),
 // (col + 2, col + 3) of the group are rotated or neither is. Every branch on p is uniform across the kernel.
+// kVec: all four columns exist and every tensor written is 8-byte aligned at them (see ld_bf16x4).
 // ---------------------------------------------------------------------------------------------
+template <class Form, bool kVec = false>
 __device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long boff, int row, int col, float (&v)[4],
-                                           const EpiIn& in) {
+                                           const float (&bias)[4], const EpiIn& in) {
   const int n = min(4, p.N - col);
-  if (p.bias) {
+  if (Form::bias(p)) {
 #pragma unroll
-    for (int e = 0; e < 4; ++e) v[e] += in.bias[e];
+    for (int e = 0; e < 4; ++e) v[e] += bias[e];
   }
-  if (p.rope_mode != 0 && col < p.rope_ncols) {
+  if (Form::rope(p) && col < p.rope_ncols) {
     const int dim = col % p.rope_hd;
     if (dim < p.rope_rot) {
       const float2* tp = p.rope_tab + (long long)(row % p.rope_S) * (p.rope_rot >> 1) + (dim >> 1);
@@ -155,35 +210,35 @@ __device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long 
     }
   }
   const long long coff = boff + (long long)row * p.ldc + col;
-  if (p.aux_out) st_bf16x4(p.aux_out + coff, n, v);
+  if (Form::aux_out(p)) st_bf16x4<kVec>(p.aux_out + coff, n, v);
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
-    if (p.act == MB200_ACT_GELU_NEW) v[e] = gelu_new_f(v[e]);
-    else if (p.act == MB200_ACT_QUICK_GELU) v[e] = quick_gelu_f(v[e]);
-    else if (p.act == MB200_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
+    if (Form::act(p) == MB200_ACT_GELU_NEW) v[e] = gelu_new_f(v[e]);
+    else if (Form::act(p) == MB200_ACT_QUICK_GELU) v[e] = quick_gelu_f(v[e]);
+    else if (Form::act(p) == MB200_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
   }
-  if (p.dact) {
+  if (Form::dact(p)) {
 #pragma unroll
     for (int e = 0; e < 4; ++e)
-      v[e] = p.dact == MB200_DACT_GELU_NEW ? v[e] * gelu_new_grad_f(in.aux[e]) : (in.aux[e] > 0.f ? v[e] : 0.f);
+      v[e] = Form::dact(p) == MB200_DACT_GELU_NEW ? v[e] * gelu_new_grad_f(in.aux[e]) : (in.aux[e] > 0.f ? v[e] : 0.f);
   }
-  if (p.res1) {
+  if (Form::res1(p)) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) v[e] += in.res1[e];
   }
-  if (p.res2) {
+  if (Form::res2(p)) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) v[e] += in.res2[e];
   }
-  if (p.act == MB200_ACT_RELU_POST) {
+  if (Form::act(p) == MB200_ACT_RELU_POST) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) v[e] = fmaxf(v[e], 0.f);
   }
-  if (p.c_f32) {  // C is 16-byte aligned and ldc, the batch strides and col are multiples of 4
+  if (Form::c_f32(p)) {  // C is 16-byte aligned and ldc, the batch strides and col are multiples of 4
     float* dst = reinterpret_cast<float*>(p.C) + coff;
-    if (n == 4) {
+    if (kVec || n == 4) {
       float4 o = make_float4(v[0], v[1], v[2], v[3]);
-      if (p.accumulate) {
+      if (Form::accumulate(p)) {
         const float4 old = *reinterpret_cast<const float4*>(dst);
         o.x += old.x;
         o.y += old.y;
@@ -194,10 +249,10 @@ __device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long 
     } else {
 #pragma unroll
       for (int e = 0; e < 4; ++e)
-        if (e < n) dst[e] = p.accumulate ? dst[e] + v[e] : v[e];
+        if (e < n) dst[e] = Form::accumulate(p) ? dst[e] + v[e] : v[e];
     }
   } else {
-    st_bf16x4(reinterpret_cast<bf16*>(p.C) + coff, n, v);
+    st_bf16x4<kVec>(reinterpret_cast<bf16*>(p.C) + coff, n, v);
   }
 }
 
@@ -206,7 +261,9 @@ __device__ __forceinline__ void epi_store4(const GemmKernelParams& p, long long 
 // fragment chunk is written to the warpgroup's 64 x 64 fp32 slice of the staging buffer; after a barrier over the
 // warpgroup, a rolled loop hands each thread groups of 4 consecutive columns of a row (16 threads per row), so a warp's
 // global loads and stores cover two contiguous 128-byte (bf16) or 256-byte (fp32) row segments, and one copy of the
-// feature code serves every chunk. Staging layout: row-major, 16-byte chunk q of row r stored at q ^ 2 (r & 3). A
+// feature code serves every chunk. In the runtime form that loop takes one row per pass; in a compiled form (EpiForm) it
+// takes Form::kRows rows, reading the staged values and inputs of all of them before the arithmetic and the stores, so
+// that many independent load -> convert -> store chains are in flight per thread. Staging layout: row-major, 16-byte chunk q of row r stored at q ^ 2 (r & 3). A
 // half-warp's 8-byte fragment writes (4 rows x 2 chunks) and a quarter-warp's 16-byte reads (8 chunks of one row) then
 // fall on distinct banks.
 // Split-K work items store alpha x the fp32 tile into their slice of the workspace instead (EK_SPLITK).
@@ -239,7 +296,7 @@ __device__ __forceinline__ uint8_t* epi_box(const EpiRing& ring, int s, int k) {
   return k == 0 ? ring.a + s * Cfg<BN>::kABytes : ring.b + s * Cfg<BN>::kBBytes + (k - 1) * kEpiBoxBytes;
 }
 
-template <int BN, bool EPI_TMA>
+template <int BN, bool EPI_TMA, class Form>
 __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float (&acc)[BN / 2], float* stage,
                                          int bar_id, long long boff, int row0, int col0, int ks, const EpiRing& ring,
                                          int& ring_stage, uint32_t& ring_phase) {
@@ -249,7 +306,7 @@ __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float 
   const int fq = wt & 3;
   const int pr = wt >> 4, pc = wt & 15;  // processing: rows pr + 8 i, 16-byte chunk pc
   const int nch = epi_chunks<BN>(p, col0);
-  const int nin = EPI_TMA ? p.epi_in : 0;
+  const int nin = !EPI_TMA ? 0 : Form::kRuntime ? p.epi_in : Form::kInputs;
   // cursor over the staged boxes: the next one is slot bk of stage bs (phase bph); stages before rs are released
   int bs = ring_stage, bk = 0, rs = ring_stage;
   uint32_t bph = ring_phase;
@@ -291,32 +348,54 @@ __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, const float 
     // this chunk's input boxes, in epi_in order: aux_in (dact), res1, res2
     const uint8_t *src_aux = nullptr, *src_res1 = nullptr, *src_res2 = nullptr;
     if (nin) {
-      if (p.dact) src_aux = next_box() + box_off;
-      if (p.res1) src_res1 = next_box() + box_off;
-      if (p.res2) src_res2 = next_box() + box_off;
+      if (Form::dact(p)) src_aux = next_box() + box_off;
+      if (Form::res1(p)) src_res1 = next_box() + box_off;
+      if (Form::res2(p)) src_res2 = next_box() + box_off;
     }
-    EpiIn in;
-    if (p.bias && col < p.N) ld_bf16x4(p.bias + col, min(4, p.N - col), in.bias);
+    const int n = min(4, p.N - col);
+    float bias[4];
+    if (Form::bias(p) && col < p.N) ld_bf16x4(p.bias + col, n, bias);
+    // rows pr + 8 i, i in [i0, i0 + kRows), of this thread's column group
+    auto rows = [&](auto rows_c, auto vec_c, int i0) {
+      constexpr int kRows = decltype(rows_c)::value;
+      constexpr bool kVec = decltype(vec_c)::value;
+      float4 s[kRows];
+      EpiIn in[kRows];
+#pragma unroll
+      for (int u = 0; u < kRows; ++u) {
+        const int i = i0 + u, r = pr + 8 * i;
+        s[u] = *reinterpret_cast<const float4*>(stage + r * kEpiCols + ((pc ^ ((r & 3) << 1)) * 4));
+        if (nin) {
+          if (Form::dact(p)) ld_smem_bf16x4(src_aux + i * 1024, in[u].aux);
+          if (Form::res1(p)) ld_smem_bf16x4(src_res1 + i * 1024, in[u].res1);
+          if (Form::res2(p)) ld_smem_bf16x4(src_res2 + i * 1024, in[u].res2);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kRows; ++u) {
+        const int row = row0 + pr + 8 * (i0 + u);
+        if (row >= p.M) continue;
+        // __fmul_rn: never fused into the add of a following feature, so every form rounds alpha x acc on its own
+        float v[4] = {__fmul_rn(s[u].x, p.alpha), __fmul_rn(s[u].y, p.alpha), __fmul_rn(s[u].z, p.alpha),
+                      __fmul_rn(s[u].w, p.alpha)};
+        if (Form::splitk(p)) {  // ld_ws % 4 == 0: the padded columns of the group exist
+          *reinterpret_cast<float4*>(p.splitk_ws + ((long long)ks * p.M + row) * p.ld_ws + col) =
+              make_float4(v[0], v[1], v[2], v[3]);
+          continue;
+        }
+        if (!nin) epi_load_inputs<Form>(p, boff, row, col, in[u]);
+        epi_store4<Form, kVec>(p, boff, row, col, v, bias, in[u]);
+      }
+    };
+    if (col < p.N) {
+      if (Form::kRuntime || n == 4) {
 #pragma unroll 1
-    for (int i = 0; i < 64 / 8; ++i) {
-      const int r = pr + 8 * i;
-      const int row = row0 + r;
-      if (row >= p.M || col >= p.N) continue;
-      const float4 s = *reinterpret_cast<const float4*>(stage + r * kEpiCols + ((pc ^ ((r & 3) << 1)) * 4));
-      float v[4] = {s.x * p.alpha, s.y * p.alpha, s.z * p.alpha, s.w * p.alpha};
-      if (p.epi_kind == EK_SPLITK) {  // ld_ws % 4 == 0: the padded columns of the group exist
-        *reinterpret_cast<float4*>(p.splitk_ws + ((long long)ks * p.M + row) * p.ld_ws + col) =
-            make_float4(v[0], v[1], v[2], v[3]);
-        continue;
+        for (int i0 = 0; i0 < 64 / 8; i0 += Form::kRows)
+          rows(std::integral_constant<int, Form::kRows>(), std::integral_constant<bool, !Form::kRuntime>(), i0);
+      } else {  // compiled form, the ragged group at the right edge of an N that is not a multiple of 4: guarded accesses
+#pragma unroll 1
+        for (int i0 = 0; i0 < 64 / 8; ++i0) rows(std::integral_constant<int, 1>(), std::false_type(), i0);
       }
-      if (nin) {
-        if (p.dact) ld_smem_bf16x4(src_aux + i * 1024, in.aux);
-        if (p.res1) ld_smem_bf16x4(src_res1 + i * 1024, in.res1);
-        if (p.res2) ld_smem_bf16x4(src_res2 + i * 1024, in.res2);
-      } else {
-        epi_load_inputs(p, boff, row, col, in);
-      }
-      epi_store4(p, boff, row, col, v, in);
     }
     named_bar_sync(bar_id, 128);  // the slice is rewritten by the next chunk; the items read so far may be refilled
     if (nin) {

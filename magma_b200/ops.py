@@ -52,6 +52,7 @@ def gemm(
     res2=None,
     accumulate=False,
     force_bn=0,
+    generic_epilogue=False,
     rope_tab=None,
     rope_mode=0,
     rope_S=0,
@@ -120,6 +121,7 @@ def gemm(
             ld_res = m[2]
     g.ld_res = ld_res
     g.force_bn = force_bn
+    g.generic_epilogue = int(bool(generic_epilogue))
     if rope_tab is not None and rope_mode:
         g.rope_tab, g.rope_mode = rope_tab.data_ptr(), int(rope_mode)
         g.rope_S, g.rope_hd, g.rope_rot, g.rope_ncols = int(rope_S), int(rope_hd), int(rope_rot), int(rope_ncols)

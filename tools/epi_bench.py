@@ -76,13 +76,15 @@ def main():
             kw["splitk_ws"] = torch.empty(32 << 20, device=dev, dtype=torch.float32)
         us = timed(lambda i: ops.gemm(A, Bs[i % nbuf], out=C, **kw), max(8, 2 * nbuf), s)
         tf = 2.0 * M * N * K / us / 1e6
-        ref = ""
+        # the same launch on the runtime epilogue form (the same kernel when no compiled form matches the case)
+        us_rt = timed(lambda i: ops.gemm(A, Bs[i % nbuf], out=C, generic_epilogue=True, **kw), max(8, 2 * nbuf), s)
+        ref = f"  runtime form {us_rt:8.1f} us"
         if cublas:  # torch.matmul on the same operands (no epilogue): the rate this card reaches at this shape
             Ct = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
             Af = A.t() if a_mn else A
             us_ref = timed(lambda i: torch.matmul(Af, Bs[i % nbuf] if b_mn else Bs[i % nbuf].t(), out=Ct),
                            max(8, 2 * nbuf), s)
-            ref = f"  cuBLAS {us_ref:8.1f} us {2.0 * M * N * K / us_ref / 1e6:7.1f} TFLOP/s"
+            ref += f"  cuBLAS {us_ref:8.1f} us {2.0 * M * N * K / us_ref / 1e6:7.1f} TFLOP/s"
         err = float("nan")
         if check:
             ops.gemm(A, Bs[0], out=C, **kw)
