@@ -134,6 +134,8 @@ typedef struct {
 } mb200_gemm_args;
 
 int mb200_gemm(const mb200_gemm_args* args, void* stream);
+/* The plan of the calling thread's last successful mb200_gemm: tile width and K splits (1 = none). For tests and tools. */
+int mb200_gemm_last_plan(int32_t* bn, int32_t* split_k);
 
 
 /* -------------------------------------------------------------------------------------------

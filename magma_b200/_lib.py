@@ -175,7 +175,7 @@ def _setup_signatures(L):
 
 
 EXPORTED_SYMBOLS = [
-    "mb200_version", "mb200_last_error", "mb200_check_device", "mb200_gemm",
+    "mb200_version", "mb200_last_error", "mb200_check_device", "mb200_gemm", "mb200_gemm_last_plan",
     "mb200_launch_count", "mb200_prof_enable", "mb200_prof_read",
     "mb200_layernorm_fwd", "mb200_layernorm_bwd", "mb200_layernorm_param_grad", "mb200_rope", "mb200_rope_table",
     "mb200_softmax_fwd", "mb200_softmax_bwd", "mb200_build_labels", "mb200_embed_assemble", "mb200_embed_gather",

@@ -316,23 +316,26 @@ static int dispatch_bn(int bn, bool a_mn, bool b_mn, const CUtensorMap& tmA, con
   }
 }
 
-// The compiled epilogue forms: the feature sets the GEMMs of a GPT-J training step with MLP adapters launch at the
-// 256-wide tile, each for the operand majors it is launched with. Returns false when (form, majors) is not one of them.
+// The compiled epilogue forms: the feature sets the GEMMs of a GPT-J training step with MLP adapters and of the ViT-L/14
+// forward launch at the 256-wide tile, each for the operand majors it is launched with. Returns false when (form,
+// majors) is not one of them; with kp == nullptr only answers whether it is.
 template <uint32_t F, bool A_MN, bool B_MN>
 static bool launch_form(uint32_t form, bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                        const EpiMaps<true>& tmE, const GemmKernelParams& kp, cudaStream_t s, int* rc) {
+                        const EpiMaps<true>& tmE, const GemmKernelParams* kp, cudaStream_t s, int* rc) {
   if (form != F || a_mn != A_MN || b_mn != B_MN) return false;
-  *rc = launch_gemm<256, A_MN, B_MN, EpiForm<F>::kInputs != 0, F>(tmA, tmB, tmE, kp, s);
+  if (kp) *rc = launch_gemm<256, A_MN, B_MN, EpiForm<F>::kInputs != 0, F>(tmA, tmB, tmE, *kp, s);
   return true;
 }
 static bool dispatch_form(uint32_t form, bool a_mn, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                          const EpiMaps<true>& tmE, const GemmKernelParams& kp, cudaStream_t s, int* rc) {
+                          const EpiMaps<true>& tmE, const GemmKernelParams* kp, cudaStream_t s, int* rc) {
 #define MB_FORM(F, A_MN, B_MN) launch_form<(F), A_MN, B_MN>(form, a_mn, b_mn, tmA, tmB, tmE, kp, s, rc)
   return MB_FORM(EF_ROPE, false, false) ||                           // qkv forward
          MB_FORM(EF_RES1, false, false) ||                           // attention out forward
          MB_FORM(EF_BIAS | EF_GELU | EF_AUX_OUT, false, false) ||    // fc_in forward
-         MB_FORM(EF_BIAS, false, false) ||                           // fc_out forward, LM head
+         MB_FORM(EF_BIAS, false, false) ||                           // fc_out forward, LM head, ViT qkv
          MB_FORM(EF_BIAS | EF_RES1 | EF_RES2, false, false) ||       // adapter up
+         MB_FORM(EF_BIAS | EF_RES1, false, false) ||                 // ViT out and proj
+         MB_FORM(EF_BIAS | EF_QGELU, false, false) ||                // ViT fc
          MB_FORM(EF_DGELU, false, true) ||                           // fc_out dgrad
          MB_FORM(0u, false, true) ||                                 // fc_in, attention out and LM-head dgrad
          MB_FORM(EF_RES1, false, true) ||                            // qkv dgrad, adapter dgrad-down
@@ -340,20 +343,26 @@ static bool dispatch_form(uint32_t form, bool a_mn, bool b_mn, const CUtensorMap
 #undef MB_FORM
 }
 
-// The compiled form a launch qualifies for, or EF_RUNTIME: its features must all be ones a form can express, every
-// [M, N] input staged by TMA (kp.epi_in), and bias and aux_out 8-byte aligned, which with the alignment gemm_impl
-// requires of C, ldc and the batch strides makes every 4-column access of a compiled form a vector.
-static uint32_t epi_form(const mb200_gemm_args* a, const GemmKernelParams& kp, int bn) {
-  if (a->generic_epilogue || bn != 256) return EF_RUNTIME;
-  if ((a->act != MB200_ACT_NONE && a->act != MB200_ACT_GELU_NEW) ||
+// The compiled form a launch qualifies for at the 256-wide tile, or EF_RUNTIME: its features must all be ones a form
+// can express, every [M, N] input staged by TMA (kp.epi_in), and bias and aux_out 8-byte aligned, which with the
+// alignment gemm_impl requires of C, ldc and the batch strides makes every 4-column access of a compiled form a vector.
+// generic_epilogue is not looked at here: the plan must not depend on it.
+static uint32_t epi_form(const mb200_gemm_args* a, const GemmKernelParams& kp) {
+  if ((a->act != MB200_ACT_NONE && a->act != MB200_ACT_GELU_NEW && a->act != MB200_ACT_QUICK_GELU) ||
       (a->dact != MB200_DACT_NONE && a->dact != MB200_DACT_GELU_NEW))
     return EF_RUNTIME;
   if (((reinterpret_cast<uintptr_t>(a->bias) | reinterpret_cast<uintptr_t>(a->aux_out)) & 7) != 0) return EF_RUNTIME;
   const uint32_t f = (a->bias ? EF_BIAS : 0u) | (kp.rope_mode ? EF_ROPE : 0u) | (a->aux_out ? EF_AUX_OUT : 0u) |
-                     (a->act ? EF_GELU : 0u) | (a->dact ? EF_DGELU : 0u) | (a->res1 ? EF_RES1 : 0u) |
-                     (a->res2 ? EF_RES2 : 0u) | (kp.c_f32 ? EF_F32 : 0u);
+                     (a->act == MB200_ACT_GELU_NEW ? EF_GELU : 0u) | (a->act == MB200_ACT_QUICK_GELU ? EF_QGELU : 0u) |
+                     (a->dact ? EF_DGELU : 0u) | (a->res1 ? EF_RES1 : 0u) | (a->res2 ? EF_RES2 : 0u) |
+                     (kp.c_f32 ? EF_F32 : 0u);
   const int inputs = (a->dact != 0) + (a->res1 != nullptr) + (a->res2 != nullptr);
-  return kp.epi_in == inputs ? f : EF_RUNTIME;
+  if (kp.epi_in != inputs) return EF_RUNTIME;
+  CUtensorMap unused;  // not read: no launch
+  EpiMaps<true> unused_e;
+  return dispatch_form(f, a->A.mn_major != 0, a->B.mn_major != 0, unused, unused, unused_e, nullptr, 0, nullptr)
+             ? f
+             : EF_RUNTIME;
 }
 
 // Tensor maps for the epilogue's [M, N] inputs (aux_in when dact, res1, res2), fetched by the producer through the
@@ -392,23 +401,37 @@ static int make_epi_maps(EpiMaps<true>* maps, GemmKernelParams* kp, const mb200_
   return 0;
 }
 
-static int pick_bn(int M, int N, int batches) {
+// The GEMM's tile width when it is not split along K. Model: time ~ waves x (cost of one tile).
+//  * Runtime epilogue form (no compiled form matches the launch): the relative tile costs of the three widths,
+//    kTile, independent of K. A wide tile streams A once per BN columns and keeps more MMA work per smem byte; narrower
+//    tiles only win when wide tiles leave most SMs idle, e.g. the adapter down-projection (M = 1024, N = 1024: 32 tiles
+//    of 256, 128 of 64).
+//  * A compiled form exists at BN = 256 and the GEMM has at least 8 row tiles: only 256 has the form, so the epilogue
+//    is counted too, in k-blocks of a 128 x 256 tile: num_kb x kTile[bn] + epi, with epi = kEpiForm at 256 and kEpiRuntime x bn / 256 at the narrower widths on
+//    the runtime form. The runtime epilogue costs about half a K = 4096 main loop per tile and a compiled one about a
+//    quarter of that (README, "Kernels on Hopper"). At short K the runtime
+//    epilogue dominates a narrow tile, so the GEMM stays at 256 with a badly filled last wave: ViT-L/14 fc at M = 2056
+//    runs 272 tiles in 3 waves instead of 1088 tiles of 64 in 9 waves. With fewer row tiles each weight tile is shared
+//    by few CTAs and the GEMM streams its weights from HBM, so filling the SMs matters more than the epilogue: the
+//    decode workload, whose GPT-J prompt GEMMs run at M = 256 (qkv: 96 tiles of 256 against 384 of 64), was 6 % slower
+//    with them planned this way, so they keep the first model.
+static int pick_bn(int M, int N, int K, int batches, bool compiled_form) {
   if (N <= 64) return 64;
-  // Model: time ~ waves * (cost of one tile). A wide tile streams A once per BN columns and keeps more MMA work per
-  // smem byte; narrower tiles only win when wide tiles leave most SMs idle (few tiles) — e.g. the adapter
-  // down-projection (M=1024, N=1024: 64 tiles at BN=128, 128 at BN=64). The relative tile costs are estimates.
   const int tiles_m = (M + BM - 1) / BM;
+  const int num_kb = (K + BK - 1) / BK;
   const int sms = num_sms();
+  const bool weigh_epi = compiled_form && tiles_m >= 8;
+  const double kTile[3] = {1.0, 0.55, 0.3}, kEpiRuntime = 32.0, kEpiForm = 8.0;
+  const int cands[3] = {256, 128, 64};
   double best = 1e300;
   int best_bn = 256;
-  const int cands[3] = {256, 128, 64};
-  const double tile_cost[3] = {1.0, 0.55, 0.3};  // relative time of one (BM x BN x K) tile
   for (int i = 0; i < 3; ++i) {
     const int bn = cands[i];
     if (bn > 64 && N <= bn / 2) continue;
     const long long t = (long long)tiles_m * ((N + bn - 1) / bn) * batches;
     const long long waves = (t + sms - 1) / sms;
-    const double cost = (double)waves * tile_cost[i];
+    const double epi = bn == 256 ? kEpiForm : kEpiRuntime * bn / 256;
+    const double cost = (double)waves * (weigh_epi ? num_kb * kTile[i] + epi : kTile[i]);
     if (cost < best - 1e-12) {
       best = cost;
       best_bn = bn;
@@ -416,6 +439,9 @@ static int pick_bn(int M, int N, int batches) {
   }
   return best_bn;
 }
+
+// The plan of this thread's last successful mb200_gemm call (mb200_gemm_last_plan)
+static thread_local int t_plan[2] = {0, 0};
 
 // Small-M (decode, M = batch <= 32) GEMMs stream their weight matrix once and are HBM-bound: what matters is bytes in
 // flight, i.e. every SM pulling weights all the time. The plan picks the tile width and a K split so that
@@ -477,8 +503,8 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
   int rc = check_arch();
   if (rc) return rc;
 
-  int bn = a->force_bn ? a->force_bn : pick_bn(a->M, a->N, a->nb0 * a->nb1);
-  MB_REQUIRE(bn == 64 || bn == 128 || bn == 256, MB200_E_ARG, "gemm: force_bn must be 64, 128 or 256");
+  int bn = a->force_bn;  // 0: planned below
+  MB_REQUIRE(bn == 0 || bn == 64 || bn == 128 || bn == 256, MB200_E_ARG, "gemm: force_bn must be 64, 128 or 256");
 
   CUtensorMap tmA, tmB;
   EpiMaps<true> tmE;
@@ -574,21 +600,37 @@ int gemm_impl(const mb200_gemm_args* a, cudaStream_t stream) {
       kp.alpha = 1.f;  // already applied to the partials
       MB_CUDA(launch_pdl(splitk_finalize_kernel, dim3(fgrid), dim3(256), 0, stream, kp));
       count_launch();
+      t_plan[0] = bn;  // recorded once every launch of the call has succeeded
+      t_plan[1] = split;
       return 0;
     }
   }
+  rc = make_epi_maps(&tmE, &kp, a);
+  if (rc) return rc;
+  const uint32_t form = epi_form(a, kp);
+  if (bn == 0) bn = pick_bn(a->M, a->N, a->K, a->nb0 * a->nb1, form != EF_RUNTIME);
   rc = make_operand_map(&tmB, a->B, a->N, a->K, a->nb0, a->nb1, bn);
   if (rc) return rc;
   kp.tiles_n = (a->N + bn - 1) / bn;
   kp.total_tiles = tiles_m * kp.tiles_n * a->nb0 * a->nb1;
-  rc = make_epi_maps(&tmE, &kp, a);
-  if (rc) return rc;
-  if (dispatch_form(epi_form(a, kp, bn), amn, bmn, tmA, tmB, tmE, kp, stream, &rc)) return rc;
-  return dispatch_bn(bn, amn, bmn, tmA, tmB, tmE, kp, stream);
+  if (!(!a->generic_epilogue && bn == 256 && form != EF_RUNTIME &&
+        dispatch_form(form, amn, bmn, tmA, tmB, tmE, &kp, stream, &rc)))
+    rc = dispatch_bn(bn, amn, bmn, tmA, tmB, tmE, kp, stream);
+  if (rc == 0) {
+    t_plan[0] = bn;
+    t_plan[1] = 1;
+  }
+  return rc;
 }
 
 }  // namespace mb200
 
 extern "C" int mb200_gemm(const mb200_gemm_args* args, void* stream) {
   return mb200::gemm_impl(args, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int mb200_gemm_last_plan(int32_t* bn, int32_t* split_k) {
+  if (bn) *bn = mb200::t_plan[0];
+  if (split_k) *split_k = mb200::t_plan[1];
+  return 0;
 }

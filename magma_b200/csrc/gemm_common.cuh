@@ -124,6 +124,7 @@ enum : uint32_t {
   EF_RES1 = 32,
   EF_RES2 = 64,
   EF_F32 = 128,
+  EF_QGELU = 256,  // act == MB200_ACT_QUICK_GELU
   EF_RUNTIME = 1u << 31
 };
 
@@ -142,7 +143,10 @@ struct EpiForm {
     return kRuntime ? p.aux_out != nullptr : (F & EF_AUX_OUT) != 0;
   }
   static __device__ __forceinline__ int act(const P& p) {
-    return kRuntime ? p.act : (F & EF_GELU) ? MB200_ACT_GELU_NEW : MB200_ACT_NONE;
+    return kRuntime ? p.act
+           : (F & EF_GELU) ? MB200_ACT_GELU_NEW
+           : (F & EF_QGELU) ? MB200_ACT_QUICK_GELU
+                            : MB200_ACT_NONE;
   }
   static __device__ __forceinline__ int dact(const P& p) {
     return kRuntime ? p.dact : (F & EF_DGELU) ? MB200_DACT_GELU_NEW : MB200_DACT_NONE;

@@ -131,6 +131,13 @@ def gemm(
     return out
 
 
+def gemm_last_plan():
+    """(tile width, K splits) of this thread's last gemm call"""
+    v = [ctypes.c_int32() for _ in range(2)]
+    lib().mb200_gemm_last_plan(*[ctypes.byref(x) for x in v])
+    return tuple(x.value for x in v)
+
+
 # --------------------------------------------------------------------------------------------
 # HBM-bound operators
 # --------------------------------------------------------------------------------------------
