@@ -179,6 +179,11 @@ static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 blo
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
+// plain launch, for kernels that do not call pdl_wait; launch errors surface through cudaGetLastError
+template <typename... KArgs, typename... Args>
+static inline void launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+  kern<<<grid, block, smem, st>>>(static_cast<KArgs>(args)...);
+}
 #endif
 
 }  // namespace mb200

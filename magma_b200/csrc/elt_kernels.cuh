@@ -1,6 +1,6 @@
 // magma_b200 — the HBM-bound kernels of the hot path (LayerNorm, rotary, softmax, cross-entropy, gathers, label
-// building, reductions, dropout, ViT / conv-trunk layout kernels, argmax, fused AdamW). FRAGMENT: included by
-// elementwise.cu inside `namespace mb200` (its host wrappers / C ABI follow there), and, unchanged, by
+// building, reductions, dropout, ViT / conv-trunk layout kernels, argmax, fused AdamW, the decode loop). FRAGMENT:
+// included by elementwise.cu inside `namespace mb200` (its C ABI follows in elt_abi.cuh), and, unchanged, by
 // oracle/kernel_host_exec.cpp, which executes kernel source on the CPU under an emulated thread model.
 
 // ---------------------------------------------------------------------------------------------
@@ -750,3 +750,48 @@ __global__ void cast_bf16_f32_kernel(const bf16* __restrict__ src, float* __rest
     dst[i] = __bfloat162float(src[i]);
 }
 
+
+// ---------------------------------------------------------------------------------------------
+// Device-resident decode loop (magma/sampling.py:78-109 runs one host-driven LM call per token with an `.all()` sync
+// each step): the step's cache position lives in DEVICE memory, so one CUDA graph of the whole decode step is replayed
+// per token with no host-side argument changing. These are the three small kernels around the LM call that read /
+// advance that position; the LM schedule itself takes it through mb200_gptj_sched_decode_step.
+// ---------------------------------------------------------------------------------------------
+__global__ void rope_table_dev_kernel(float2* __restrict__ tab, int S, int half, int rot, const int* __restrict__ pos0) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S * half) return;
+  const int p = i % half, s = i / half;
+  const float inv_freq = 1.0f / powf(10000.0f, (float)(2 * p) / (float)rot);
+  float sn, cs;
+  sincosf((float)(*pos0 + s) * inv_freq, &sn, &cs);
+  tab[i] = make_float2(cs, sn);
+}
+
+// x[b] = wte[tokens[b][pos]] : the input embedding of the decode step at cache position `pos` (the token emitted last)
+__global__ void decode_embed_kernel(const long long* __restrict__ tokens, long long ld_tok, const int* __restrict__ pos,
+                                    const bf16* __restrict__ wte, bf16* __restrict__ out, int d, int vocab) {
+  long long tok = tokens[(long long)blockIdx.x * ld_tok + *pos];
+  if (tok < 0 || tok >= vocab) tok = 0;
+  const uint4* src = reinterpret_cast<const uint4*>(wte + tok * (long long)d);
+  uint4* dst = reinterpret_cast<uint4*>(out + (long long)blockIdx.x * d);
+  for (int c = threadIdx.x; c < (d >> 3); c += blockDim.x) dst[c] = __ldg(src + c);
+}
+
+// tokens[b][pos + 1] = next[b]; flags[pos + 1 - s0] = every row emitted EOS (sampling.py:109); pos += 1. One CTA.
+__global__ void decode_advance_kernel(const long long* __restrict__ next, long long* __restrict__ tokens, long long ld_tok,
+                                      int* __restrict__ pos, long long eos, unsigned char* __restrict__ flags, int s0,
+                                      int n_flags, int B) {
+  const int p = *pos;
+  int is_eos = 1;
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const long long t = next[b];
+    if (p + 1 < ld_tok) tokens[(long long)b * ld_tok + p + 1] = t;
+    is_eos &= (t == eos);
+  }
+  const int all = __syncthreads_and(is_eos);
+  if (threadIdx.x == 0) {
+    const int i = p + 1 - s0;
+    if (flags != nullptr && i >= 0 && i < n_flags) flags[i] = (unsigned char)all;
+    *pos = p + 1;
+  }
+}

@@ -1,5 +1,18 @@
-// The body of mb200_sample (sampling.cu), kept in a fragment of its own so that oracle/kernel_host_exec.cpp can execute
-// the same source on the CPU. Included inside namespace mb200 after <curand_kernel.h>; needs bf16 and INFINITY.
+// Token sampling for temperature > 0 (magma/sampling.py:7-30,97-105): top-k filter, the reference's (inverted) nucleus
+// filter, softmax(logits / T) and one multinomial draw per row, in ONE kernel launch with no host round trip.
+//
+// One CTA of 1024 threads per row; thread t owns the contiguous slice [t*C, (t+1)*C) of the vocabulary, so that "the
+// first n elements equal to a value, in index order" — how ties are resolved here, = the reference run with a stable
+// sort — is a per-thread counter plus one block scan. The row (200 KB at V = 50258) is re-read from L2 in every pass.
+//   top-k      : 4-pass radix select (8 bits per pass) of the k-th largest order-preserving key; kept = the k largest.
+//   top-p quirk: sampling.py:13-17 removes the sorted ranks j >= 1 whose PRECEDING cumulative probability is below
+//                (1 - threshold), i.e. ranks 1..m with m = #{j : cum[j] < 1 - threshold}: the top m+1 tokens except the
+//                very first. The boundary rank is found by a radix descent on probability MASS instead of a sort.
+//   multinomial: inverse CDF over the surviving weights exp((x - max)/T) in index order, u from Philox(seed, row, offset).
+//
+// FRAGMENT: the body of mb200_sample (elt_abi.cuh), included by elementwise.cu inside an anonymous namespace in
+// namespace mb200 after <curand_kernel.h>, and, unchanged, by oracle/kernel_host_exec.cpp, which executes it on the CPU.
+// Needs bf16 and INFINITY.
 constexpr int kSampThreads = 1024;
 
 // larger float <=> larger key (-inf is the smallest). -0 takes the key of +0: the two are one value to the order, as

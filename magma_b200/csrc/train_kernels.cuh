@@ -1,6 +1,6 @@
 // magma_b200 — the kernels added for encoder training and the general adapter schedule (LayerNorm parameter gradients
 // over many rows, QuickGELU backward, BatchNorm / ReLU / convolution-adjoint support for the conv trunk, adapter_scale).
-// FRAGMENT: included by elementwise.cu inside `namespace mb200`; the host wrappers (C ABI) are in elementwise.cu.
+// FRAGMENT: included by elementwise.cu inside `namespace mb200`; the host wrappers (C ABI) are in elt_abi.cuh.
 // Checked on the GPU by tests/test_training_paths_gpu.py; their SOURCE is also executed on the CPU by oracle/kernel_host_exec.cpp (threads of a
 // block as OS threads, __syncthreads / shuffles / atomics emulated) and held to torch in tests/test_kernel_source_cpu.py.
 // LayerNorm parameter gradients for MANY rows (ViT training: 2056 rows x 49 LayerNorms; adapters with a leading LN):

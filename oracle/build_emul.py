@@ -37,14 +37,15 @@ def build(force=False):
 
 KX_OUT = os.path.join(OUT_DIR, "libkernel_host_exec.so")
 KX_SRC = os.path.join(ROOT, "oracle", "kernel_host_exec.cpp")
-KX_DEPS = [KX_SRC] + [os.path.join(ROOT, "magma_b200", "csrc", f) for f in ("warp_helpers.cuh", "elt_helpers.cuh",
+KX_DEPS = [KX_SRC, os.path.join(ROOT, "include", "magma_b200.h")] + [os.path.join(ROOT, "magma_b200", "csrc", f) for f in ("warp_helpers.cuh", "elt_helpers.cuh",
                                                                           "elt_kernels.cuh", "train_kernels.cuh",
-                                                                          "samp_kernels.cuh")]
+                                                                          "samp_kernels.cuh", "elt_abi.cuh")]
 
 
 def build_kernel_exec(force=False):
-    """oracle/_build/libkernel_host_exec.so: the product's kernel SOURCE (csrc/train_kernels.cuh and the helper fragments it
-    uses) compiled as host C++ and executed with the CUDA thread model emulated (oracle/kernel_host_exec.cpp)."""
+    """oracle/_build/libkernel_host_exec.so: the product's kernel SOURCE (the csrc/*.cuh fragments elementwise.cu includes,
+    C-ABI wrappers in elt_abi.cuh included) compiled as host C++ and executed with the CUDA thread model emulated
+    (oracle/kernel_host_exec.cpp)."""
     os.makedirs(OUT_DIR, exist_ok=True)
     if not force and os.path.exists(KX_OUT) and os.path.getmtime(KX_OUT) >= max(os.path.getmtime(d) for d in KX_DEPS):
         return KX_OUT

@@ -1,8 +1,8 @@
 """CPU replay of the test bodies of tests/test_elementwise_reference_gpu.py at small sizes, on the kernel source of
-csrc/elt_kernels.cuh and csrc/train_kernels.cuh executed on the CPU (oracle/kernel_host_exec.cpp). Keeps the float64
-references, the bounds, the rounding rule and the sentinel and input checks honest without a GPU. The executor uses
-other launch configurations and the accurate expf for __expf, so it says nothing about GPU bits or launch counts. The
-decode-loop kernels and the argument checks live only in elementwise.cu and run on the GPU only."""
+csrc/elt_kernels.cuh and csrc/train_kernels.cuh and the C-ABI wrappers of csrc/elt_abi.cuh executed on the CPU
+(oracle/kernel_host_exec.cpp). Keeps the float64 references, the bounds, the rounding rule, the sentinel and input checks
+and the wrappers' argument checks honest without a GPU. The executor runs the grid of a one-SM device and the accurate
+expf for __expf, so it says nothing about GPU bits or launch counts."""
 import pytest
 
 import test_elementwise_reference_gpu as E
@@ -96,3 +96,11 @@ def test_batchnorm_bookkeeping_on_kernel_source(kernel_ops, on_cpu, ratio):
 @pytest.mark.parametrize("case", ["plain", "clip_scale", "late_step", "no_decay_no_zero"])
 def test_adamw_on_kernel_source(kernel_ops, on_cpu, case):
     E.test_adamw(case)
+
+
+def test_decode_loop_on_kernel_source(kernel_ops, on_cpu):
+    E.test_decode_embed_and_advance()
+
+
+def test_argument_checks_on_kernel_source(kernel_ops, on_cpu):
+    E.test_misaligned_views_are_rejected()

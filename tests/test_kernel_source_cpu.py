@@ -1,10 +1,11 @@
 """The SOURCE of the training kernels (magma_b200/csrc/train_kernels.cuh), executed on the CPU.
 
-oracle/kernel_host_exec.cpp compiles those kernels unchanged as host C++ and runs them with the CUDA execution model
-emulated (threads of a block = OS threads, __syncthreads = barrier, warp shuffles and atomicAdd emulated, blocks in
-sequence). Here each kernel is held to the torch formula its GPU test uses (tests/test_training_paths_gpu.py): this checks
-what a kernel COMPUTES — indexing, 8-wide vector handling, masks, smem reductions, row-chunk accumulation through atomics —
-not what the hardware does with it."""
+oracle/kernel_host_exec.cpp compiles those kernels and their C-ABI wrappers (csrc/elt_abi.cuh) unchanged as host C++ and
+runs them with the CUDA execution model emulated (threads of a block = OS threads, __syncthreads = barrier, warp shuffles
+and atomicAdd emulated, blocks in sequence); the hx_* names are the wrappers without their stream argument. Here each
+kernel is held to the torch formula its GPU test uses (tests/test_training_paths_gpu.py): this checks what a kernel
+COMPUTES — indexing, 8-wide vector handling, masks, smem reductions, row-chunk accumulation through atomics — not what
+the hardware does with it."""
 import ctypes
 
 import pytest
@@ -259,8 +260,8 @@ def test_batchnorm_bookkeeping_kernel_source(kx):
 
 def test_sumsq_kernel_source_parts_cover_every_element(kx):
     """The grid-independent squared norm (elt_kernels.cuh::sumsq_kernel): 2048 logical parts over float4 chunks, a scalar
-    tail, and the scalar path for a view that is not 16-byte aligned. (The CPU executor runs it on a 4-block grid; the GPU
-    test checks that any grid gives the same bits.)"""
+    tail, and the scalar path for a view that is not 16-byte aligned. (The CPU executor runs it on a 16-block grid, the
+    grid of one SM; the GPU test checks that any grid gives the same bits.)"""
     g = torch.Generator().manual_seed(3)
     for n in (150 * 256 * 4 + 4 * 77 + 3, 1000, 5):   # (inputs long enough for several chunks per part: GPU test)
         x = torch.randn(n + 1, generator=g)

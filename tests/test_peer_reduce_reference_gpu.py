@@ -108,7 +108,7 @@ def test_peer_reduce_argument_checks_do_not_launch():
         arr = (ctypes.c_void_p * len(p))(*[ctypes.c_void_p(q) for q in p])
         n0 = launches()
         rc = lib().mb200_peer_reduce_bcast(arr, world, ctypes.c_int64(offset), ctypes.c_int64(n), 0, None)
-        torch.cuda.synchronize()
+        _sync()
         assert launches() == n0
         return rc
 

@@ -1,9 +1,9 @@
 """CPU replay of the test bodies of tests/test_sampling_reference_gpu.py and tests/test_peer_reduce_reference_gpu.py at
-small sizes, on the kernel source of csrc/samp_kernels.cuh and csrc/elt_kernels.cuh executed on the CPU
-(oracle/kernel_host_exec.cpp, 1024 threads per block as on the GPU). Keeps the float64 reference rule, its bounds, the
-Philox restatement and the layout checks honest without a GPU. The executor's expf is the host library's and its
-double atomics land in thread-scheduling order, so it says nothing about GPU bits, launch counts or the argument
-checks, which live in the host wrappers."""
+small sizes, on the kernel source of csrc/samp_kernels.cuh and csrc/elt_kernels.cuh and their C-ABI wrappers in
+csrc/elt_abi.cuh executed on the CPU (oracle/kernel_host_exec.cpp, 1024 threads per block as on the GPU). Keeps the
+float64 reference rule, its bounds, the Philox restatement, the layout checks and the argument checks honest without a
+GPU. The executor's expf is the host library's and its double atomics land in thread-scheduling order, so it says
+nothing about GPU bits."""
 import ctypes
 
 import numpy as np
@@ -64,3 +64,8 @@ def test_peer_reduce_on_kernel_source(kernel_ops, on_cpu):
         for offset, n in ((0, 4), (4, 1020), (8, 1040)):
             P._case(world, 1100, offset, n)
     P.test_peer_reduce_n0_launches_nothing()
+
+
+def test_argument_checks_on_kernel_source(kernel_ops, on_cpu):
+    S.test_argument_checks_do_not_launch()
+    P.test_peer_reduce_argument_checks_do_not_launch()
