@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libmagma_b200.so")
 
 _lib = None
+_configured = None  # the handle lib() last configured
 
 
 class MB200Error(RuntimeError):
@@ -65,20 +66,30 @@ class GemmArgs(ctypes.Structure):
 
 
 def lib():
-    """Load (once) and return the ctypes handle. Raises MB200Error when the library is not built."""
-    global _lib
+    """Load (once) and return the ctypes handle, configured with SIGNATURES. Raises MB200Error when the library is not
+    built. A handle installed in `_lib` from outside (the CPU emulation libraries of the tests) is configured the first
+    time it is returned."""
+    global _lib, _configured
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise MB200Error(
                 f"{LIB_PATH} not found: build it with `python -m magma_b200.build` "
                 "(magma_b200 has no CPU / eager fallback)"
             )
-        L = ctypes.CDLL(LIB_PATH)
-        L.mb200_last_error.restype = ctypes.c_char_p
-        L.mb200_version.restype = ctypes.c_int
-        _setup_signatures(L)
-        _lib = L
+        _lib = ctypes.CDLL(LIB_PATH)
+    if _lib is not _configured:
+        _configured = configure(_lib)
     return _lib
+
+
+def configure(L):
+    """Give every entry point of SIGNATURES that the handle L exports its restype and argtypes, so ctypes converts
+    plain Python values and rejects a wrong argument count or type before the call. Returns L."""
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name, None)
+        if fn is not None:
+            fn.restype, fn.argtypes = restype, argtypes
+    return L
 
 
 def check(rc):
@@ -165,33 +176,90 @@ class VitGradsC(ctypes.Structure):
                                                "ln_post_b", "proj")] + [("layers", ctypes.POINTER(VitLayerGradsC))]
 
 
-def _setup_signatures(L):
-    L.mb200_vit_workspace_bytes.restype = ctypes.c_size_t
-    L.mb200_vit_train_workspace_bytes.restype = ctypes.c_size_t
-    L.mb200_gptj_sched_workspace_bytes.restype = ctypes.c_size_t
-    L.mb200_gptj_sched_infer_workspace_bytes.restype = ctypes.c_size_t
-    L.mb200_gptj_sched_recompute_workspace_bytes.restype = ctypes.c_size_t
-    L.mb200_launch_count.restype = ctypes.c_longlong
+# ---- (restype, argtypes) of every entry point, in the order of include/magma_b200.h ----
+# int32_t / int -> c_int32, int64_t -> c_int64, uint64_t -> c_uint64, size_t -> c_size_t, float -> c_float,
+# long long -> c_longlong, const char* (return) -> c_char_p, const mb200_<struct>* -> POINTER(<its mirror above>),
+# void* const* -> POINTER(c_void_p), every other data pointer and the stream -> c_void_p.
+_i32, _i64, _u64, _f32 = ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64, ctypes.c_float
+_sz, _vp = ctypes.c_size_t, ctypes.c_void_p
+_GEMM, _VIT, _VITG, _GPTJ = (ctypes.POINTER(t) for t in (GemmArgs, VitModelC, VitGradsC, GptjModelExC))
 
+SIGNATURES = {
+    "mb200_version": (_i32, []),
+    "mb200_last_error": (ctypes.c_char_p, []),
+    "mb200_check_device": (_i32, []),
+    "mb200_set_gemm_sm_limit": (_i32, [_i32]),
+    "mb200_set_optimizer_grid": (_i32, [_i32]),
+    "mb200_launch_count": (ctypes.c_longlong, []),
+    "mb200_prof_enable": (_i32, [_i32]),
+    "mb200_prof_read": (_i32, [_vp, _vp, _vp, _vp]),
+    "mb200_gemm": (_i32, [_GEMM, _vp]),
+    "mb200_gemm_last_plan": (_i32, [_vp, _vp]),
+    "mb200_layernorm_fwd": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _i32, _f32, _vp]),
+    "mb200_layernorm_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),
+    "mb200_layernorm_param_grad": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_layernorm_param_grad_rows": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_rope": (_i32, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_rope_table": (_i32, [_vp, _i32, _i32, _i32, _vp]),
+    "mb200_softmax_fwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _f32, _i32, _i32, _vp]),
+    "mb200_softmax_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _f32, _vp]),
+    "mb200_build_labels": (_i32, [_vp, _i64, _vp, _i32, _i32, _i32, _i64, _vp]),
+    "mb200_embed_assemble": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_embed_gather": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_cross_entropy": (_i32, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _vp]),
+    "mb200_colsum": (_i32, [_vp, _i64, _i32, _i32, _vp, _i32, _vp]),
+    "mb200_dropout_fwd": (_i32, [_vp, _vp, _vp, _i64, _f32, _u64, _vp]),
+    "mb200_dropout_apply": (_i32, [_vp, _vp, _vp, _i64, _f32, _vp]),
+    "mb200_patchify": (_i32, [_vp, _vp, _i64, _i32, _i32, _i32, _vp]),
+    "mb200_vit_assemble": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_nchw_to_nhwc8": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_im2col3x3": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_avgpool_nhwc": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_col_moments": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "mb200_channel_affine": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _i32, _vp]),
+    "mb200_bn_finalize_fwd": (_i32, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "mb200_bn_bwd_coeffs": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp]),
+    "mb200_col2im3x3": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_avgpool_nhwc_bwd": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_argmax": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp]),
+    "mb200_sample": (_i32, [_vp, _i32, _i64, _i32, _i32, _f32, _i32, _f32, _u64, _u64, _vp, _vp, _vp]),
+    "mb200_add": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp]),
+    "mb200_peer_reduce_bcast": (_i32, [ctypes.POINTER(_vp), _i32, _i64, _i64, _i32, _vp]),
+    "mb200_sumsq": (_i32, [_vp, _i64, _vp, _vp]),
+    "mb200_adamw_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _f32, _vp, _f32, _i32,
+                                _i32, _vp]),
+    "mb200_cast_f32_to_bf16": (_i32, [_vp, _vp, _i64, _vp]),
+    "mb200_cast_bf16_to_f32": (_i32, [_vp, _vp, _i64, _vp]),
+    "mb200_vit_workspace_bytes": (_sz, [_VIT, _i32]),
+    "mb200_vit_forward": (_i32, [_VIT, _vp, _vp, _i32, _vp, _sz, _vp]),
+    "mb200_vit_train_workspace_bytes": (_sz, [_VIT, _i32]),
+    "mb200_vit_forward_train": (_i32, [_VIT, _vp, _vp, _i32, _vp, _sz, _vp]),
+    "mb200_vit_backward": (_i32, [_VIT, _VITG, _vp, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_quick_gelu_bwd": (_i32, [_vp, _vp, _vp, _i64, _vp]),
+    "mb200_gptj_sched_workspace_bytes": (_sz, [_GPTJ, _i32, _i32]),
+    "mb200_gptj_sched_forward": (_i32, [_GPTJ, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_backward": (_i32, [_GPTJ, _vp, _f32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_backward_range": (_i32, [_GPTJ, _vp, _f32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_recompute_workspace_bytes": (_sz, [_GPTJ, _i32, _i32]),
+    "mb200_gptj_sched_forward_recompute": (_i32, [_GPTJ, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_backward_range_recompute": (_i32, [_GPTJ, _vp, _f32, _i32, _i32, _i32, _i32, _i32, _vp, _sz,
+                                                         _vp]),
+    "mb200_gptj_sched_infer_workspace_bytes": (_sz, [_GPTJ, _i32, _i32, _i32]),
+    "mb200_gptj_sched_infer": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz,
+                                      _vp]),
+    "mb200_gptj_sched_decode_step": (_i32, [_GPTJ, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
+    "mb200_decode_embed": (_i32, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_decode_advance": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_rope_table_dev": (_i32, [_vp, _i32, _i32, _vp, _vp]),
+    "mb200_attn_decode_dev": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "mb200_scale_add": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "mb200_dot": (_i32, [_vp, _vp, _i64, _vp, _i32, _vp]),
+    "mb200_attn_fwd_tile": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_attn_bwd_tile": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_attn_fwd_flash": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _vp,
+                                    _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_attn_decode": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_kv_append": (_i32, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+}
 
-EXPORTED_SYMBOLS = [
-    "mb200_version", "mb200_last_error", "mb200_check_device", "mb200_gemm", "mb200_gemm_last_plan",
-    "mb200_launch_count", "mb200_prof_enable", "mb200_prof_read",
-    "mb200_layernorm_fwd", "mb200_layernorm_bwd", "mb200_layernorm_param_grad", "mb200_rope", "mb200_rope_table",
-    "mb200_softmax_fwd", "mb200_softmax_bwd", "mb200_build_labels", "mb200_embed_assemble", "mb200_embed_gather",
-    "mb200_cross_entropy", "mb200_colsum", "mb200_dropout_fwd", "mb200_dropout_apply", "mb200_patchify",
-    "mb200_nchw_to_nhwc8", "mb200_im2col3x3", "mb200_avgpool_nhwc",
-    "mb200_vit_assemble", "mb200_argmax", "mb200_sample", "mb200_add", "mb200_peer_reduce_bcast", "mb200_sumsq", "mb200_adamw_step",
-    "mb200_cast_f32_to_bf16", "mb200_cast_bf16_to_f32",
-    "mb200_vit_workspace_bytes", "mb200_vit_forward", "mb200_attn_decode", "mb200_attn_fwd_tile", "mb200_attn_fwd_flash",
-    "mb200_attn_bwd_tile",
-    "mb200_vit_train_workspace_bytes", "mb200_vit_forward_train", "mb200_vit_backward", "mb200_quick_gelu_bwd",
-    "mb200_layernorm_param_grad_rows", "mb200_set_gemm_sm_limit", "mb200_set_optimizer_grid", "mb200_scale_add", "mb200_dot",
-    "mb200_gptj_sched_workspace_bytes", "mb200_gptj_sched_forward", "mb200_gptj_sched_backward",
-    "mb200_col_moments", "mb200_channel_affine", "mb200_col2im3x3", "mb200_avgpool_nhwc_bwd",
-    "mb200_kv_append", "mb200_gptj_sched_infer_workspace_bytes", "mb200_gptj_sched_infer",
-    "mb200_gptj_sched_backward_range", "mb200_bn_finalize_fwd", "mb200_bn_bwd_coeffs",
-    "mb200_gptj_sched_decode_step", "mb200_decode_embed", "mb200_decode_advance", "mb200_rope_table_dev",
-    "mb200_attn_decode_dev", "mb200_gptj_sched_recompute_workspace_bytes", "mb200_gptj_sched_forward_recompute",
-    "mb200_gptj_sched_backward_range_recompute",
-]
+EXPORTED_SYMBOLS = list(SIGNATURES)

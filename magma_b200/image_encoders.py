@@ -255,16 +255,16 @@ class B200VisionTransformer(nn.Module):
         ws = self._train_ws(B)
         self._generation += 1
         feats = torch.empty(B, self.output_dim, dtype=torch.bfloat16, device=self._device)
-        check(lib().mb200_vit_forward_train(ctypes.byref(m), ops._ptr(x), ops._ptr(feats), B, ops._ptr(ws),
-                                            ctypes.c_size_t(ws.numel()), ops._stream()))
+        check(lib().mb200_vit_forward_train(ctypes.byref(m), ops._ptr(x), ops._ptr(feats), B, ops._ptr(ws), ws.numel(),
+                                            ops._stream()))
         return feats
 
     def _run_backward(self, dfeats, B):
         ar = self._arena
         ws = self._train_ws(B)
-        acc = int(bool(getattr(ar, "_accumulate_current", False)))
+        acc = bool(getattr(ar, "_accumulate_current", False))
         check(lib().mb200_vit_backward(ctypes.byref(self._cmodel()[0]), ctypes.byref(self._cgrads()), ops._ptr(dfeats),
-                                       acc, B, ops._ptr(ws), ctypes.c_size_t(ws.numel()), ops._stream()))
+                                       acc, B, ops._ptr(ws), ws.numel(), ops._stream()))
         ar.publish_grads()
 
     def forward(self, x):
@@ -285,8 +285,8 @@ class B200VisionTransformer(nn.Module):
             self._ws[B] = torch.empty(n, dtype=torch.uint8, device=self._device)
         ws = self._ws[B]
         feats = torch.empty(B, self.output_dim, dtype=torch.bfloat16, device=self._device)
-        check(lib().mb200_vit_forward(ctypes.byref(m), ops._ptr(x), ops._ptr(feats), B, ops._ptr(ws),
-                                      ctypes.c_size_t(ws.numel()), ops._stream()))
+        check(lib().mb200_vit_forward(ctypes.byref(m), ops._ptr(x), ops._ptr(feats), B, ops._ptr(ws), ws.numel(),
+                                      ops._stream()))
         return feats
 
 

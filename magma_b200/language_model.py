@@ -406,8 +406,8 @@ class B200GPTJForCausalLM(nn.Module):
             self._generation += 1  # this pass records its activations in the workspace
             self._generation_recompute = recompute
             fwd = lib().mb200_gptj_sched_forward_recompute if recompute else lib().mb200_gptj_sched_forward
-            check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ctypes.c_int64(ldv),
-                      ops._ptr(loss), B, S, ops._ptr(ws), ctypes.c_size_t(ws.numel()), ops._stream()))
+            check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ldv, ops._ptr(loss), B, S,
+                      ops._ptr(ws), ws.numel(), ops._stream()))
             self._last_hidden = None
             lg = logits.view(B, S, ldv)[..., :V] if logits is not None else None
             return (loss.squeeze(0) if loss is not None else None), lg
@@ -425,10 +425,10 @@ class B200GPTJForCausalLM(nn.Module):
         logits = torch.empty(rows, ldv, dtype=torch.bfloat16, device=x.device) if want_logits else None
         hidden = torch.empty(rows, d, dtype=torch.bfloat16, device=x.device) if want_hidden else None
         check(lib().mb200_gptj_sched_infer(
-            ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ctypes.c_int64(ldv), int(last_only), ops._ptr(hidden),
+            ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, ops._ptr(hidden),
             ops._ptr(cache.k) if cache is not None else None, ops._ptr(cache.v) if cache is not None else None,
-            S_kv if cache is not None else 0, cache.pos if cache is not None else 0, B, S, ops._ptr(ws),
-            ctypes.c_size_t(ws.numel()), ops._stream()))
+            S_kv if cache is not None else 0, cache.pos if cache is not None else 0, B, S, ops._ptr(ws), ws.numel(),
+            ops._stream()))
         if cache is not None:
             cache.pos += S
         self._last_hidden = hidden
@@ -444,10 +444,10 @@ class B200GPTJForCausalLM(nn.Module):
             raise MB200Error("backward called on a workspace of the other activation path (stored / recomputed) than "
                              "its forward's")
         bwd = lib().mb200_gptj_sched_backward_range_recompute if recompute else lib().mb200_gptj_sched_backward_range
-        accumulate = int(arena.grads_live()) if arena is not None else 0
+        accumulate = arena is not None and arena.grads_live()
         for hi, lo in (self._bwd_chunks or [(len(self.transformer.h), 0)]):
-            check(bwd(ctypes.byref(self._cmodel_ex()[0]), ops._ptr(dx) if lo == 0 else None, ctypes.c_float(loss_scale),
-                      hi, lo, accumulate, B, S, ops._ptr(ws), ctypes.c_size_t(ws.numel()), ops._stream()))
+            check(bwd(ctypes.byref(self._cmodel_ex()[0]), ops._ptr(dx) if lo == 0 else None, loss_scale, hi, lo,
+                      accumulate, B, S, ops._ptr(ws), ws.numel(), ops._stream()))
             if self._after_chunk is not None:
                 self._after_chunk(hi, lo)
         if arena is not None and self._own_arena:
@@ -497,10 +497,9 @@ class B200GPTJForCausalLM(nn.Module):
         if ws is None or ws.numel() < nbytes:
             self._ws.pop("infer", None)
             ws = self._ws["infer"] = torch.empty(nbytes, dtype=torch.uint8, device=self._device)
-        check(lib().mb200_gptj_sched_decode_step(ctypes.byref(m), ops._ptr(x), ops._ptr(logits),
-                                                 ctypes.c_int64(logits.stride(0)), ops._ptr(cache.k), ops._ptr(cache.v),
-                                                 cache.S_max, ops._ptr(pos_dev), B, ops._ptr(ws),
-                                                 ctypes.c_size_t(ws.numel()), ops._stream()))
+        check(lib().mb200_gptj_sched_decode_step(ctypes.byref(m), ops._ptr(x), ops._ptr(logits), logits.stride(0),
+                                                 ops._ptr(cache.k), ops._ptr(cache.v), cache.S_max, ops._ptr(pos_dev),
+                                                 B, ops._ptr(ws), ws.numel(), ops._stream()))
         return logits
 
     @torch.no_grad()

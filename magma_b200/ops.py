@@ -12,11 +12,11 @@ DACT_NONE, DACT_GELU_NEW, DACT_RELU = 0, 1, 3
 
 
 def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+    return t.data_ptr() if t is not None else None
 
 
 def _mat_meta(t, name):
@@ -159,9 +159,8 @@ def layernorm_fwd(x, gamma, beta, eps=1e-5, save_stats=True, out=None):
     y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if out is None else out
     mean = torch.empty(rows, dtype=torch.float32, device=x.device) if save_stats else None
     rstd = torch.empty(rows, dtype=torch.float32, device=x.device) if save_stats else None
-    check(lib().mb200_layernorm_fwd(_ptr(x), ctypes.c_int64(ldx), _ptr(gamma), _ptr(beta), _ptr(y),
-                                    ctypes.c_int64(_rows(y)[2]), _ptr(mean), _ptr(rstd), rows, d,
-                                    ctypes.c_float(eps), _stream()))
+    check(lib().mb200_layernorm_fwd(_ptr(x), ldx, _ptr(gamma), _ptr(beta), _ptr(y), _rows(y)[2], _ptr(mean), _ptr(rstd),
+                                    rows, d, eps, _stream()))
     return y, mean, rstd
 
 
@@ -169,38 +168,36 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, res=None, out=None):
     """dx of LayerNorm (+ res); into `out` (any row stride) when given."""
     rows, d, ldx = _rows(x)
     dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if out is None else out
-    check(lib().mb200_layernorm_bwd(_ptr(dy), ctypes.c_int64(_rows(dy)[2]), _ptr(x), ctypes.c_int64(ldx), _ptr(gamma),
-                                    _ptr(mean), _ptr(rstd), _ptr(res), ctypes.c_int64(_rows(res)[2] if res is not None else 0),
-                                    _ptr(dx), ctypes.c_int64(_rows(dx)[2]), rows, d, _stream()))
+    check(lib().mb200_layernorm_bwd(_ptr(dy), _rows(dy)[2], _ptr(x), ldx, _ptr(gamma), _ptr(mean), _ptr(rstd),
+                                    _ptr(res), _rows(res)[2] if res is not None else 0, _ptr(dx), _rows(dx)[2], rows, d,
+                                    _stream()))
     return dx
 
 
 def layernorm_param_grad(dy, x, mean, rstd, dgamma, dbeta, accumulate=False):
     rows, d, ldx = _rows(x)
-    check(lib().mb200_layernorm_param_grad(_ptr(dy), ctypes.c_int64(_rows(dy)[2]), _ptr(x), ctypes.c_int64(ldx),
-                                           _ptr(mean), _ptr(rstd), _ptr(dgamma), _ptr(dbeta), rows, d,
-                                           int(accumulate), _stream()))
+    check(lib().mb200_layernorm_param_grad(_ptr(dy), _rows(dy)[2], _ptr(x), ldx, _ptr(mean), _ptr(rstd), _ptr(dgamma),
+                                           _ptr(dbeta), rows, d, accumulate, _stream()))
 
 
 def layernorm_param_grad_rows(dy, x, mean, rstd, dgamma, dbeta, accumulate=False):
     """Same result as layernorm_param_grad with a (column strip) x (row chunk) grid — for thousands of rows."""
     rows, d, ldx = _rows(x)
-    check(lib().mb200_layernorm_param_grad_rows(_ptr(dy), ctypes.c_int64(_rows(dy)[2]), _ptr(x), ctypes.c_int64(ldx),
-                                                _ptr(mean), _ptr(rstd), _ptr(dgamma), _ptr(dbeta), rows, d,
-                                                int(accumulate), _stream()))
+    check(lib().mb200_layernorm_param_grad_rows(_ptr(dy), _rows(dy)[2], _ptr(x), ldx, _ptr(mean), _ptr(rstd),
+                                                _ptr(dgamma), _ptr(dbeta), rows, d, accumulate, _stream()))
 
 
 def quick_gelu_bwd(dy, pre, out=None):
     """dx = dy * d/dx[x sigmoid(1.702 x)] at x = pre (CLIP QuickGELU backward); `out` may be dy itself."""
     out = torch.empty_like(dy) if out is None else out
-    check(lib().mb200_quick_gelu_bwd(_ptr(dy), _ptr(pre), _ptr(out), ctypes.c_int64(dy.numel()), _stream()))
+    check(lib().mb200_quick_gelu_bwd(_ptr(dy), _ptr(pre), _ptr(out), dy.numel(), _stream()))
     return out
 
 
 def rope_(qkv, S, H, hd, rot, pos0=0, inverse=False):
     """In place on a [rows, 3*H*hd] fused qkv buffer."""
     rows = qkv.shape[0]
-    check(lib().mb200_rope(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), rows, S, H, hd, rot, pos0, int(inverse), _stream()))
+    check(lib().mb200_rope(_ptr(qkv), qkv.stride(0), rows, S, H, hd, rot, pos0, inverse, _stream()))
     return qkv
 
 
@@ -217,9 +214,8 @@ def softmax_fwd(s, scale, causal, koff=0, out=None):
     lds = s.stride(1)
     p = torch.zeros(nz, Sq, lds, dtype=torch.bfloat16, device=s.device)[..., :Sk] if out is None else out
     _batched_out(p, "out", (nz, Sq, Sk))
-    check(lib().mb200_softmax_fwd(_ptr(s), ctypes.c_int64(lds), ctypes.c_int64(s.stride(0)), _ptr(p),
-                                  ctypes.c_int64(p.stride(1)), ctypes.c_int64(p.stride(0)), nz, Sq, Sk,
-                                  ctypes.c_float(scale), int(causal), koff, _stream()))
+    check(lib().mb200_softmax_fwd(_ptr(s), lds, s.stride(0), _ptr(p), p.stride(1), p.stride(0), nz, Sq, Sk, scale,
+                                  causal, koff, _stream()))
     return p
 
 
@@ -235,10 +231,8 @@ def softmax_bwd(dp, p, scale, out=None):
     nz, Sq, Sk = dp.shape
     ds = torch.zeros(nz, Sq, p.stride(1), dtype=torch.bfloat16, device=dp.device)[..., :Sk] if out is None else out
     _batched_out(ds, "out", (nz, Sq, Sk))
-    check(lib().mb200_softmax_bwd(_ptr(dp), ctypes.c_int64(dp.stride(1)), ctypes.c_int64(dp.stride(0)), _ptr(p),
-                                  ctypes.c_int64(p.stride(1)), ctypes.c_int64(p.stride(0)), _ptr(ds),
-                                  ctypes.c_int64(ds.stride(1)), ctypes.c_int64(ds.stride(0)), nz, Sq, Sk,
-                                  ctypes.c_float(scale), _stream()))
+    check(lib().mb200_softmax_bwd(_ptr(dp), dp.stride(1), dp.stride(0), _ptr(p), p.stride(1), p.stride(0), _ptr(ds),
+                                  ds.stride(1), ds.stride(0), nz, Sq, Sk, scale, _stream()))
     return ds
 
 
@@ -248,8 +242,8 @@ def build_labels(captions, prefix_len, eos_token):
     if captions.dtype != torch.int64:
         raise TypeError("captions must be int64")
     labels = torch.empty(B, S, dtype=torch.int64, device=captions.device)
-    check(lib().mb200_build_labels(_ptr(captions), ctypes.c_int64(captions.stride(0)), _ptr(labels), B, S,
-                                   int(prefix_len), ctypes.c_int64(int(eos_token)), _stream()))
+    check(lib().mb200_build_labels(_ptr(captions), captions.stride(0), _ptr(labels), B, S, int(prefix_len),
+                                   int(eos_token), _stream()))
     return labels
 
 
@@ -259,7 +253,7 @@ def embed_assemble(captions, wte, prefix, S=None, out=None):
     L = 0 if prefix is None else prefix.shape[1]
     V, d = wte.shape
     x = torch.empty(B, S, d, dtype=torch.bfloat16, device=wte.device) if out is None else out
-    check(lib().mb200_embed_assemble(_ptr(captions), ctypes.c_int64(captions.stride(0)), _ptr(wte), _ptr(prefix), L,
+    check(lib().mb200_embed_assemble(_ptr(captions), captions.stride(0), _ptr(wte), _ptr(prefix), L,
                                      _ptr(x), B, S, d, V, _stream()))
     return x
 
@@ -284,8 +278,8 @@ def cross_entropy(logits, labels, V, write_grad=False, grad_scale=1.0, dlogits=N
     if dlogits is not None and dlogits.stride() != logits.stride():
         raise ValueError("cross_entropy: dlogits must share the strides of logits")
     dl = dlogits if dlogits is not None else (torch.zeros_like(logits) if write_grad else None)
-    check(lib().mb200_cross_entropy(_ptr(logits), ctypes.c_int64(ldv), _ptr(labels), B, S, V, _ptr(row_loss),
-                                    _ptr(n_valid), _ptr(loss), _ptr(dl), ctypes.c_float(grad_scale), _stream()))
+    check(lib().mb200_cross_entropy(_ptr(logits), ldv, _ptr(labels), B, S, V, _ptr(row_loss),
+                                    _ptr(n_valid), _ptr(loss), _ptr(dl), grad_scale, _stream()))
     return loss, dl
 
 
@@ -293,21 +287,20 @@ def colsum(x, out=None, accumulate=False):
     rows, cols = x.shape
     if out is None:
         out = torch.empty(cols, dtype=torch.float32, device=x.device)
-    check(lib().mb200_colsum(_ptr(x), ctypes.c_int64(x.stride(0)), rows, cols, _ptr(out), int(accumulate), _stream()))
+    check(lib().mb200_colsum(_ptr(x), x.stride(0), rows, cols, _ptr(out), accumulate, _stream()))
     return out
 
 
 def dropout_fwd(x, p, seed, out=None):
     y = torch.empty_like(x) if out is None else out
     mask = torch.empty(x.numel(), dtype=torch.uint8, device=x.device)
-    check(lib().mb200_dropout_fwd(_ptr(x), _ptr(y), _ptr(mask), ctypes.c_int64(x.numel()), ctypes.c_float(p),
-                                  ctypes.c_uint64(seed), _stream()))
+    check(lib().mb200_dropout_fwd(_ptr(x), _ptr(y), _ptr(mask), x.numel(), p, seed, _stream()))
     return y, mask
 
 
 def dropout_apply(x, mask, p, out=None):
     y = torch.empty_like(x) if out is None else out
-    check(lib().mb200_dropout_apply(_ptr(x), _ptr(mask), _ptr(y), ctypes.c_int64(x.numel()), ctypes.c_float(p), _stream()))
+    check(lib().mb200_dropout_apply(_ptr(x), _ptr(mask), _ptr(y), x.numel(), p, _stream()))
     return y
 
 
@@ -316,7 +309,7 @@ def argmax(x, V=None, out=None):
     V = x.shape[1] if V is None else V
     if out is None:
         out = torch.empty(rows, dtype=torch.int64, device=x.device)
-    check(lib().mb200_argmax(_ptr(x), ctypes.c_int64(x.stride(0)), rows, V, _ptr(out), _stream()))
+    check(lib().mb200_argmax(_ptr(x), x.stride(0), rows, V, _ptr(out), _stream()))
     return out
 
 
@@ -324,15 +317,15 @@ def decode_embed(tokens, pos_dev, wte, out):
     """out[b] = wte[tokens[b, pos]] with the column `pos` read from DEVICE memory (int32 [1]) — the input embedding of
     a graph-replayed decode step (mb200_decode_embed)."""
     V, d = wte.shape
-    check(lib().mb200_decode_embed(_ptr(tokens), ctypes.c_int64(tokens.stride(0)), _ptr(pos_dev), _ptr(wte), _ptr(out),
+    check(lib().mb200_decode_embed(_ptr(tokens), tokens.stride(0), _ptr(pos_dev), _ptr(wte), _ptr(out),
                                    tokens.shape[0], d, V, _stream()))
     return out
 
 
 def decode_advance(next_tokens, tokens, pos_dev, eos, flags, s0):
     """tokens[:, pos + 1] = next_tokens; flags[pos + 1 - s0] = all rows emitted `eos`; pos += 1 (all on the device)."""
-    check(lib().mb200_decode_advance(_ptr(next_tokens), _ptr(tokens), ctypes.c_int64(tokens.stride(0)), _ptr(pos_dev),
-                                     ctypes.c_int64(-1 if eos is None else int(eos)), _ptr(flags), int(s0),
+    check(lib().mb200_decode_advance(_ptr(next_tokens), _ptr(tokens), tokens.stride(0), _ptr(pos_dev),
+                                     -1 if eos is None else int(eos), _ptr(flags), int(s0),
                                      flags.numel() if flags is not None else 0, tokens.shape[0], _stream()))
 
 
@@ -370,8 +363,8 @@ def col_moments(u, v, mask=None):
     assert u.dtype == v.dtype == torch.bfloat16 and v.shape == u.shape and u.stride(1) == 1 and v.stride(1) == 1
     o1 = torch.empty(C, dtype=torch.float32, device=u.device)
     o2 = torch.empty(C, dtype=torch.float32, device=u.device)
-    check(lib().mb200_col_moments(_ptr(u), ctypes.c_int64(u.stride(0)), _ptr(v), ctypes.c_int64(v.stride(0)), _ptr(mask),
-                                  ctypes.c_int64(mask.stride(0) if mask is not None else 0), rows, C, _ptr(o1), _ptr(o2),
+    check(lib().mb200_col_moments(_ptr(u), u.stride(0), _ptr(v), v.stride(0), _ptr(mask),
+                                  mask.stride(0) if mask is not None else 0, rows, C, _ptr(o1), _ptr(o2),
                                   _stream()))
     return o1, o2
 
@@ -385,8 +378,8 @@ def channel_affine(x1, a1, x2=None, a2=None, c0=None, mask=None, res=None, relu=
     for t in (a1, a2, c0):
         assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.numel() == C)
     y = torch.empty_like(x1) if out is None else out
-    check(lib().mb200_channel_affine(_ptr(x1), _ptr(a1), _ptr(x2), _ptr(a2), _ptr(c0), _ptr(mask), _ptr(res), int(relu),
-                                     _ptr(y), ctypes.c_int64(rows), C, _stream()))
+    check(lib().mb200_channel_affine(_ptr(x1), _ptr(a1), _ptr(x2), _ptr(a2), _ptr(c0), _ptr(mask), _ptr(res), relu,
+                                     _ptr(y), rows, C, _stream()))
     return y
 
 
@@ -396,8 +389,8 @@ def bn_finalize_fwd(s1, s2, gamma, beta, rows, eps, momentum, running_mean=None,
     for t in (s1, s2, gamma, beta, running_mean, running_var):
         assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.numel() == C)
     out = torch.empty(4, C, dtype=torch.float32, device=s1.device)
-    check(lib().mb200_bn_finalize_fwd(_ptr(s1), _ptr(s2), _ptr(gamma), _ptr(beta), ctypes.c_int64(rows), ctypes.c_float(eps),
-                                      ctypes.c_float(momentum), _ptr(running_mean), _ptr(running_var), _ptr(out[0]),
+    check(lib().mb200_bn_finalize_fwd(_ptr(s1), _ptr(s2), _ptr(gamma), _ptr(beta), rows, eps,
+                                      momentum, _ptr(running_mean), _ptr(running_var), _ptr(out[0]),
                                       _ptr(out[1]), _ptr(out[2]), _ptr(out[3]), C, _stream()))
     return out[0], out[1], out[2], out[3]
 
@@ -409,8 +402,8 @@ def bn_bwd_coeffs(s1, t, mean, rstd, gamma, rows, dgamma, dbeta, accumulate=Fals
     for x in (s1, t, mean, rstd, gamma, dgamma, dbeta):
         assert x.dtype == torch.float32 and x.is_contiguous() and x.numel() == C
     out = torch.empty(3, C, dtype=torch.float32, device=s1.device)
-    check(lib().mb200_bn_bwd_coeffs(_ptr(s1), _ptr(t), _ptr(mean), _ptr(rstd), _ptr(gamma), ctypes.c_int64(rows),
-                                    _ptr(dgamma), _ptr(dbeta), int(accumulate), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), C,
+    check(lib().mb200_bn_bwd_coeffs(_ptr(s1), _ptr(t), _ptr(mean), _ptr(rstd), _ptr(gamma), rows,
+                                    _ptr(dgamma), _ptr(dbeta), accumulate, _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), C,
                                     _stream()))
     return out[0], out[1], out[2]
 
@@ -439,37 +432,37 @@ def sample(logits, temperature, top_k=0, top_p=0.0, seed=0, offset=0, return_mas
     rows, V = logits.shape
     out = torch.empty(rows, dtype=torch.int64, device=logits.device)
     mask = torch.empty(rows, V, dtype=torch.uint8, device=logits.device) if return_mask else None
-    check(lib().mb200_sample(_ptr(logits), 0 if logits.dtype == torch.bfloat16 else 1, ctypes.c_int64(logits.stride(0)), rows, V,
-                             ctypes.c_float(temperature), int(top_k), ctypes.c_float(top_p), ctypes.c_uint64(seed & (2**64 - 1)),
-                             ctypes.c_uint64(offset), _ptr(out), _ptr(mask), _stream()))
+    check(lib().mb200_sample(_ptr(logits), 0 if logits.dtype == torch.bfloat16 else 1, logits.stride(0), rows, V,
+                             temperature, int(top_k), top_p, seed & (2**64 - 1), offset, _ptr(out), _ptr(mask),
+                             _stream()))
     return (out, mask) if return_mask else out
 
 
 def add(a, b, c=None, out=None):
     y = torch.empty_like(a) if out is None else out
-    check(lib().mb200_add(_ptr(a), _ptr(b), _ptr(c), _ptr(y), ctypes.c_int64(a.numel()), _stream()))
+    check(lib().mb200_add(_ptr(a), _ptr(b), _ptr(c), _ptr(y), a.numel(), _stream()))
     return y
 
 
 def peer_reduce_bcast(buffer_ptrs, offset, n, max_blocks=0):
     """mb200_peer_reduce_bcast: `buffer_ptrs` = device addresses of every rank's exchange buffer as mapped here."""
-    arr = (ctypes.c_void_p * len(buffer_ptrs))(*[ctypes.c_void_p(int(p)) for p in buffer_ptrs])
-    check(lib().mb200_peer_reduce_bcast(arr, len(buffer_ptrs), ctypes.c_int64(offset), ctypes.c_int64(n), int(max_blocks),
+    arr = (ctypes.c_void_p * len(buffer_ptrs))(*[int(p) for p in buffer_ptrs])
+    check(lib().mb200_peer_reduce_bcast(arr, len(buffer_ptrs), offset, n, int(max_blocks),
                                         _stream()))
 
 
 def cast_f32_to_bf16(src, dst):
-    check(lib().mb200_cast_f32_to_bf16(_ptr(src), _ptr(dst), ctypes.c_int64(src.numel()), _stream()))
+    check(lib().mb200_cast_f32_to_bf16(_ptr(src), _ptr(dst), src.numel(), _stream()))
 
 
 def cast_bf16_to_f32(src, dst):
-    check(lib().mb200_cast_bf16_to_f32(_ptr(src), _ptr(dst), ctypes.c_int64(src.numel()), _stream()))
+    check(lib().mb200_cast_bf16_to_f32(_ptr(src), _ptr(dst), src.numel(), _stream()))
 
 
 def patchify(img, P, out):
     """images bf16 [B, 3, R, R] -> out [B * (R/P)^2, >= 3 P P] (row stride out.stride(0)), columns ordered (c, py, px)."""
     B, _, R, _ = img.shape
-    check(lib().mb200_patchify(_ptr(img), _ptr(out), ctypes.c_int64(out.stride(0)), B, R, P, _stream()))
+    check(lib().mb200_patchify(_ptr(img), _ptr(out), out.stride(0), B, R, P, _stream()))
     return out
 
 
@@ -483,13 +476,13 @@ def vit_assemble(x, pe, cls, pos):
 def scale_add(u, s=None, r1=None, r2=None, out=None):
     """out = s[0] * u + r1 + r2 (s: device fp32 scalar or None for 1; r1 / r2 optional), bf16."""
     out = torch.empty_like(u) if out is None else out
-    check(lib().mb200_scale_add(_ptr(u), _ptr(s), _ptr(r1), _ptr(r2), _ptr(out), ctypes.c_int64(u.numel()), _stream()))
+    check(lib().mb200_scale_add(_ptr(u), _ptr(s), _ptr(r1), _ptr(r2), _ptr(out), u.numel(), _stream()))
     return out
 
 
 def dot(a, b, out, accumulate=False):
     """out[0] (+)= sum a * b over bf16 vectors, fp32."""
-    check(lib().mb200_dot(_ptr(a), _ptr(b), ctypes.c_int64(a.numel()), _ptr(out), int(accumulate), _stream()))
+    check(lib().mb200_dot(_ptr(a), _ptr(b), a.numel(), _ptr(out), accumulate, _stream()))
     return out
 
 
@@ -506,16 +499,13 @@ def set_optimizer_grid(n_blocks):
 
 
 def sumsq(x, out):
-    check(lib().mb200_sumsq(_ptr(x), ctypes.c_int64(x.numel()), _ptr(out), _stream()))
+    check(lib().mb200_sumsq(_ptr(x), x.numel(), _ptr(out), _stream()))
 
 
 def adamw_step(master, grad, m1, m2, shadow, lr, beta1, beta2, eps, wd, grad_scale, gnorm_sq, max_norm, step,
                zero_grad=True):
-    check(lib().mb200_adamw_step(_ptr(master), _ptr(grad), _ptr(m1), _ptr(m2), _ptr(shadow),
-                                 ctypes.c_int64(master.numel()), ctypes.c_float(lr), ctypes.c_float(beta1),
-                                 ctypes.c_float(beta2), ctypes.c_float(eps), ctypes.c_float(wd),
-                                 ctypes.c_float(grad_scale), _ptr(gnorm_sq), ctypes.c_float(max_norm), int(step),
-                                 int(zero_grad), _stream()))
+    check(lib().mb200_adamw_step(_ptr(master), _ptr(grad), _ptr(m1), _ptr(m2), _ptr(shadow), master.numel(), lr, beta1,
+                                 beta2, eps, wd, grad_scale, _ptr(gnorm_sq), max_norm, int(step), zero_grad, _stream()))
 
 
 def _rows_out(t, name, rows, cols, dtype=torch.bfloat16):
@@ -549,8 +539,7 @@ def attn_fwd_tile(qkv, B, S, H, hd, O=None, P=None):
     if O is None:
         O = torch.empty(B * S, H * hd, dtype=torch.bfloat16, device=qkv.device)
     ldo = _rows_out(O, "O", B * S, H * hd)
-    check(lib().mb200_attn_fwd_tile(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(P), ctypes.c_int64(ldP), _ptr(O),
-                                    ctypes.c_int64(ldo), B, S, H, hd, _stream()))
+    check(lib().mb200_attn_fwd_tile(_ptr(qkv), qkv.stride(0), _ptr(P), ldP, _ptr(O), ldo, B, S, H, hd, _stream()))
     return O, P
 
 
@@ -581,10 +570,8 @@ def attn_fwd_flash(qkv, B, S, H, hd, causal=True, want_p=False, want_stats=False
         kk, vv, ldk, bsh, bsb = kcache.data_ptr(), vcache.data_ptr(), hd, Smax * hd, H * Smax * hd
     else:
         kk, vv, ldk, bsh, bsb = qkv.data_ptr() + 2 * d, qkv.data_ptr() + 4 * d, ld, hd, S * ld
-    c64, vp = ctypes.c_int64, ctypes.c_void_p
-    check(lib().mb200_attn_fwd_flash(_ptr(qkv), c64(ld), c64(hd), c64(S * ld), vp(kk), c64(ldk), c64(bsh), c64(bsb),
-                                     vp(vv), c64(ldk), c64(bsh), c64(bsb), _ptr(O), c64(ldo), _ptr(P), c64(ldP),
-                                     _ptr(stats), B, S, Sk, H, hd, int(bool(causal)), _stream()))
+    check(lib().mb200_attn_fwd_flash(_ptr(qkv), ld, hd, S * ld, kk, ldk, bsh, bsb, vv, ldk, bsh, bsb, _ptr(O), ldo,
+                                     _ptr(P), ldP, _ptr(stats), B, S, Sk, H, hd, bool(causal), _stream()))
     out = (O,)
     if want_p:
         out += (P,)
@@ -599,16 +586,15 @@ def attn_bwd_tile(qkv, dO, P, B, S, H, hd, rope_tab=None, rot=0, dqkv=None):
     if dqkv is None:
         dqkv = torch.empty(B * S, 3 * H * hd, dtype=torch.bfloat16, device=qkv.device)
     ld = _rows_out(dqkv, "dqkv", B * S, 3 * H * hd)
-    check(lib().mb200_attn_bwd_tile(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(dO), ctypes.c_int64(dO.stride(0)),
-                                    _ptr(P), ctypes.c_int64(_p_out(P, B, H, S, S)), _ptr(dqkv), ctypes.c_int64(ld),
-                                    _ptr(rope_tab), int(rot), B, S, H, hd, _stream()))
+    check(lib().mb200_attn_bwd_tile(_ptr(qkv), qkv.stride(0), _ptr(dO), dO.stride(0), _ptr(P), _p_out(P, B, H, S, S),
+                                    _ptr(dqkv), ld, _ptr(rope_tab), int(rot), B, S, H, hd, _stream()))
     return dqkv
 
 
 def kv_append(qkv, kcache, vcache, B, S, H, hd, pos0):
     """K / V of the fused qkv rows [B*S, 3*H*hd] (row stride qkv.stride(0)) into the caches [B, H, Smax, hd] at
     positions [pos0, pos0 + S) (mb200_kv_append)."""
-    check(lib().mb200_kv_append(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(kcache), _ptr(vcache), B, S, H, hd,
+    check(lib().mb200_kv_append(_ptr(qkv), qkv.stride(0), _ptr(kcache), _ptr(vcache), B, S, H, hd,
                                 kcache.shape[2], pos0, _stream()))
 
 
@@ -619,8 +605,8 @@ def attn_decode(qkv, kcache, vcache, B, H, hd, pos, out=None):
     if out is None:
         out = torch.empty(B, H * hd, dtype=torch.bfloat16, device=qkv.device)
     ldo = _rows_out(out, "out", B, H * hd)
-    check(lib().mb200_attn_decode(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(kcache), _ptr(vcache), _ptr(out),
-                                  ctypes.c_int64(ldo), B, H, hd, kcache.shape[2], int(pos), _stream()))
+    check(lib().mb200_attn_decode(_ptr(qkv), qkv.stride(0), _ptr(kcache), _ptr(vcache), _ptr(out), ldo, B, H, hd,
+                                  kcache.shape[2], int(pos), _stream()))
     return out
 
 
@@ -629,6 +615,6 @@ def attn_decode_dev(qkv, kcache, vcache, B, H, hd, pos_dev, out=None):
     if out is None:
         out = torch.empty(B, H * hd, dtype=torch.bfloat16, device=qkv.device)
     ldo = _rows_out(out, "out", B, H * hd)
-    check(lib().mb200_attn_decode_dev(_ptr(qkv), ctypes.c_int64(qkv.stride(0)), _ptr(kcache), _ptr(vcache), _ptr(out),
-                                      ctypes.c_int64(ldo), B, H, hd, kcache.shape[2], _ptr(pos_dev), _stream()))
+    check(lib().mb200_attn_decode_dev(_ptr(qkv), qkv.stride(0), _ptr(kcache), _ptr(vcache), _ptr(out), ldo, B, H, hd,
+                                      kcache.shape[2], _ptr(pos_dev), _stream()))
     return out

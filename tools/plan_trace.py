@@ -64,12 +64,10 @@ def vit_model(L):
 
 
 def trace(fn):
+    from magma_b200._lib import configure
     from oracle import build_emul
 
-    L = ctypes.CDLL(build_emul.build())
-    L.mb200_last_error.restype = ctypes.c_char_p
-    for f in ("mb200_gptj_sched_workspace_bytes", "mb200_gptj_sched_infer_workspace_bytes", "mb200_vit_workspace_bytes"):
-        getattr(L, f).restype = ctypes.c_size_t
+    L = configure(ctypes.CDLL(build_emul.build()))
     with tempfile.NamedTemporaryFile("r", suffix=".trace", delete=False) as t:
         path = t.name
     L.mb200_emul_trace(path.encode())
