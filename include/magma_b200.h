@@ -425,6 +425,27 @@ int mb200_gptj_sched_forward_recompute(const mb200_gptj_model_ex* m, const void*
 int mb200_gptj_sched_backward_range_recompute(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t layer_hi,
                                               int32_t layer_lo, int32_t accumulate, int32_t B, int32_t S, void* ws,
                                               size_t ws_bytes, void* stream);
+/* output_hidden_states of the training pass (GPTNeoModel.forward's all_hidden_states, magma/magma.py:242,270-274):
+ * copies the n_layer + 1 hidden states of the forward recorded in `ws` — entry 0 the input x, entry l the output of
+ * block l (l = 1 .. n_layer-1), entry n_layer ln_f of the last block's output — to hidden[l] (bf16 [B*S, d]; a NULL
+ * entry is skipped). Nothing is recomputed: the workspace holds them until the next forward. The _recompute variant takes
+ * a recompute workspace. */
+int mb200_gptj_sched_hidden_states(const mb200_gptj_model_ex* m, void* const* hidden, int32_t B, int32_t S, void* ws,
+                                   size_t ws_bytes, void* stream);
+int mb200_gptj_sched_hidden_states_recompute(const mb200_gptj_model_ex* m, void* const* hidden, int32_t B, int32_t S,
+                                             void* ws, size_t ws_bytes, void* stream);
+/* mb200_gptj_sched_backward_range(_recompute) of a loss that also reads those hidden states: dhidden holds n_layer + 1
+ * pointers, each NULL (no gradient) or the bf16 [B*S, d] gradient of entry l. The gradient of entry l < n_layer joins the
+ * residual-stream gradient where the backward crosses the input of layer l (entry 0 thus reaches dx); that of the ln_f
+ * entry joins the LM head's dgrad before the ln_f backward. Each entry is added by the call whose layer range holds it.
+ * With every pointer NULL the result equals mb200_gptj_sched_backward_range(_recompute). */
+int mb200_gptj_sched_backward_range_hidden(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden, float loss_scale,
+                                           int32_t layer_hi, int32_t layer_lo, int32_t accumulate, int32_t B, int32_t S,
+                                           void* ws, size_t ws_bytes, void* stream);
+int mb200_gptj_sched_backward_range_hidden_recompute(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                     float loss_scale, int32_t layer_hi, int32_t layer_lo,
+                                                     int32_t accumulate, int32_t B, int32_t S, void* ws, size_t ws_bytes,
+                                                     void* stream);
 /* Inference pass (no saved activations) — use_cache=True of magma/sampling.py:81-90: kcache / vcache bf16
  * [n_layer][B][H][S_kv_max][hd] or NULL; the K / V of this call are written at positions [pos0, pos0 + S) and attention
  * runs over [0, pos0 + S) (prefill S > 1 through mb200_attn_fwd_flash, decode S == 1 through mb200_attn_decode).
@@ -434,6 +455,14 @@ size_t mb200_gptj_sched_infer_workspace_bytes(const mb200_gptj_model_ex* m, int3
 int mb200_gptj_sched_infer(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv, int32_t last_only,
                            void* hidden, void* kcache, void* vcache, int32_t S_kv_max, int32_t pos0, int32_t B, int32_t S,
                            void* ws, size_t ws_bytes, void* stream);
+/* The same pass with output_hidden_states: hidden_all receives the n_layer + 1 hidden states of the S positions of this
+ * call (with a cache, the new positions only, as GPTNeoModel returns them), entry l at hidden_all + l * ld_hidden
+ * elements as bf16 [B*S, d] (ld_hidden >= B*S*d and % 8): x, the outputs of blocks 1 .. n_layer-1 (each block writes
+ * its output there, no copy) and ln_f of the last block's output over all S rows, also when last_only != 0 projects the
+ * last position only. */
+int mb200_gptj_sched_infer_hidden(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv, int32_t last_only,
+                                  void* hidden_all, int64_t ld_hidden, void* kcache, void* vcache, int32_t S_kv_max,
+                                  int32_t pos0, int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream);
 
 /* Device-resident decode loop (magma/sampling.py:78-109 issues one LM call per generated token from the host and syncs
  * on `.all()` every step). Here the cache position of the step lives in DEVICE memory (pos_dev, int32[1]): no argument

@@ -182,6 +182,7 @@ class VitGradsC(ctypes.Structure):
 # void* const* -> POINTER(c_void_p), every other data pointer and the stream -> c_void_p.
 _i32, _i64, _u64, _f32 = ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64, ctypes.c_float
 _sz, _vp = ctypes.c_size_t, ctypes.c_void_p
+_VPP = ctypes.POINTER(_vp)
 _GEMM, _VIT, _VITG, _GPTJ = (ctypes.POINTER(t) for t in (GemmArgs, VitModelC, VitGradsC, GptjModelExC))
 
 SIGNATURES = {
@@ -244,9 +245,17 @@ SIGNATURES = {
     "mb200_gptj_sched_forward_recompute": (_i32, [_GPTJ, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _vp, _sz, _vp]),
     "mb200_gptj_sched_backward_range_recompute": (_i32, [_GPTJ, _vp, _f32, _i32, _i32, _i32, _i32, _i32, _vp, _sz,
                                                          _vp]),
+    "mb200_gptj_sched_hidden_states": (_i32, [_GPTJ, _VPP, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_hidden_states_recompute": (_i32, [_GPTJ, _VPP, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_backward_range_hidden": (_i32, [_GPTJ, _vp, _VPP, _f32, _i32, _i32, _i32, _i32, _i32, _vp, _sz,
+                                                      _vp]),
+    "mb200_gptj_sched_backward_range_hidden_recompute": (_i32, [_GPTJ, _vp, _VPP, _f32, _i32, _i32, _i32, _i32, _i32,
+                                                                _vp, _sz, _vp]),
     "mb200_gptj_sched_infer_workspace_bytes": (_sz, [_GPTJ, _i32, _i32, _i32]),
     "mb200_gptj_sched_infer": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz,
                                       _vp]),
+    "mb200_gptj_sched_infer_hidden": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32,
+                                             _vp, _sz, _vp]),
     "mb200_gptj_sched_decode_step": (_i32, [_GPTJ, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
     "mb200_decode_embed": (_i32, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "mb200_decode_advance": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _vp]),

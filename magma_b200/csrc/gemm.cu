@@ -226,6 +226,14 @@ int make_operand_map(CUtensorMap* out, const mb200_operand& op, int rows, int K,
                             int box_rows) {
   PFN_encodeTiled enc = get_encode_fn();
   MB_REQUIRE(enc != nullptr, MB200_E_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
+  // The encoder is a driver call and needs a current context. A thread whose first CUDA work is a GEMM (an autograd
+  // worker thread entering the backward pass with nothing to allocate, say) has none bound yet: one runtime call binds
+  // the current device's primary context to it.
+  static thread_local bool ctx_bound = false;
+  if (!ctx_bound) {
+    MB_CUDA(cudaFree(nullptr));
+    ctx_bound = true;
+  }
   MB_REQUIRE((reinterpret_cast<uintptr_t>(op.ptr) & 15) == 0, MB200_E_ALIGN, "gemm operand pointer not 16B aligned");
   MB_REQUIRE(op.ld % 8 == 0, MB200_E_ALIGN, "gemm operand ld (%lld) must be a multiple of 8 elements",
              (long long)op.ld);

@@ -362,8 +362,12 @@ int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels,
 // recompute: each layer's activations are rebuilt from its x_in first. The rebuilt block output goes to P.dh, which is
 // dead at that point, so x_in, x_final and everything else the forward left stay as they were and a second backward
 // gives the same result.
-int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int layer_hi, int layer_lo, int acc, int B, int S,
-             void* ws, size_t ws_bytes, void* st, bool recompute) {
+// dhid (NULL, or n_layer + 1 pointers, each NULL or bf16 [M,d]): gradients of the hidden states hidden_states() returns.
+// Entry l < n_layer is layer l's input, so its gradient joins the residual-stream gradient once layer l's backward has
+// produced it (entry 0 thus reaches dx); the ln_f entry joins the LM head's dgrad in that GEMM's epilogue. Each entry is
+// added by the one call whose range holds its layer, so a chunked backward adds it once.
+int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, float loss_scale, int layer_hi,
+             int layer_lo, int acc, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute) {
   Plan P;
   MBS_TRY(make_plan(P, m, B, S, ws, recompute));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_backward: workspace too small");
@@ -376,6 +380,10 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int laye
   if (layer_hi == m->n_layer) {  // dxf = loss_scale * dlogits Wlm ; g = LN_f backward
     Epi e;
     e.alpha = loss_scale;
+    if (dhid && dhid[m->n_layer]) {
+      e.res1 = dhid[m->n_layer];
+      e.ld_res = d;
+    }
     MBS_TRY(gemm(st, M, d, m->vocab, mat(P.dlogits, P.ldv), wmat(m->w_lm, d, 1), P.dh, d, 0, e));
     MBS_TRY(mb200_layernorm_bwd(P.dh, d, P.x_final, d, m->lnf_g, P.lnf_mean, P.lnf_rstd, nullptr, 0, gb[m->n_layer & 1], d,
                                 M, d, st));
@@ -431,7 +439,22 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, float loss_scale, int laye
       MBS_TRY(gemm(st, M, d, 3 * d, mat(P.dqkv, 3 * d), wmat(L.w_qkv, d, 1), P.dh, d, 0, e));  // dh = dqkv Wqkv + ...
     }
     MBS_TRY(mb200_layernorm_bwd(P.dh, d, a.x_in, d, L.ln1_g, a.mean, a.rstd, g, d, gout, d, M, d, st));
+    if (dhid && dhid[l]) MBS_TRY(mb200_add(gout, dhid[l], nullptr, gout, (int64_t)M * d, st));
   }
+  return 0;
+}
+
+// The hidden states of the forward recorded in `ws` (GPTNeoModel.forward's all_hidden_states): entry l < n_layer is
+// layer l's input, entry n_layer the ln_f output. Both stay in the workspace until the next forward, on either path.
+int hidden_states(const mb200_gptj_model_ex* m, bf16s* const* hid, int B, int S, void* ws, size_t ws_bytes, void* st,
+                  bool recompute) {
+  Plan P;
+  MBS_TRY(make_plan(P, m, B, S, ws, recompute));
+  MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_hidden_states: workspace too small");
+  MBS_REQUIRE(hid != nullptr, MB200_E_ARG, "gptj_sched_hidden_states: hidden is NULL");
+  const size_t bytes = (size_t)P.M * P.d * sizeof(bf16s);
+  for (int l = 0; l <= m->n_layer; ++l)
+    if (hid[l]) MBS_TRY(rt_copy(hid[l], l < m->n_layer ? P.acts[l].x_in : P.xf_ln, bytes, st));
   return 0;
 }
 
@@ -484,9 +507,12 @@ int make_infer_plan(InferPlan& P, const mb200_gptj_model_ex* m, int B, int S, in
 // pos_dev != NULL: decode step (S == 1) whose cache position is read from DEVICE memory by the kernels that need it
 // (rotary table, fused cache attention) — nothing in the launch sequence depends on the position, so the whole step can
 // be captured once in a CUDA graph and replayed per token (pos0 is ignored).
+// hidden_all != NULL: n_layer + 1 hidden states of the S positions of this call, entry l at hidden_all + l * ld_hidden:
+// x, the outputs of blocks 0 .. n_layer-2 (each block writes its output there directly) and ln_f of the last block's
+// output over all S rows, also when last_only projects the last row alone.
 int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, long long ldv, int last_only, bf16s* hidden,
                   bf16s* kcache, bf16s* vcache, int Smax, int pos0, int B, int S, void* ws, size_t ws_bytes, void* st,
-                  const int32_t* pos_dev = nullptr) {
+                  const int32_t* pos_dev = nullptr, bf16s* hidden_all = nullptr, long long ld_hidden = 0) {
   InferPlan P;
   MBS_TRY(make_infer_plan(P, m, B, S, kcache ? Smax : S, ws));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_infer: workspace too small (%zu < %zu)",
@@ -503,15 +529,19 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
                     has_scale(m->layers[l].attn_ad) == has_scale(m->layers[0].attn_ad),
                 MB200_E_ARG, "gptj_sched_infer: every layer must carry the same adapter options");
   const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd;
+  MBS_REQUIRE(!hidden_all || (ld_hidden >= (long long)M * d && ld_hidden % 8 == 0), MB200_E_ALIGN,
+              "gptj_sched_infer_hidden: ld_hidden=%lld must be >= B*S*d and %%8", ld_hidden);
   const int Sk = kcache ? pos0 + S : S;
   const size_t cache_layer = (size_t)B * H * Smax * hd;
   ScratchScope scratch(P.splitk, P.splitk_bytes);
   if (pos_dev) MBS_TRY(mb200_rope_table_dev(P.rope_tab, S, m->rotary_dim, pos_dev, st));
   else MBS_TRY(mb200_rope_table(P.rope_tab, S, m->rotary_dim, pos0, st));
+  if (hidden_all) MBS_TRY(rt_copy(hidden_all, x, (size_t)M * d * sizeof(bf16s), st));
   const bf16s* xin = x;
   for (int l = 0; l < m->n_layer; ++l) {
     const mb200_gptj_layer_ex& L = m->layers[l];
     bf16s* xout = (l & 1) ? P.xb : P.xa;
+    if (hidden_all && l + 1 < m->n_layer) xout = hidden_all + (size_t)(l + 1) * ld_hidden;
     MBS_TRY(mb200_layernorm_fwd(xin, d, L.ln1_g, L.ln1_b, P.h, d, nullptr, nullptr, M, d, m->ln_eps, st));
     MBS_TRY(gemm(st, M, 3 * d, d, mat(P.h, d), wmat(L.w_qkv, d), P.qkv, 3 * d, 0,
                  rope_epi(P.rope_tab, 1, S, hd, m->rotary_dim, 2 * d)));
@@ -582,19 +612,25 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
     }
     xin = xout;
   }
+  bf16s* xf = P.xf_ln;
+  if (hidden_all) {
+    bf16s* h_lnf = hidden_all + (size_t)m->n_layer * ld_hidden;
+    MBS_TRY(mb200_layernorm_fwd(xin, d, m->lnf_g, m->lnf_b, h_lnf, d, nullptr, nullptr, M, d, m->ln_eps, st));
+    if (!last_only) xf = h_lnf;  // the full-sequence logits read the ln_f entry itself
+  }
   if (!logits && !hidden) return 0;
   const int rows = last_only ? B : M;
   if (last_only)
     MBS_TRY(mb200_layernorm_fwd(xin + (size_t)(S - 1) * d, (long long)S * d, m->lnf_g, m->lnf_b, P.xf_ln, d, nullptr, nullptr,
                                 B, d, m->ln_eps, st));
-  else
+  else if (xf == P.xf_ln)
     MBS_TRY(mb200_layernorm_fwd(xin, d, m->lnf_g, m->lnf_b, P.xf_ln, d, nullptr, nullptr, M, d, m->ln_eps, st));
-  if (hidden) MBS_TRY(rt_copy(hidden, P.xf_ln, (size_t)rows * d * sizeof(bf16s), st));
+  if (hidden) MBS_TRY(rt_copy(hidden, xf, (size_t)rows * d * sizeof(bf16s), st));
   if (logits) {
     MBS_REQUIRE(ldv % 8 == 0 && ldv >= m->vocab, MB200_E_ALIGN, "gptj_sched_infer: ldv=%lld must be >= vocab and %%8", ldv);
     Epi e;
     e.bias = m->b_lm;
-    MBS_TRY(gemm(st, rows, m->vocab, d, mat(P.xf_ln, d), wmat(m->w_lm, d), logits, ldv, 0, e));
+    MBS_TRY(gemm(st, rows, m->vocab, d, mat(xf, d), wmat(m->w_lm, d), logits, ldv, 0, e));
   }
   return 0;
 }
@@ -616,6 +652,18 @@ extern "C" int mb200_gptj_sched_infer(const mb200_gptj_model_ex* m, const void* 
   if (rc) return rc;
   return mb200::forward_infer(m, (const mb200::bf16s*)x, (mb200::bf16s*)logits, ldv, last_only, (mb200::bf16s*)hidden,
                               (mb200::bf16s*)kcache, (mb200::bf16s*)vcache, S_kv_max, pos0, B, S, ws, ws_bytes, stream);
+}
+
+extern "C" int mb200_gptj_sched_infer_hidden(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv,
+                                             int32_t last_only, void* hidden_all, int64_t ld_hidden, void* kcache,
+                                             void* vcache, int32_t S_kv_max, int32_t pos0, int32_t B, int32_t S, void* ws,
+                                             size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  MBS_REQUIRE(hidden_all != nullptr, MB200_E_ARG, "gptj_sched_infer_hidden: hidden_all is NULL");
+  return mb200::forward_infer(m, (const mb200::bf16s*)x, (mb200::bf16s*)logits, ldv, last_only, nullptr,
+                              (mb200::bf16s*)kcache, (mb200::bf16s*)vcache, S_kv_max, pos0, B, S, ws, ws_bytes, stream,
+                              nullptr, (mb200::bf16s*)hidden_all, ld_hidden);
 }
 
 extern "C" int mb200_gptj_sched_decode_step(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv,
@@ -647,8 +695,8 @@ extern "C" int mb200_gptj_sched_backward(const mb200_gptj_model_ex* m, void* dx,
                                          int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream) {
   int rc = mb200::rt_check_arch();
   if (rc) return rc;
-  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, m ? m->n_layer : 0, 0, accumulate, B, S, ws, ws_bytes, stream,
-                         false);
+  return mb200::backward(m, (mb200::bf16s*)dx, nullptr, loss_scale, m ? m->n_layer : 0, 0, accumulate, B, S, ws, ws_bytes,
+                         stream, false);
 }
 
 extern "C" int mb200_gptj_sched_backward_range(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t layer_hi,
@@ -656,8 +704,25 @@ extern "C" int mb200_gptj_sched_backward_range(const mb200_gptj_model_ex* m, voi
                                                size_t ws_bytes, void* stream) {
   int rc = mb200::rt_check_arch();
   if (rc) return rc;
-  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes, stream,
-                         false);
+  return mb200::backward(m, (mb200::bf16s*)dx, nullptr, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes,
+                         stream, false);
+}
+
+extern "C" int mb200_gptj_sched_hidden_states(const mb200_gptj_model_ex* m, void* const* hidden, int32_t B, int32_t S,
+                                              void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::hidden_states(m, (mb200::bf16s* const*)hidden, B, S, ws, ws_bytes, stream, false);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_hidden(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                      float loss_scale, int32_t layer_hi, int32_t layer_lo,
+                                                      int32_t accumulate, int32_t B, int32_t S, void* ws, size_t ws_bytes,
+                                                      void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
+                         accumulate, B, S, ws, ws_bytes, stream, false);
 }
 
 extern "C" size_t mb200_gptj_sched_recompute_workspace_bytes(const mb200_gptj_model_ex* m, int32_t B, int32_t S) {
@@ -680,6 +745,23 @@ extern "C" int mb200_gptj_sched_backward_range_recompute(const mb200_gptj_model_
                                                          int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream) {
   int rc = mb200::rt_check_arch();
   if (rc) return rc;
-  return mb200::backward(m, (mb200::bf16s*)dx, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes, stream,
-                         true);
+  return mb200::backward(m, (mb200::bf16s*)dx, nullptr, loss_scale, layer_hi, layer_lo, accumulate, B, S, ws, ws_bytes,
+                         stream, true);
+}
+
+extern "C" int mb200_gptj_sched_hidden_states_recompute(const mb200_gptj_model_ex* m, void* const* hidden, int32_t B,
+                                                        int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::hidden_states(m, (mb200::bf16s* const*)hidden, B, S, ws, ws_bytes, stream, true);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_hidden_recompute(const mb200_gptj_model_ex* m, void* dx,
+                                                                void* const* dhidden, float loss_scale, int32_t layer_hi,
+                                                                int32_t layer_lo, int32_t accumulate, int32_t B, int32_t S,
+                                                                void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
+                         accumulate, B, S, ws, ws_bytes, stream, true);
 }

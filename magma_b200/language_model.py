@@ -5,7 +5,7 @@
 (callable on int64 ids), `.transformer.h[l].{mlp,attn}` (get/settable — the seam `Magma.add_adapters` rewires,
 magma/magma.py:128-169), `named_parameters()` with "adapter" in adapter names, and
 `__call__(inputs_embeds=|input_ids=, labels=, use_cache=, past_key_values=, output_hidden_states=)` returning an
-object with `.loss`, `.logits`, `.past_key_values`.
+object with `.loss`, `.logits`, `.past_key_values`, `.hidden_states`.
 
 All frozen weights are bf16 tensors on the GPU; parameter names follow HF GPT-J (`attn.q_proj.weight`, `mlp.fc_in.*`,
 `ln_1`, `ln_f`, `lm_head`) — the executable stand-in for the reference's fork. The whole
@@ -184,6 +184,11 @@ def _split_attn(attn):
     raise MB200Error(f"unsupported attention wrapper {type(attn).__name__}")
 
 
+def _ptr_array(tensors):
+    """A C array of the tensors' data pointers (NULL for None) for the per-hidden-state arguments of the C ABI."""
+    return (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
+
+
 def _use_recompute(stored_bytes, other_bytes, free_bytes):
     """Whether a training pass recomputes block activations in its backward: yes when the stored-activation workspace
     plus the pass's other allocations does not fit in the memory the process can still allocate. Both paths run the
@@ -200,30 +205,39 @@ def _free_bytes(device):
     return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
 
 
+def _backward_scale(model, dloss):
+    """The loss gradient the LM head's backward scales by: B200Engine.backward's hint, else dloss (a host sync), or 0
+    when only hidden states feed the loss."""
+    if model._loss_scale_hint is not None:
+        return model._loss_scale_hint
+    return 0.0 if dloss is None else float(dloss)
+
+
 class _LMTrainFn(torch.autograd.Function):
     """loss = LM(inputs_embeds, labels) with the backward pass of the C++ runtime (LM frozen: dgrad through every
-    GEMM, wgrad only for adapters, written straight into the parameter arena's fp32 gradient buffer)."""
+    GEMM, wgrad only for adapters, written straight into the parameter arena's fp32 gradient buffer). With
+    want_hidden the n_layer + 1 hidden states follow (loss, logits) as outputs, and their gradients flow back through
+    the same backward pass."""
 
     @staticmethod
-    def forward(ctx, model, x, labels, anchor):
-        loss, logits = model._run_forward(x, labels, training=True)
+    def forward(ctx, model, x, labels, anchor, want_hidden=False):
+        loss, logits, hidden = model._run_forward(x, labels, training=True, want_hidden=want_hidden)
         ctx.model = model
         ctx.generation = model._generation
         ctx.shape = x.shape
         ctx.x_dtype = x.dtype
         ctx.mark_non_differentiable(logits)
-        return loss, logits
+        if want_hidden:
+            ctx.set_materialize_grads(False)  # an unused hidden state has no gradient to add
+        return (loss, logits, *(hidden or ()))
 
     @staticmethod
-    def backward(ctx, dloss, _dlogits):
+    def backward(ctx, dloss, _dlogits, *dhidden):
         model = ctx.model
         if ctx.generation != model._generation:
             raise MB200Error("backward called after another training forward overwrote the saved activations")
-        scale = model._loss_scale_hint
-        if scale is None:
-            scale = float(dloss)  # host sync; B200Engine.backward passes the scale as a hint instead
-        dx = model._run_backward(ctx.shape, scale)
-        return None, dx.to(ctx.x_dtype), None, None
+        dx = model._run_backward(ctx.shape, _backward_scale(model, dloss), dhidden)
+        return None, dx.to(ctx.x_dtype), None, None, None
 
 
 class B200GPTJForCausalLM(nn.Module):
@@ -383,6 +397,8 @@ class B200GPTJForCausalLM(nn.Module):
 
     # ---- passes --------------------------------------------------------------------------------
     def _run_forward(self, x, labels, training, cache=None, last_only=False, want_hidden=False, want_logits=True):
+        """(loss, logits, hidden states): the hidden states are output_hidden_states' tuple of n_layer + 1 [B, S, d]
+        tensors when want_hidden, else None."""
         B, S, d = x.shape
         x = x.to(torch.bfloat16).contiguous()
         if self._arena is not None or self.adapter_parameters():
@@ -391,13 +407,13 @@ class B200GPTJForCausalLM(nn.Module):
 
     def _run_pass(self, x, labels, training, cache, last_only, want_hidden, want_logits):
         """csrc/gptj_sched.cu: the training pass (activations saved for backward) when a loss is asked for, else the
-        inference pass — full sequence, KV-cache prefill / decode step, last-position logits, ln_f output."""
+        inference pass — full sequence, KV-cache prefill / decode step, last-position logits, every hidden state."""
         B, S, d = x.shape
         m = self._cmodel_ex()[0]
         V, ldv = self.lm_head.weight.shape[0], self.ldv
         if labels is not None or training:
-            if cache is not None or last_only or want_hidden:
-                raise MB200Error("a loss together with a KV cache / last-position logits / hidden states is not supported")
+            if cache is not None or last_only:
+                raise MB200Error("a loss together with a KV cache / last-position logits is not supported")
             ws, recompute = self._workspace_ex(B, S)
             logits = torch.empty(B * S, ldv, dtype=torch.bfloat16, device=x.device) if want_logits else None
             loss = torch.zeros(1, dtype=torch.float32, device=x.device) if labels is not None else None
@@ -408,9 +424,15 @@ class B200GPTJForCausalLM(nn.Module):
             fwd = lib().mb200_gptj_sched_forward_recompute if recompute else lib().mb200_gptj_sched_forward
             check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ldv, ops._ptr(loss), B, S,
                       ops._ptr(ws), ws.numel(), ops._stream()))
-            self._last_hidden = None
+            hidden = None
+            if want_hidden:  # copied out of the workspace, which the next forward overwrites
+                hidden = tuple(torch.empty(B, S, d, dtype=torch.bfloat16, device=x.device)
+                               for _ in range(len(self.transformer.h) + 1))
+                copy = (lib().mb200_gptj_sched_hidden_states_recompute if recompute
+                        else lib().mb200_gptj_sched_hidden_states)
+                check(copy(ctypes.byref(m), _ptr_array(hidden), B, S, ops._ptr(ws), ws.numel(), ops._stream()))
             lg = logits.view(B, S, ldv)[..., :V] if logits is not None else None
-            return (loss.squeeze(0) if loss is not None else None), lg
+            return (loss.squeeze(0) if loss is not None else None), lg, hidden
         S_kv = cache.S_max if cache is not None else S
         # ONE grow-only inference workspace: a serving process sees many (B, prompt length, cache length) combinations,
         # and the C side only needs `nbytes` of scratch for the pass at hand (nothing survives between calls)
@@ -423,19 +445,26 @@ class B200GPTJForCausalLM(nn.Module):
             ws = self._ws["infer"] = torch.empty(nbytes, dtype=torch.uint8, device=self._device)
         rows = B if last_only else B * S
         logits = torch.empty(rows, ldv, dtype=torch.bfloat16, device=x.device) if want_logits else None
-        hidden = torch.empty(rows, d, dtype=torch.bfloat16, device=x.device) if want_hidden else None
-        check(lib().mb200_gptj_sched_infer(
-            ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, ops._ptr(hidden),
-            ops._ptr(cache.k) if cache is not None else None, ops._ptr(cache.v) if cache is not None else None,
-            S_kv if cache is not None else 0, cache.pos if cache is not None else 0, B, S, ops._ptr(ws), ws.numel(),
-            ops._stream()))
+        kv = (ops._ptr(cache.k), ops._ptr(cache.v), S_kv, cache.pos) if cache is not None else (None, None, 0, 0)
+        hidden = None
+        if want_hidden:  # one buffer, entry l at l * B*S*d: each block writes its output into its entry
+            hidden = torch.empty(len(self.transformer.h) + 1, B, S, d, dtype=torch.bfloat16, device=x.device)
+            check(lib().mb200_gptj_sched_infer_hidden(
+                ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, ops._ptr(hidden), hidden.stride(0), *kv,
+                B, S, ops._ptr(ws), ws.numel(), ops._stream()))
+            hidden = hidden.unbind(0)
+        else:
+            check(lib().mb200_gptj_sched_infer(
+                ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, None, *kv, B, S, ops._ptr(ws),
+                ws.numel(), ops._stream()))
         if cache is not None:
             cache.pos += S
-        self._last_hidden = hidden
         lg = logits.view(B, 1 if last_only else S, ldv)[..., :V] if logits is not None else None
-        return None, lg
+        return None, lg, hidden
 
-    def _run_backward(self, shape, loss_scale):
+    def _run_backward(self, shape, loss_scale, dhidden=()):
+        """dhidden: the gradients of the hidden states the forward returned (each None or [B, S, d]); all None or
+        empty runs the backward of the loss alone."""
         B, S, d = shape
         arena = self._arena
         dx = torch.empty(B, S, d, dtype=torch.bfloat16, device=self._device)
@@ -443,10 +472,17 @@ class B200GPTJForCausalLM(nn.Module):
         if recompute != self._generation_recompute:
             raise MB200Error("backward called on a workspace of the other activation path (stored / recomputed) than "
                              "its forward's")
-        bwd = lib().mb200_gptj_sched_backward_range_recompute if recompute else lib().mb200_gptj_sched_backward_range
+        if any(g is not None for g in dhidden):
+            dh = [None if g is None else g.to(device=self._device, dtype=torch.bfloat16).contiguous() for g in dhidden]
+            extra = (_ptr_array(dh),)
+            bwd = (lib().mb200_gptj_sched_backward_range_hidden_recompute if recompute
+                   else lib().mb200_gptj_sched_backward_range_hidden)
+        else:
+            extra = ()
+            bwd = lib().mb200_gptj_sched_backward_range_recompute if recompute else lib().mb200_gptj_sched_backward_range
         accumulate = arena is not None and arena.grads_live()
         for hi, lo in (self._bwd_chunks or [(len(self.transformer.h), 0)]):
-            check(bwd(ctypes.byref(self._cmodel_ex()[0]), ops._ptr(dx) if lo == 0 else None, loss_scale, hi, lo,
+            check(bwd(ctypes.byref(self._cmodel_ex()[0]), ops._ptr(dx) if lo == 0 else None, *extra, loss_scale, hi, lo,
                       accumulate, B, S, ops._ptr(ws), ws.numel(), ops._stream()))
             if self._after_chunk is not None:
                 self._after_chunk(hi, lo)
@@ -465,7 +501,10 @@ class B200GPTJForCausalLM(nn.Module):
         has_trainable = any(p.requires_grad for _, p in self.adapter_parameters()) or inputs_embeds.requires_grad
         if labels is not None and torch.is_grad_enabled() and has_trainable and not use_cache:
             anchor = next((p for _, p in self.adapter_parameters() if p.requires_grad), None)
-            out.loss, out.logits = _LMTrainFn.apply(self, inputs_embeds, labels, anchor)
+            res = _LMTrainFn.apply(self, inputs_embeds, labels, anchor, output_hidden_states)
+            out.loss, out.logits = res[0], res[1]
+            if output_hidden_states:
+                out.hidden_states = tuple(res[2:])
             return out
         cache = past_key_values
         if use_cache and cache is None:
@@ -473,12 +512,11 @@ class B200GPTJForCausalLM(nn.Module):
             cfg = self.config
             cache = KVCache(cfg.num_layers, B, cfg.num_heads, S_max, cfg.hidden_size // cfg.num_heads, self._device)
         with torch.no_grad():
-            loss, logits = self._run_forward(inputs_embeds, labels, training=False, cache=cache if use_cache else None,
-                                             last_only=False, want_hidden=output_hidden_states)
-        out.loss, out.logits = loss, logits
+            loss, logits, hidden = self._run_forward(inputs_embeds, labels, training=False,
+                                                     cache=cache if use_cache else None, last_only=False,
+                                                     want_hidden=output_hidden_states)
+        out.loss, out.logits, out.hidden_states = loss, logits, hidden
         out.past_key_values = cache if use_cache else None
-        if output_hidden_states:
-            out.hidden_states = (self._last_hidden.view(B, S, -1),)  # final ln_f output only
         return out
 
     @torch.no_grad()
@@ -505,7 +543,7 @@ class B200GPTJForCausalLM(nn.Module):
     @torch.no_grad()
     def decode_logits(self, inputs_embeds, cache):
         """Last-position logits only (what magma/sampling.py:92 consumes): the LM head runs on B rows, not B*S."""
-        _, lg = self._run_forward(inputs_embeds, None, training=False, cache=cache, last_only=True)
+        _, lg, _ = self._run_forward(inputs_embeds, None, training=False, cache=cache, last_only=True)
         return lg[:, 0, :]
 
 

@@ -22,41 +22,41 @@ from .adapters import Adapter, AdapterWrapper, ParallelAdapter, ParallelAdapterW
 from .arena import ParamArena
 from .config import MultimodalConfig
 from .image_prefix import ImagePrefix
-from .language_model import LMOutput, _LMTrainFn, get_gptj
+from .language_model import LMOutput, _backward_scale, get_gptj
 from .sampling import generate
 from .utils import build_labels, get_tokenizer, print_main
 
 
 class _EmbedLMFn(torch.autograd.Function):
     """loss = LM(cat(prefix, wte[captions][:, :S-L]), labels): assembles the input in one gather kernel, runs the
-    fused forward, and routes d(input)[:, :L] back to the image prefix."""
+    fused forward, and routes d(input)[:, :L] back to the image prefix. With want_hidden the LM's n_layer + 1 hidden
+    states follow (loss, logits), and their gradients join the same backward pass (entry 0's prefix rows included)."""
 
     @staticmethod
-    def forward(ctx, magma, prefix, captions, labels, anchor):
+    def forward(ctx, magma, prefix, captions, labels, anchor, want_hidden=False):
         lm = magma.lm
         x = ops.embed_assemble(captions, lm.transformer.wte.weight, prefix.to(torch.bfloat16).contiguous())
-        loss, logits = lm._run_forward(x, labels, training=True)
+        loss, logits, hidden = lm._run_forward(x, labels, training=True, want_hidden=want_hidden)
         ctx.magma, ctx.generation = magma, lm._generation
         ctx.shape, ctx.L, ctx.pdtype = x.shape, prefix.shape[1], prefix.dtype
         ctx.mark_non_differentiable(logits)
-        return loss, logits
+        if want_hidden:
+            ctx.set_materialize_grads(False)  # an unused hidden state has no gradient to add
+        return (loss, logits, *(hidden or ()))
 
     @staticmethod
-    def backward(ctx, dloss, _dlogits):
+    def backward(ctx, dloss, _dlogits, *dhidden):
         lm = ctx.magma.lm
         if ctx.generation != lm._generation:
             raise RuntimeError("backward called after another training forward overwrote the saved activations")
-        scale = lm._loss_scale_hint
-        if scale is None:
-            scale = float(dloss)
         arena = ctx.magma._arena
         if arena is not None:
             arena._accumulate_current = arena.grads_live()
-        dx = lm._run_backward(ctx.shape, scale)
+        dx = lm._run_backward(ctx.shape, _backward_scale(lm, dloss), dhidden)
         if arena is not None:
             arena.publish_grads()
         dprefix = dx[:, : ctx.L, :].contiguous().to(ctx.pdtype)
-        return None, dprefix, None, None, None
+        return None, dprefix, None, None, None, None
 
 
 class Magma(nn.Module):
@@ -245,8 +245,9 @@ class Magma(nn.Module):
         trainable = self._arena is not None and torch.is_grad_enabled()
         if trainable:
             anchor = self._arena.params[0]
-            loss, logits = _EmbedLMFn.apply(self, input_embeddings, captions, labels, anchor)
-            return LMOutput(loss=loss, logits=logits, past_key_values=None, hidden_states=None)
+            res = _EmbedLMFn.apply(self, input_embeddings, captions, labels, anchor, output_hidden_states)
+            return LMOutput(loss=res[0], logits=res[1], past_key_values=None,
+                            hidden_states=tuple(res[2:]) if output_hidden_states else None)
         with torch.no_grad():
             x = ops.embed_assemble(captions, self.lm.transformer.wte.weight,
                                    input_embeddings.to(torch.bfloat16).contiguous())
