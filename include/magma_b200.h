@@ -468,9 +468,10 @@ int mb200_gptj_sched_infer_hidden(const mb200_gptj_model_ex* m, const void* x, v
  * on `.all()` every step). Here the cache position of the step lives in DEVICE memory (pos_dev, int32[1]): no argument
  * of a decode step changes from token to token, so the caller captures ONE step in a CUDA graph — mb200_decode_embed
  * (input embedding of the token emitted last) -> mb200_gptj_sched_decode_step (= mb200_gptj_sched_infer with S = 1,
- * last_only, position read on the device) -> mb200_argmax -> mb200_decode_advance (store the new ids at column pos + 1 of
- * the [B, ld_tok] id buffer, record whether every row emitted EOS, pos += 1) — and replays it per token. Token ids are
- * the same as the host-driven loop's (same kernels, same order). */
+ * last_only, position read on the device) -> mb200_argmax (temperature 0) or mb200_sample_dev (temperature > 0) ->
+ * mb200_decode_advance (store the new ids at column pos + 1 of the [B, ld_tok] id buffer, record whether every row
+ * emitted EOS, pos += 1) — and replays it per token. Token ids are the same as the host-driven loop's (same kernels,
+ * same order, same Philox offsets). */
 int mb200_gptj_sched_decode_step(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv, void* kcache,
                                  void* vcache, int32_t S_kv_max, const int32_t* pos_dev, int32_t B, void* ws,
                                  size_t ws_bytes, void* stream);
@@ -478,6 +479,14 @@ int mb200_decode_embed(const int64_t* tokens, int64_t ld_tok, const int32_t* pos
                        int32_t d, int32_t vocab, void* stream);
 int mb200_decode_advance(const int64_t* next, int64_t* tokens, int64_t ld_tok, int32_t* pos_dev, int64_t eos,
                          uint8_t* flags, int32_t s0, int32_t n_flags, int32_t B, void* stream);
+/* mb200_sample with the Philox offset read from device memory: offset = *pos_dev - s0 + 1 (as a 64-bit unsigned value),
+ * one load in the kernel before the generator is seeded. pos_dev is the decode loop's int32 cache position and s0 the
+ * prompt length; at decode step i >= 1 the position holds s0 + i - 1, so the offset is the step index i that the
+ * host-driven loop passes to mb200_sample, and the draws are the same for the same (seed, row, offset). Same kernel,
+ * arguments and checks as mb200_sample, plus pos_dev != NULL (MB200_E_ARG). */
+int mb200_sample_dev(const void* logits, int32_t dtype, int64_t ld, int32_t rows, int32_t V, float temperature,
+                     int32_t top_k, float top_p, uint64_t seed, const int32_t* pos_dev, int32_t s0, int64_t* tokens,
+                     uint8_t* keep_mask, void* stream);
 /* mb200_rope_table / mb200_attn_decode with the position read from device memory (shared memory sized for S_kv_max). */
 int mb200_rope_table_dev(float* tab, int32_t S, int32_t rot, const int32_t* pos0_dev, void* stream);
 int mb200_attn_decode_dev(const void* qkv, int64_t ld_qkv, void* kcache, void* vcache, void* out, int64_t ld_out,

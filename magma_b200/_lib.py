@@ -259,6 +259,7 @@ SIGNATURES = {
     "mb200_gptj_sched_decode_step": (_i32, [_GPTJ, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
     "mb200_decode_embed": (_i32, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "mb200_decode_advance": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_sample_dev": (_i32, [_vp, _i32, _i64, _i32, _i32, _f32, _i32, _f32, _u64, _vp, _i32, _vp, _vp, _vp]),
     "mb200_rope_table_dev": (_i32, [_vp, _i32, _i32, _vp, _vp]),
     "mb200_attn_decode_dev": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "mb200_scale_add": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp]),

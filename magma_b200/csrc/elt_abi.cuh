@@ -513,21 +513,40 @@ extern "C" int mb200_decode_advance(const int64_t* next, int64_t* tokens, int64_
   return 0;
 }
 
-// Token sampling for temperature > 0 (kernel and method in samp_kernels.cuh).
+// Token sampling for temperature > 0 (kernel and method in samp_kernels.cuh). `name` prefixes the error messages; Off is
+// the kernel's offset source.
+template <typename Off>
+static int sample_launch(const char* name, const void* logits, int32_t dtype, int64_t ld, int32_t rows, int32_t V,
+                         float temperature, int32_t top_k, float top_p, uint64_t seed, Off offset, int64_t* tokens,
+                         uint8_t* keep_mask, void* stream) {
+  MB_REQUIRE(rows > 0 && V > 0 && ld >= V, MB200_E_SHAPE, "%s: rows=%d V=%d ld=%lld", name, rows, V, (long long)ld);
+  MB_REQUIRE(temperature > 0.f, MB200_E_ARG, "%s: temperature must be > 0 (use mb200_argmax for greedy decoding)", name);
+  MB_REQUIRE(top_k >= 0 && top_p >= 0.f && top_p <= 1.f, MB200_E_ARG, "%s: top_k=%d top_p=%f", name, top_k, top_p);
+  MB_REQUIRE(dtype == MB200_BF16 || dtype == MB200_F32, MB200_E_DTYPE, "%s: logits must be bf16 or f32", name);
+  if (dtype == MB200_F32)
+    launch(sample_kernel<float, Off>, rows, kSampThreads, 0, ST(stream), (const float*)logits, ld, V, 1.f / temperature,
+           top_k, top_p, seed, offset, (long long*)tokens, keep_mask);
+  else
+    launch(sample_kernel<bf16, Off>, rows, kSampThreads, 0, ST(stream), (const bf16*)logits, ld, V, 1.f / temperature,
+           top_k, top_p, seed, offset, (long long*)tokens, keep_mask);
+  MB_LAUNCH_CHECK();
+  return 0;
+}
+
 extern "C" int mb200_sample(const void* logits, int32_t dtype, int64_t ld, int32_t rows, int32_t V, float temperature,
                             int32_t top_k, float top_p, uint64_t seed, uint64_t offset, int64_t* tokens,
                             uint8_t* keep_mask, void* stream) {
   MB_ENTER();
-  MB_REQUIRE(rows > 0 && V > 0 && ld >= V, MB200_E_SHAPE, "sample: rows=%d V=%d ld=%lld", rows, V, (long long)ld);
-  MB_REQUIRE(temperature > 0.f, MB200_E_ARG, "sample: temperature must be > 0 (use mb200_argmax for greedy decoding)");
-  MB_REQUIRE(top_k >= 0 && top_p >= 0.f && top_p <= 1.f, MB200_E_ARG, "sample: top_k=%d top_p=%f", top_k, top_p);
-  MB_REQUIRE(dtype == MB200_BF16 || dtype == MB200_F32, MB200_E_DTYPE, "sample: logits must be bf16 or f32");
-  if (dtype == MB200_F32)
-    launch(sample_kernel<float>, rows, kSampThreads, 0, ST(stream), (const float*)logits, ld, V, 1.f / temperature,
-           top_k, top_p, seed, offset, (long long*)tokens, keep_mask);
-  else
-    launch(sample_kernel<bf16>, rows, kSampThreads, 0, ST(stream), (const bf16*)logits, ld, V, 1.f / temperature, top_k,
-           top_p, seed, offset, (long long*)tokens, keep_mask);
-  MB_LAUNCH_CHECK();
-  return 0;
+  return sample_launch<unsigned long long>("sample", logits, dtype, ld, rows, V, temperature, top_k, top_p, seed,
+                                           offset, tokens, keep_mask, stream);
+}
+
+// The Philox offset is read on the device: pos_dev - s0 + 1, the decode loop's step index (DecodeOffset).
+extern "C" int mb200_sample_dev(const void* logits, int32_t dtype, int64_t ld, int32_t rows, int32_t V, float temperature,
+                                int32_t top_k, float top_p, uint64_t seed, const int32_t* pos_dev, int32_t s0,
+                                int64_t* tokens, uint8_t* keep_mask, void* stream) {
+  MB_ENTER();
+  MB_REQUIRE(pos_dev != nullptr, MB200_E_ARG, "sample_dev: pos_dev is NULL");
+  return sample_launch("sample_dev", logits, dtype, ld, rows, V, temperature, top_k, top_p, seed,
+                       DecodeOffset{pos_dev, s0}, tokens, keep_mask, stream);
 }

@@ -10,7 +10,7 @@
 //                very first. The boundary rank is found by a radix descent on probability MASS instead of a sort.
 //   multinomial: inverse CDF over the surviving weights exp((x - max)/T) in index order, u from Philox(seed, row, offset).
 //
-// FRAGMENT: the body of mb200_sample (elt_abi.cuh), included by elementwise.cu inside an anonymous namespace in
+// FRAGMENT: the body of mb200_sample and mb200_sample_dev (elt_abi.cuh), included by elementwise.cu inside an anonymous namespace in
 // namespace mb200 after <curand_kernel.h>, and, unchanged, by oracle/kernel_host_exec.cpp, which executes it on the CPU.
 // Needs bf16 and INFINITY.
 constexpr int kSampThreads = 1024;
@@ -98,11 +98,24 @@ struct TopSet {
   }
 };
 
+// Where the Philox offset of the draw comes from. mb200_sample passes it by value. mb200_sample_dev reads it from the
+// decode loop's cache position in device memory, so a CUDA graph of the decode step draws at a new offset per replay:
+// offset = pos - s0 + 1, the step index i of the host-driven loop (at step i >= 1 the position holds s0 + i - 1).
+struct DecodeOffset {
+  const int* pos;
+  int s0;
+};
+__device__ __forceinline__ unsigned long long philox_offset(unsigned long long offset) { return offset; }
+__device__ __forceinline__ unsigned long long philox_offset(DecodeOffset o) {
+  return (unsigned long long)((long long)*o.pos - o.s0 + 1);
+}
+
 // One block per SM, said explicitly: with the default bound ptxas aims at 32 registers and spills the Philox state.
-template <typename T>
+// Off: unsigned long long (mb200_sample) or DecodeOffset (mb200_sample_dev); the body is the same.
+template <typename T, typename Off>
 __global__ void __launch_bounds__(kSampThreads, 1)
 sample_kernel(const T* __restrict__ logits, long long ld, int V, float inv_temp, int top_k, float top_p,
-              unsigned long long seed, unsigned long long offset, long long* __restrict__ tokens,
+              unsigned long long seed, Off offset, long long* __restrict__ tokens,
               uint8_t* __restrict__ keep_mask) {
   __shared__ Shared s;
   const T* x = logits + (long long)blockIdx.x * ld;
@@ -266,7 +279,7 @@ sample_kernel(const T* __restrict__ logits, long long ld, int V, float inv_temp,
   double W;
   const double wbase = block_excl_scan_d(wloc, s, &W);
   curandStatePhilox4_32_10_t st;
-  curand_init(seed, (unsigned long long)blockIdx.x, offset, &st);
+  curand_init(seed, (unsigned long long)blockIdx.x, philox_offset(offset), &st);
   const double u = (double)curand_uniform(&st) * W;  // (0, W]: identical in every thread of the row
   if (tid == 0) s.winner = 0x7fffffff;
   __syncthreads();

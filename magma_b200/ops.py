@@ -438,6 +438,19 @@ def sample(logits, temperature, top_k=0, top_p=0.0, seed=0, offset=0, return_mas
     return (out, mask) if return_mask else out
 
 
+def sample_dev(logits, pos_dev, s0, temperature, top_k, top_p, seed, out):
+    """`sample` with the Philox offset read on the device, pos_dev[0] - s0 + 1 (pos_dev: int32 [1], the decode loop's
+    cache position; s0: the prompt length), into the preallocated int64 `out` [rows] — capturable in a CUDA graph of
+    the decode step (mb200_sample_dev)."""
+    assert logits.ndim == 2 and logits.stride(1) == 1 and logits.dtype in (torch.bfloat16, torch.float32)
+    assert out.dtype == torch.int64 and out.numel() == logits.shape[0] and pos_dev.dtype == torch.int32
+    rows, V = logits.shape
+    check(lib().mb200_sample_dev(_ptr(logits), 0 if logits.dtype == torch.bfloat16 else 1, logits.stride(0), rows, V,
+                                 temperature, int(top_k), top_p, seed & (2**64 - 1), _ptr(pos_dev), int(s0), _ptr(out),
+                                 None, _stream()))
+    return out
+
+
 def add(a, b, c=None, out=None):
     y = torch.empty_like(a) if out is None else out
     check(lib().mb200_add(_ptr(a), _ptr(b), _ptr(c), _ptr(y), a.numel(), _stream()))

@@ -5,13 +5,14 @@ cache) but: the cache is a static [layer,B,H,S_max,hd] buffer appended in place 
 kernel (no torch.cat growth), the LM head runs on the B last-position rows only, temperature-0 argmax is a device
 kernel with torch.argmax tie-breaking (lowest index), and the all-EOS early-exit check (sampling.py:109) is polled
 every `eos_check_every` steps instead of forcing a host sync per token — emitted tokens are identical because
-rows are truncated at the first all-EOS step afterwards. With temperature 0 on the GPU the decode step runs as ONE
+rows are truncated at the first all-EOS step afterwards. On the GPU the decode step, greedy or sampled, runs as ONE
 replayed CUDA graph whose state (cache position included) lives in device memory.
 
 `top_p_filter`, `top_k_filter` and `remove_tokens_after_eos` below are the reference's public host-side helpers kept
 VERBATIM in behaviour and near-verbatim in text (magma/sampling.py:7-40, ~20 lines, each cited): callers of the
 reference import them by name and the nucleus filter's inverted comparison is a quirk that must be reproduced, not
-fixed. `generate` itself does not use them — it samples with the one-launch kernel `mb200_sample`."""
+fixed. `generate` itself does not use them — it samples with the one-launch kernel `mb200_sample` (`mb200_sample_dev` in
+the replayed graph)."""
 import os
 from typing import List, Union
 
@@ -19,6 +20,10 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
+
+# The library's sampler. A caller may replace ops.sample (a custom draw, a recorder); generate then keeps calling it
+# once per step (see use_graph below), as it did before sampled decoding was captured in the graph.
+_LIB_SAMPLE = ops.sample
 
 
 def top_p_filter(logits, threshold: float = 0.9):
@@ -68,12 +73,15 @@ def generate(model, embeddings, max_steps: int = 100, temperature: float = 0.7, 
     all_eos = torch.zeros(max_steps, dtype=torch.bool, device=dev)
     # Philox seed of this call, drawn from torch's CPU generator: reproducible under torch.manual_seed, new per call
     sample_seed = int(torch.randint(0, 2**62, (1,)).item()) if temperature != 0.0 else 0
-    # T = 0 on the GPU: after the prefill, ONE decode step — embedding of the token emitted last, the LM step, argmax,
-    # store + EOS flag + position increment — is captured in a CUDA graph whose only state is device memory (the cache
-    # position included) and replayed per token: no per-step host work besides the replay, same kernels in the same order
-    # as the host-driven loop (token ids identical). MB200_DECODE_GRAPH=0 keeps the host-driven loop.
-    use_graph = (temperature == 0.0 and dev.type == "cuda" and max_steps > 2
-                 and os.environ.get("MB200_DECODE_GRAPH", "1") != "0")
+    # On the GPU, after the prefill, ONE decode step — embedding of the token emitted last, the LM step, the next token
+    # (argmax at T = 0, else mb200_sample_dev), store + EOS flag + position increment — is captured in a CUDA graph whose
+    # only state is device memory (the cache position included) and replayed per token: no per-step host work besides the
+    # replay, same kernels in the same order as the host-driven loop. The sampler reads its Philox offset from the cache
+    # position (position - s + 1 = the step index i the host loop passes), so with the same seed every draw, and every
+    # token id, is identical. MB200_DECODE_GRAPH=0 keeps the host-driven loop, and so does a replaced ops.sample at T > 0:
+    # the graph would bypass it.
+    use_graph = (dev.type == "cuda" and max_steps > 2 and os.environ.get("MB200_DECODE_GRAPH", "1") != "0"
+                 and (temperature == 0.0 or ops.sample is _LIB_SAMPLE))
     graph = None
     for i in range(max_steps):
         if i == 0:
@@ -95,7 +103,10 @@ def generate(model, embeddings, max_steps: int = 100, temperature: float = 0.7, 
                 def dev_step():
                     ops.decode_embed(out, pos_dev, lm.transformer.wte.weight, x_buf)
                     lm.decode_step_dev(x_buf, cache, pos_dev, lg_buf)
-                    ops.argmax(lg_buf, V, out=nxt_buf)
+                    if temperature == 0.0:
+                        ops.argmax(lg_buf, V, out=nxt_buf)
+                    else:
+                        ops.sample_dev(lg_buf[:, :V], pos_dev, s, temperature, top_k, top_p, sample_seed, nxt_buf)
                     ops.decode_advance(nxt_buf, out, pos_dev, eos_i, flags, s)
 
                 dev_step()                                                      # step 1 eagerly (also warms every launch)
