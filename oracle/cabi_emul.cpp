@@ -70,6 +70,23 @@ extern "C" int mb200_emul_tracing(void) { return g_trace != nullptr; }
     }                                                                 \
   } while (0)
 
+// ---- launch records (tools/plan_trace.py, tests/test_production_launches_*.py): with a record file open, every
+// primitive a schedule issues also writes one JSON line holding every scalar argument its kernel or its plan depends
+// on, and every pointer as a raw address (the caller gives each tensor its own placeholder base and resolves the
+// address into (region, byte offset)). Written whether or not the trace is on, next to the trace line: after the
+// argument checks for mb200_gemm and mb200_layernorm_param_grad_rows (a call they reject leaves no record), before
+// them elsewhere, and always before the primitive computes anything.
+static FILE* g_rec = nullptr;
+extern "C" void mb200_emul_record(const char* path) {
+  if (g_rec) fclose(g_rec);
+  g_rec = path ? fopen(path, "w") : nullptr;
+}
+#define EM_RECORD(op, fmt, ...)                                          \
+  do {                                                                   \
+    if (g_rec) fprintf(g_rec, "{\"op\":\"" op "\"," fmt "}\n", __VA_ARGS__); \
+  } while (0)
+#define EM_P(p) (unsigned long long)reinterpret_cast<uintptr_t>(p)
+
 typedef uint16_t bf16_t;
 static inline float b2f(bf16_t v) {
   uint32_t u = (uint32_t)v << 16;
@@ -134,6 +151,22 @@ int mb200_gemm(const mb200_gemm_args* a, void*) {
     EM_REQUIRE(a->rope_S > 0 && a->rope_hd > 0 && a->rope_rot % 4 == 0 && a->rope_rot <= a->rope_hd &&
                    a->rope_hd % 4 == 0 && a->rope_ncols % 4 == 0,
                MB200_E_ARG, "gemm: bad rope epilogue parameters");
+  EM_RECORD("gemm",
+            "\"M\":%d,\"N\":%d,\"K\":%d,\"nb0\":%d,\"nb1\":%d,"
+            "\"A\":%llu,\"a_ld\":%lld,\"a_bs0\":%lld,\"a_bs1\":%lld,\"a_mn\":%d,"
+            "\"B\":%llu,\"b_ld\":%lld,\"b_bs0\":%lld,\"b_bs1\":%lld,\"b_mn\":%d,\"b_static\":%d,"
+            "\"c_dtype\":%d,\"C\":%llu,\"ldc\":%lld,\"c_bs0\":%lld,\"c_bs1\":%lld,\"alpha\":%.9g,"
+            "\"act\":%d,\"dact\":%d,\"accumulate\":%d,\"bias\":%llu,\"aux_out\":%llu,\"aux_in\":%llu,"
+            "\"res1\":%llu,\"res2\":%llu,\"ld_res\":%lld,\"force_bn\":%d,\"generic_epilogue\":%d,"
+            "\"rope_mode\":%d,\"rope_tab\":%llu,\"rope_S\":%d,\"rope_hd\":%d,\"rope_rot\":%d,\"rope_ncols\":%d,"
+            "\"splitk_ws\":%llu,\"splitk_ws_bytes\":%lld",
+            a->M, a->N, a->K, a->nb0, a->nb1, EM_P(a->A.ptr), (long long)a->A.ld, (long long)a->A.bs0,
+            (long long)a->A.bs1, a->A.mn_major, EM_P(a->B.ptr), (long long)a->B.ld, (long long)a->B.bs0,
+            (long long)a->B.bs1, a->B.mn_major, a->B.static_data, a->c_dtype, EM_P(a->C), (long long)a->ldc,
+            (long long)a->c_bs0, (long long)a->c_bs1, (double)a->alpha, a->act, a->dact, a->accumulate, EM_P(a->bias),
+            EM_P(a->aux_out), EM_P(a->aux_in), EM_P(a->res1), EM_P(a->res2), (long long)a->ld_res, a->force_bn,
+            a->generic_epilogue, a->rope_mode, EM_P(a->rope_tab), a->rope_S, a->rope_hd, a->rope_rot, a->rope_ncols,
+            EM_P(a->splitk_ws), (long long)a->splitk_ws_bytes);
   {
     const double nb = (double)a->nb0 * a->nb1, csz = a->c_dtype == MB200_F32 ? 4.0 : 2.0;
     const double MN = (double)a->M * a->N;
@@ -209,6 +242,11 @@ int mb200_gemm(const mb200_gemm_args* a, void*) {
 // ---- LayerNorm (elementwise.cu: layernorm_fwd_kernel / layernorm_bwd_kernel / layernorm_param_grad*_kernel) ----
 int mb200_layernorm_fwd(const void* x_, int64_t ldx, const void* gamma_, const void* beta_, void* y_, int64_t ldy,
                         float* mean, float* rstd, int32_t rows, int32_t d, float eps, void*) {
+  EM_RECORD("layernorm_fwd",
+            "\"x\":%llu,\"ldx\":%lld,\"gamma\":%llu,\"beta\":%llu,\"y\":%llu,\"ldy\":%lld,\"mean\":%llu,"
+            "\"rstd\":%llu,\"rows\":%d,\"d\":%d,\"eps\":%.9g",
+            EM_P(x_), (long long)ldx, EM_P(gamma_), EM_P(beta_), EM_P(y_), (long long)ldy, EM_P(mean), EM_P(rstd), rows,
+            d, (double)eps);
   EM_TRACE(8.0 * rows * d, (double)rows * d * 4 + (mean ? rows * 8.0 : 0), "layernorm_fwd\trows=%d d=%d", rows, d);
   EM_REQUIRE(rows > 0 && d > 0 && d % 8 == 0 && d <= 8192, MB200_E_SHAPE, "layernorm: bad d=%d", d);
   EM_REQUIRE(ldx % 8 == 0 && ldy % 8 == 0, MB200_E_ALIGN, "layernorm: row strides must be multiples of 8");
@@ -235,6 +273,11 @@ int mb200_layernorm_fwd(const void* x_, int64_t ldx, const void* gamma_, const v
 int mb200_layernorm_bwd(const void* dy_, int64_t lddy, const void* x_, int64_t ldx, const void* gamma_,
                         const float* mean, const float* rstd, const void* res_, int64_t ldres, void* dx_, int64_t lddx,
                         int32_t rows, int32_t d, void*) {
+  EM_RECORD("layernorm_bwd",
+            "\"dy\":%llu,\"lddy\":%lld,\"x\":%llu,\"ldx\":%lld,\"gamma\":%llu,\"mean\":%llu,\"rstd\":%llu,"
+            "\"res\":%llu,\"ldres\":%lld,\"dx\":%llu,\"lddx\":%lld,\"rows\":%d,\"d\":%d",
+            EM_P(dy_), (long long)lddy, EM_P(x_), (long long)ldx, EM_P(gamma_), EM_P(mean), EM_P(rstd), EM_P(res_),
+            (long long)ldres, EM_P(dx_), (long long)lddx, rows, d);
   EM_TRACE(12.0 * rows * d, (double)rows * d * (res_ ? 8 : 6), "layernorm_bwd\trows=%d d=%d res=%d", rows, d, res_ != nullptr);
   EM_REQUIRE(rows > 0 && d > 0 && d % 8 == 0 && d <= 8192, MB200_E_SHAPE, "layernorm_bwd: bad d=%d", d);
   EM_REQUIRE(lddy % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!res_ || ldres % 8 == 0), MB200_E_ALIGN,
@@ -276,6 +319,11 @@ static int ln_param_grad(const void* dy_, int64_t lddy, const void* x_, int64_t 
 int mb200_layernorm_param_grad(const void* dy, int64_t lddy, const void* x, int64_t ldx, const float* mean,
                                const float* rstd, float* dgamma, float* dbeta, int32_t rows, int32_t d,
                                int32_t accumulate, void*) {
+  EM_RECORD("layernorm_param_grad",
+            "\"dy\":%llu,\"lddy\":%lld,\"x\":%llu,\"ldx\":%lld,\"mean\":%llu,\"rstd\":%llu,\"dgamma\":%llu,"
+            "\"dbeta\":%llu,\"rows\":%d,\"d\":%d,\"accumulate\":%d",
+            EM_P(dy), (long long)lddy, EM_P(x), (long long)ldx, EM_P(mean), EM_P(rstd), EM_P(dgamma), EM_P(dbeta), rows,
+            d, accumulate);
   return ln_param_grad(dy, lddy, x, ldx, mean, rstd, dgamma, dbeta, rows, d, accumulate);
 }
 int mb200_layernorm_param_grad_rows(const void* dy, int64_t lddy, const void* x, int64_t ldx, const float* mean,
@@ -284,12 +332,22 @@ int mb200_layernorm_param_grad_rows(const void* dy, int64_t lddy, const void* x,
   /* traced in ln_param_grad */
   EM_REQUIRE(rows > 0 && d > 0 && d % 2 == 0 && lddy % 2 == 0 && ldx % 2 == 0, MB200_E_ALIGN,
              "layernorm_param_grad_rows: d and row strides must be even");
+  EM_RECORD("layernorm_param_grad_rows",
+            "\"dy\":%llu,\"lddy\":%lld,\"x\":%llu,\"ldx\":%lld,\"mean\":%llu,\"rstd\":%llu,\"dgamma\":%llu,"
+            "\"dbeta\":%llu,\"rows\":%d,\"d\":%d,\"accumulate\":%d",
+            EM_P(dy), (long long)lddy, EM_P(x), (long long)ldx, EM_P(mean), EM_P(rstd), EM_P(dgamma), EM_P(dbeta), rows,
+            d, accumulate);
   return ln_param_grad(dy, lddy, x, ldx, mean, rstd, dgamma, dbeta, rows, d, accumulate);
 }
 
 // ---- softmax (elementwise.cu: softmax_fwd_kernel / softmax_bwd_kernel) ----
 int mb200_softmax_fwd(const float* s, int64_t lds, int64_t s_bs, void* p_, int64_t ldp, int64_t p_bs, int32_t nz,
                       int32_t Sq, int32_t Sk, float scale, int32_t causal, int32_t koff, void*) {
+  EM_RECORD("softmax_fwd",
+            "\"s\":%llu,\"lds\":%lld,\"s_bs\":%lld,\"p\":%llu,\"ldp\":%lld,\"p_bs\":%lld,\"nz\":%d,\"Sq\":%d,"
+            "\"Sk\":%d,\"scale\":%.9g,\"causal\":%d,\"koff\":%d",
+            EM_P(s), (long long)lds, (long long)s_bs, EM_P(p_), (long long)ldp, (long long)p_bs, nz, Sq, Sk,
+            (double)scale, causal, koff);
   EM_TRACE(5.0 * nz * Sq * Sk, (double)nz * Sq * Sk * 6, "softmax_fwd\tnz=%d Sq=%d Sk=%d causal=%d", nz, Sq, Sk, causal);
   bf16_t* p = (bf16_t*)p_;
   for (int z = 0; z < nz; ++z)
@@ -308,6 +366,11 @@ int mb200_softmax_fwd(const float* s, int64_t lds, int64_t s_bs, void* p_, int64
 
 int mb200_softmax_bwd(const float* dp, int64_t lddp, int64_t dp_bs, const void* p_, int64_t ldp, int64_t p_bs,
                       void* ds_, int64_t ldds, int64_t ds_bs, int32_t nz, int32_t Sq, int32_t Sk, float scale, void*) {
+  EM_RECORD("softmax_bwd",
+            "\"dp\":%llu,\"lddp\":%lld,\"dp_bs\":%lld,\"p\":%llu,\"ldp\":%lld,\"p_bs\":%lld,\"ds\":%llu,"
+            "\"ldds\":%lld,\"ds_bs\":%lld,\"nz\":%d,\"Sq\":%d,\"Sk\":%d,\"scale\":%.9g",
+            EM_P(dp), (long long)lddp, (long long)dp_bs, EM_P(p_), (long long)ldp, (long long)p_bs, EM_P(ds_), (long
+            long)ldds, (long long)ds_bs, nz, Sq, Sk, (double)scale);
   EM_TRACE(4.0 * nz * Sq * Sk, (double)nz * Sq * Sk * 8, "softmax_bwd\tnz=%d Sq=%d Sk=%d", nz, Sq, Sk);
   const bf16_t* p = (const bf16_t*)p_;
   bf16_t* ds = (bf16_t*)ds_;
@@ -325,6 +388,9 @@ int mb200_softmax_bwd(const float* dp, int64_t lddp, int64_t dp_bs, const void* 
 
 // ---- reductions / elementwise / ViT front end ----
 int mb200_colsum(const void* x_, int64_t ldx, int32_t rows, int32_t cols, float* out, int32_t accumulate, void*) {
+  EM_RECORD("colsum",
+            "\"x\":%llu,\"ldx\":%lld,\"rows\":%d,\"cols\":%d,\"out\":%llu,\"accumulate\":%d",
+            EM_P(x_), (long long)ldx, rows, cols, EM_P(out), accumulate);
   EM_TRACE((double)rows * cols, (double)rows * cols * 2, "colsum\trows=%d cols=%d", rows, cols);
   EM_REQUIRE(cols % 2 == 0 && ldx % 2 == 0, MB200_E_ALIGN, "colsum: cols and ldx must be even");
   const bf16_t* x = (const bf16_t*)x_;
@@ -337,6 +403,9 @@ int mb200_colsum(const void* x_, int64_t ldx, int32_t rows, int32_t cols, float*
 }
 
 int mb200_quick_gelu_bwd(const void* dy_, const void* pre_, void* dx_, int64_t n, void*) {
+  EM_RECORD("quick_gelu_bwd",
+            "\"dy\":%llu,\"pre\":%llu,\"dx\":%llu,\"n\":%lld",
+            EM_P(dy_), EM_P(pre_), EM_P(dx_), (long long)n);
   EM_TRACE(8.0 * n, (double)n * 6, "quick_gelu_bwd\tn=%lld", (long long)n);
   EM_REQUIRE(n > 0 && n % 8 == 0, MB200_E_SHAPE, "quick_gelu_bwd: n must be a positive multiple of 8");
   EM_REQUIRE(aligned16(dy_) && aligned16(pre_) && aligned16(dx_), MB200_E_ALIGN, "quick_gelu_bwd: 16B alignment");
@@ -351,6 +420,9 @@ int mb200_quick_gelu_bwd(const void* dy_, const void* pre_, void* dx_, int64_t n
 
 // out = s[0] * u + r1 + r2   (scale_add_kernel)
 int mb200_scale_add(const void* u_, const float* s, const void* r1_, const void* r2_, void* out_, int64_t n, void*) {
+  EM_RECORD("scale_add",
+            "\"u\":%llu,\"s\":%llu,\"r1\":%llu,\"r2\":%llu,\"out\":%llu,\"n\":%lld",
+            EM_P(u_), EM_P(s), EM_P(r1_), EM_P(r2_), EM_P(out_), (long long)n);
   EM_TRACE(3.0 * n, (double)n * (4 + (r1_ ? 2 : 0) + (r2_ ? 2 : 0)), "scale_add\tn=%lld", (long long)n);
   EM_REQUIRE(n > 0 && n % 8 == 0, MB200_E_SHAPE, "scale_add: n must be a positive multiple of 8");
   EM_REQUIRE(aligned16(u_) && aligned16(r1_) && aligned16(r2_) && aligned16(out_), MB200_E_ALIGN, "scale_add: alignment");
@@ -363,6 +435,9 @@ int mb200_scale_add(const void* u_, const float* s, const void* r1_, const void*
 
 // out[0] (+)= <a, b>   (dot_kernel)
 int mb200_dot(const void* a_, const void* b_, int64_t n, float* out, int32_t accumulate, void*) {
+  EM_RECORD("dot",
+            "\"a\":%llu,\"b\":%llu,\"n\":%lld,\"out\":%llu,\"accumulate\":%d",
+            EM_P(a_), EM_P(b_), (long long)n, EM_P(out), accumulate);
   EM_TRACE(2.0 * n, (double)n * 4, "dot\tn=%lld", (long long)n);
   EM_REQUIRE(n > 0 && n % 8 == 0, MB200_E_SHAPE, "dot: n must be a positive multiple of 8");
   EM_REQUIRE(aligned16(a_) && aligned16(b_), MB200_E_ALIGN, "dot: alignment");
@@ -375,6 +450,7 @@ int mb200_dot(const void* a_, const void* b_, int64_t n, float* out, int32_t acc
 
 // (cos, sin) fp32 [S][rot/2][2]   (rope_table_kernel)
 int mb200_rope_table(float* tab, int32_t S, int32_t rot, int32_t pos0, void*) {
+  EM_RECORD("rope_table", "\"tab\":%llu,\"S\":%d,\"rot\":%d,\"pos0\":%d", EM_P(tab), S, rot, pos0);
   EM_TRACE(0, (double)S * rot * 4, "rope_table\tS=%d rot=%d", S, rot);
   EM_REQUIRE(S > 0 && rot > 0 && rot % 2 == 0, MB200_E_SHAPE, "rope_table: bad S / rot");
   const int half = rot / 2;
@@ -392,6 +468,11 @@ int mb200_rope_table(float* tab, int32_t S, int32_t rot, int32_t pos0, void*) {
 // zero rows where the target is ignored; dlogits may alias logits   (ce_count / ce_row / ce_reduce kernels)
 int mb200_cross_entropy(const void* logits_, int64_t ldv, const int64_t* labels, int32_t B, int32_t S, int32_t V,
                         float* row_loss, int32_t* n_valid, float* loss, void* dlogits_, float grad_scale, void*) {
+  EM_RECORD("cross_entropy",
+            "\"logits\":%llu,\"ldv\":%lld,\"labels\":%llu,\"B\":%d,\"S\":%d,\"V\":%d,\"row_loss\":%llu,"
+            "\"n_valid\":%llu,\"loss\":%llu,\"dlogits\":%llu,\"grad_scale\":%.9g",
+            EM_P(logits_), (long long)ldv, EM_P(labels), B, S, V, EM_P(row_loss), EM_P(n_valid), EM_P(loss),
+            EM_P(dlogits_), (double)grad_scale);
   EM_TRACE(6.0 * B * S * V, (double)B * S * V * (dlogits_ ? 4 : 2), "cross_entropy\trows=%d V=%d grad=%d", B * S, V, dlogits_ != nullptr);
   EM_REQUIRE(ldv % 8 == 0 && V <= ldv, MB200_E_ALIGN, "cross_entropy: ldv must be a multiple of 8 and >= V");
   const bf16_t* logits = (const bf16_t*)logits_;
@@ -667,6 +748,10 @@ static bool tile_supported(int S, int hd) { return S >= 1 && S <= 128 && hd >= 6
 
 int mb200_attn_fwd_tile(const void* qkv_, int64_t ld, void* P_, int64_t ldP, void* O_, int64_t ldo, int32_t B, int32_t S,
                         int32_t H, int32_t hd, void*) {
+  EM_RECORD("attn_fwd_tile",
+            "\"qkv\":%llu,\"ld\":%lld,\"P\":%llu,\"ldP\":%lld,\"O\":%llu,\"ldo\":%lld,\"B\":%d,\"S\":%d,\"H\":%d,"
+            "\"hd\":%d",
+            EM_P(qkv_), (long long)ld, EM_P(P_), (long long)ldP, EM_P(O_), (long long)ldo, B, S, H, hd);
   EM_TRACE(4.0 * B * H * S * (double)S * hd, (double)B * S * H * hd * 8 + (double)B * H * S * ldP * 2, "attn_fwd_tile\tB=%d S=%d H=%d hd=%d", B, S, H, hd);
   EM_REQUIRE(tile_supported(S, hd) && ldP % 8 == 0, MB200_E_SHAPE, "attn_fwd_tile: unsupported S=%d hd=%d", S, hd);
   const bf16_t* qkv = (const bf16_t*)qkv_;
@@ -707,6 +792,13 @@ int mb200_attn_fwd_flash(const void* q_, int64_t ldq, int64_t q_bsh, int64_t q_b
                          int64_t k_bsh, int64_t k_bsb, const void* v_, int64_t ldv, int64_t v_bsh, int64_t v_bsb, void* O_,
                          int64_t ldo, void* P_, int64_t ldP, float* stats, int32_t B, int32_t Sq, int32_t Sk, int32_t H,
                          int32_t hd, int32_t causal, void*) {
+  EM_RECORD("attn_fwd_flash",
+            "\"q\":%llu,\"ldq\":%lld,\"q_bsh\":%lld,\"q_bsb\":%lld,\"k\":%llu,\"ldk\":%lld,\"k_bsh\":%lld,"
+            "\"k_bsb\":%lld,\"v\":%llu,\"ldv\":%lld,\"v_bsh\":%lld,\"v_bsb\":%lld,\"O\":%llu,\"ldo\":%lld,"
+            "\"P\":%llu,\"ldP\":%lld,\"stats\":%llu,\"B\":%d,\"Sq\":%d,\"Sk\":%d,\"H\":%d,\"hd\":%d,\"causal\":%d",
+            EM_P(q_), (long long)ldq, (long long)q_bsh, (long long)q_bsb, EM_P(k_), (long long)ldk, (long long)k_bsh,
+            (long long)k_bsb, EM_P(v_), (long long)ldv, (long long)v_bsh, (long long)v_bsb, EM_P(O_), (long long)ldo,
+            EM_P(P_), (long long)ldP, EM_P(stats), B, Sq, Sk, H, hd, causal);
   EM_TRACE(4.0 * B * H * Sq * (double)Sk * hd,  // algorithmic count (QK^T once, full rectangle), like attn_fwd_tile
            (double)B * H * (2.0 * Sq + 2.0 * Sk) * hd * 2 + (P_ ? (double)B * H * Sq * ldP * 2 : 0.0),
            "attn_fwd_flash\tB=%d Sq=%d Sk=%d H=%d hd=%d causal=%d", B, Sq, Sk, H, hd, causal);
@@ -757,6 +849,11 @@ int mb200_attn_fwd_flash(const void* q_, int64_t ldq, int64_t q_bsh, int64_t q_b
 int mb200_attn_bwd_tile(const void* qkv_, int64_t ld, const void* dO_, int64_t ld_do, const void* P_, int64_t ldP,
                         void* dqkv_, int64_t ldd, const float* rope_tab, int32_t rot, int32_t B, int32_t S, int32_t H,
                         int32_t hd, void*) {
+  EM_RECORD("attn_bwd_tile",
+            "\"qkv\":%llu,\"ld\":%lld,\"dO\":%llu,\"ld_do\":%lld,\"P\":%llu,\"ldP\":%lld,\"dqkv\":%llu,"
+            "\"ldd\":%lld,\"rope_tab\":%llu,\"rot\":%d,\"B\":%d,\"S\":%d,\"H\":%d,\"hd\":%d",
+            EM_P(qkv_), (long long)ld, EM_P(dO_), (long long)ld_do, EM_P(P_), (long long)ldP, EM_P(dqkv_), (long
+            long)ldd, EM_P(rope_tab), rot, B, S, H, hd);
   EM_TRACE(10.0 * B * H * S * (double)S * hd, (double)B * S * H * hd * 14 + (double)B * H * S * ldP * 2, "attn_bwd_tile\tB=%d S=%d H=%d hd=%d", B, S, H, hd);
   EM_REQUIRE(tile_supported(S, hd) && ldP % 8 == 0, MB200_E_SHAPE, "attn_bwd_tile: unsupported S=%d hd=%d", S, hd);
   const bf16_t *qkv = (const bf16_t*)qkv_, *dO = (const bf16_t*)dO_, *P = (const bf16_t*)P_;
@@ -819,6 +916,10 @@ int mb200_attn_bwd_tile(const void* qkv_, int64_t ld, const void* dO_, int64_t l
 // KV cache   (kv_attention.cu: kv_append_kernel / attn_decode_kernel)
 int mb200_kv_append(const void* qkv_, int64_t ld, void* kc_, void* vc_, int32_t B, int32_t S, int32_t H, int32_t hd,
                     int32_t Smax, int32_t pos0, void*) {
+  EM_RECORD("kv_append",
+            "\"qkv\":%llu,\"ld\":%lld,\"kc\":%llu,\"vc\":%llu,\"B\":%d,\"S\":%d,\"H\":%d,\"hd\":%d,\"Smax\":%d,"
+            "\"pos0\":%d",
+            EM_P(qkv_), (long long)ld, EM_P(kc_), EM_P(vc_), B, S, H, hd, Smax, pos0);
   EM_TRACE(0, (double)B * S * H * hd * 8, "kv_append\tB=%d S=%d H=%d hd=%d", B, S, H, hd);
   EM_REQUIRE(hd % 8 == 0 && B > 0 && S > 0 && pos0 >= 0 && pos0 + S <= Smax, MB200_E_SHAPE, "kv_append: bad shape");
   const bf16_t* qkv = (const bf16_t*)qkv_;
@@ -838,6 +939,10 @@ int mb200_kv_append(const void* qkv_, int64_t ld, void* kc_, void* vc_, int32_t 
 // rounded to bf16 before P*V like the prefill path
 int mb200_attn_decode(const void* qkv_, int64_t ld_qkv, void* kc_, void* vc_, void* out_, int64_t ld_out, int32_t B,
                       int32_t H, int32_t hd, int32_t Smax, int32_t pos, void*) {
+  EM_RECORD("attn_decode",
+            "\"qkv\":%llu,\"ld_qkv\":%lld,\"kc\":%llu,\"vc\":%llu,\"out\":%llu,\"ld_out\":%lld,\"B\":%d,\"H\":%d,"
+            "\"hd\":%d,\"Smax\":%d,\"pos\":%d",
+            EM_P(qkv_), (long long)ld_qkv, EM_P(kc_), EM_P(vc_), EM_P(out_), (long long)ld_out, B, H, hd, Smax, pos);
   EM_TRACE(4.0 * B * H * (double)(pos + 1) * hd, (double)B * H * (pos + 1) * hd * 4, "attn_decode\tB=%d H=%d hd=%d pos=%d", B, H, hd, pos);
   EM_REQUIRE(hd % 8 == 0 && pos >= 0 && pos < Smax, MB200_E_SHAPE, "attn_decode: bad hd / pos");
   const bf16_t* qkv = (const bf16_t*)qkv_;
@@ -990,6 +1095,9 @@ int mb200_avgpool_nhwc_bwd(const void* dy_, void* dx_, int32_t B, int32_t H, int
 
 // images [B,3,R,R] -> patches [B*g*g][ldp], column order (c, py, px)   (patchify_kernel)
 int mb200_patchify(const void* img_, void* patches_, int64_t ldp, int32_t B, int32_t R, int32_t P, void*) {
+  EM_RECORD("patchify",
+            "\"img\":%llu,\"patches\":%llu,\"ldp\":%lld,\"B\":%d,\"R\":%d,\"P\":%d",
+            EM_P(img_), EM_P(patches_), (long long)ldp, B, R, P);
   EM_TRACE(0, (double)B * 3 * R * R * 4, "patchify\tB=%d R=%d P=%d", B, R, P);
   EM_REQUIRE(R % P == 0 && ldp >= 3 * P * P, MB200_E_SHAPE, "patchify: bad geometry");
   const bf16_t* img = (const bf16_t*)img_;
@@ -1009,6 +1117,9 @@ int mb200_patchify(const void* img_, void* patches_, int64_t ldp, int32_t B, int
 // x[b,0] = cls + pos[0]; x[b,1+p] = pe[b,p] + pos[1+p]   (vit_assemble_kernel)
 int mb200_vit_assemble(void* x_, const void* pe_, const void* cls_, const void* pos_, int32_t B, int32_t T, int32_t w,
                        void*) {
+  EM_RECORD("vit_assemble",
+            "\"x\":%llu,\"pe\":%llu,\"cls\":%llu,\"pos\":%llu,\"B\":%d,\"T\":%d,\"w\":%d",
+            EM_P(x_), EM_P(pe_), EM_P(cls_), EM_P(pos_), B, T, w);
   EM_TRACE((double)B * T * w, (double)B * T * w * 4, "vit_assemble\tB=%d T=%d w=%d", B, T, w);
   bf16_t* x = (bf16_t*)x_;
   const bf16_t *pe = (const bf16_t*)pe_, *cls = (const bf16_t*)cls_, *pos = (const bf16_t*)pos_;

@@ -652,14 +652,15 @@ def _rounded(name, got, ref, delta, limit=AMBIGUOUS_MAX):
     check_rounded(name, got, ref, 1.001 * delta + TINY, torch.ones(1, dtype=torch.bool, device=ref.device), limit=limit)
 
 
-def test_quick_gelu_bwd():
+def test_quick_gelu_bwd(n=None):
+    """n: the element count (tests/test_production_launches_gpu.py replays the production one)."""
     import torch
 
     from magma_b200 import ops
 
     name = "quick_gelu_bwd"
     dev, bf = _dev(), torch.bfloat16
-    n = 1 << 18 if dev.type == "cuda" else 4096
+    n = n or (1 << 18 if dev.type == "cuda" else 4096)
     gen = _gen("qgelu", n)
     pre = torch.linspace(-20, 20, n, dtype=torch.float64).to(bf).to(dev)
     dy = torch.randn(n, generator=gen, dtype=torch.float64).to(bf).to(dev)
@@ -754,13 +755,14 @@ def test_add(with_c):
     _rounded(name, out[:n], ref, d + _add_err(ref, q))
 
 
-def test_vit_assemble():
+def test_vit_assemble(shape=None):
+    """shape: (B, T, w) (tests/test_production_launches_gpu.py replays the production one)."""
     import torch
 
     from magma_b200 import ops
 
     dev, bf = _dev(), torch.bfloat16
-    B, T, w = (2, 257, 1024) if dev.type == "cuda" else (2, 5, 16)
+    B, T, w = shape or ((2, 257, 1024) if dev.type == "cuda" else (2, 5, 16))
     name = f"vit_assemble B={B} T={T} w={w}"
     gen = _gen("vit_assemble", B, T, w)
     pe, cls, pos = (torch.randn(*s, generator=gen, dtype=torch.float64).to(bf).to(dev)
@@ -924,13 +926,14 @@ def test_channel_affine(full, relu):
 # ---------------------------------------------------------------------------------------------
 # E. bit-exact layout, gathers, casts, dropout, argmax
 # ---------------------------------------------------------------------------------------------
-def test_patchify_vit_front_end():
+def test_patchify_vit_front_end(shape=None):
+    """shape: (B, R, P) (tests/test_production_launches_gpu.py replays the production one)."""
     import torch
 
     from magma_b200 import ops
 
     dev, bf = _dev(), torch.bfloat16
-    B, R, P = (2, 224, 14) if dev.type == "cuda" else (2, 28, 14)
+    B, R, P = shape or ((2, 224, 14) if dev.type == "cuda" else (2, 28, 14))
     g = R // P
     K = 3 * P * P
     name = f"patchify B={B} R={R} P={P}"

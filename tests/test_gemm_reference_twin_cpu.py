@@ -8,7 +8,8 @@ import pytest
 import test_gemm_reference_gpu as G
 
 
-@pytest.mark.parametrize("shape", [(65, 203, 40), (127, 45, 8), (129, 67, 72)], ids=lambda s: "x".join(map(str, s)))
+@pytest.mark.parametrize("shape", [(65, 203, 40), (127, 45, 8), (129, 67, 72), (33, 45, 12), (20, 37, 588)],
+                         ids=lambda s: "x".join(map(str, s)))
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, False), (True, True)],
                          ids=["KK", "KMN", "MNK", "MNMN"])
 def test_tiles_and_majors_body_on_emulation(emul_ops, monkeypatch, a_mn, b_mn, shape):
