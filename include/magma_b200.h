@@ -446,6 +446,32 @@ int mb200_gptj_sched_backward_range_hidden_recompute(const mb200_gptj_model_ex* 
                                                      float loss_scale, int32_t layer_hi, int32_t layer_lo,
                                                      int32_t accumulate, int32_t B, int32_t S, void* ws, size_t ws_bytes,
                                                      void* stream);
+/* output_attentions of the training pass (GPTNeoForCausalLM.forward(output_attentions=True) returns one [B, H, S, S]
+ * tensor per block, the softmax probabilities that multiply V, hf:gptj/modeling_gptj.py:145-151; the adapter wrappers
+ * pass them through, magma/adapters.py:85-92,109-116). mb200_gptj_sched_forward(_recompute) that also writes block l's
+ * bf16 probabilities to attn[l] ([B,H,S,ld_attn], NULL entries skipped) as the block runs: zeros above the causal
+ * diagonal, the values P V used. They share the layout of the saved probabilities, so ld_attn must be S rounded up to 8
+ * (MB200_E_ALIGN otherwise). */
+int mb200_gptj_sched_forward_attn(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels, void* logits,
+                                  int64_t ldv, float* loss, void* const* attn, int64_t ld_attn, int32_t B, int32_t S,
+                                  void* ws, size_t ws_bytes, void* stream);
+int mb200_gptj_sched_forward_attn_recompute(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels,
+                                            void* logits, int64_t ldv, float* loss, void* const* attn, int64_t ld_attn,
+                                            int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream);
+/* The backward of a loss that reads hidden states and / or attention probabilities, in one pass: dhidden as in
+ * mb200_gptj_sched_backward_range_hidden (NULL, or n_layer + 1 pointers each NULL or bf16 [B*S, d]); dattn NULL, or
+ * n_layer pointers each NULL or the bf16 [B,H,S,ld_attn] gradient of attn[l] (ld_attn = S rounded up to 8). Layer l's
+ * attention gradient is added to dP = dO V^T before rowsum(dP * P) (mb200_attn_bwd_tile_dp for S <= 128, the dP GEMM's
+ * residual otherwise), by the call whose layer range holds l. With every pointer NULL the result equals
+ * mb200_gptj_sched_backward_range(_recompute). */
+int mb200_gptj_sched_backward_range_attn(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden, void* const* dattn,
+                                         int64_t ld_attn, float loss_scale, int32_t layer_hi, int32_t layer_lo,
+                                         int32_t accumulate, int32_t B, int32_t S, void* ws, size_t ws_bytes,
+                                         void* stream);
+int mb200_gptj_sched_backward_range_attn_recompute(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                   void* const* dattn, int64_t ld_attn, float loss_scale,
+                                                   int32_t layer_hi, int32_t layer_lo, int32_t accumulate, int32_t B,
+                                                   int32_t S, void* ws, size_t ws_bytes, void* stream);
 /* Inference pass (no saved activations) — use_cache=True of magma/sampling.py:81-90: kcache / vcache bf16
  * [n_layer][B][H][S_kv_max][hd] or NULL; the K / V of this call are written at positions [pos0, pos0 + S) and attention
  * runs over [0, pos0 + S) (prefill S > 1 through mb200_attn_fwd_flash, decode S == 1 through mb200_attn_decode).
@@ -463,6 +489,15 @@ int mb200_gptj_sched_infer(const mb200_gptj_model_ex* m, const void* x, void* lo
 int mb200_gptj_sched_infer_hidden(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv, int32_t last_only,
                                   void* hidden_all, int64_t ld_hidden, void* kcache, void* vcache, int32_t S_kv_max,
                                   int32_t pos0, int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream);
+/* The inference pass with output_attentions (and, when hidden_all != NULL, output_hidden_states as above): attn holds
+ * n_layer pointers, each NULL or bf16 [B,H,S,ld_attn] with ld_attn >= S_kv = pos0 + S and % 8. Block l writes the
+ * probabilities it multiplies V with there — mb200_attn_fwd_flash's P output, the materialised softmax's output, or
+ * mb200_attn_decode_probs for a decode step — zeros above the causal diagonal. Not available with a device-side
+ * position (mb200_gptj_sched_decode_step). */
+int mb200_gptj_sched_infer_attn(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv, int32_t last_only,
+                                void* hidden_all, int64_t ld_hidden, void* const* attn, int64_t ld_attn, void* kcache,
+                                void* vcache, int32_t S_kv_max, int32_t pos0, int32_t B, int32_t S, void* ws,
+                                size_t ws_bytes, void* stream);
 
 /* Device-resident decode loop (magma/sampling.py:78-109 issues one LM call per generated token from the host and syncs
  * on `.all()` every step). Here the cache position of the step lives in DEVICE memory (pos_dev, int32[1]): no argument
@@ -510,6 +545,13 @@ int mb200_attn_fwd_tile(const void* qkv, int64_t ld_qkv, void* P, int64_t ldP, v
 int mb200_attn_bwd_tile(const void* qkv, int64_t ld_qkv, const void* dO, int64_t ld_do, const void* P, int64_t ldP,
                         void* dqkv, int64_t ld_dqkv, const float* rope_tab, int32_t rot, int32_t B, int32_t S, int32_t H,
                         int32_t hd, void* stream);
+/* mb200_attn_bwd_tile with a gradient on P from outside the block (output_attentions in training; the adapter wrappers
+ * pass the probabilities on, magma/adapters.py:85-92,109-116): dP_ext, bf16 [B,H,S,ld_dpe] (ld_dpe >= S and % 8;
+ * entries in rows or columns >= S are not read), is added to dP = dO V^T before dS = P * (dP - rowsum(dP * P)) /
+ * sqrt(hd). A separate instantiation of the kernel; mb200_attn_bwd_tile is unchanged. */
+int mb200_attn_bwd_tile_dp(const void* qkv, int64_t ld_qkv, const void* dO, int64_t ld_do, const void* P, int64_t ldP,
+                           const void* dP_ext, int64_t ld_dpe, void* dqkv, int64_t ld_dqkv, const float* rope_tab,
+                           int32_t rot, int32_t B, int32_t S, int32_t H, int32_t hd, void* stream);
 /* The forward attention for ANY sequence length (multi-tile): one CTA per (128-query tile, head, batch) sweeps the key
  * tiles twice (row max / sum, then bf16 probabilities and O += P V in wgmma register accumulators), so no [B,H,S,S]
  * fp32 score buffer exists and the probabilities are rounded to bf16 where the materialised softmax rounds them (the
@@ -532,6 +574,12 @@ int mb200_attn_fwd_flash(const void* q, int64_t ldq, int64_t q_bsh, int64_t q_bs
  * Replaces the torch.cat cache growth + _attn of hf:gptj/modeling_gptj.py:209-214,136-149 per step. */
 int mb200_attn_decode(const void* qkv, int64_t ld_qkv, void* kcache, void* vcache, void* out, int64_t ld_out,
                       int32_t B, int32_t H, int32_t hd, int32_t S_kv_max, int32_t pos, void* stream);
+/* mb200_attn_decode that also writes the bf16 probabilities it multiplies V with to row b*H + h of probs (row stride
+ * ld_probs > pos), zeros in columns pos + 1 .. ld_probs - 1: output_attentions of a decode step, the last query row of
+ * hf:gptj/modeling_gptj.py:145-146 over the cache. A separate instantiation; mb200_attn_decode is unchanged. */
+int mb200_attn_decode_probs(const void* qkv, int64_t ld_qkv, void* kcache, void* vcache, void* out, int64_t ld_out,
+                            void* probs, int64_t ld_probs, int32_t B, int32_t H, int32_t hd, int32_t S_kv_max, int32_t pos,
+                            void* stream);
 /* K/V of S positions (prefill) from the fused, rotated qkv rows [B*S][3][H][hd] into one layer's static cache
  * [B][H][S_kv_max][hd] at positions [pos0, pos0 + S) — the in-place replacement of the torch.cat cache growth of
  * hf:gptj/modeling_gptj.py:209-214 for S > 1. */

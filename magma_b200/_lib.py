@@ -251,11 +251,20 @@ SIGNATURES = {
                                                       _vp]),
     "mb200_gptj_sched_backward_range_hidden_recompute": (_i32, [_GPTJ, _vp, _VPP, _f32, _i32, _i32, _i32, _i32, _i32,
                                                                 _vp, _sz, _vp]),
+    "mb200_gptj_sched_forward_attn": (_i32, [_GPTJ, _vp, _vp, _vp, _i64, _vp, _VPP, _i64, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_forward_attn_recompute": (_i32, [_GPTJ, _vp, _vp, _vp, _i64, _vp, _VPP, _i64, _i32, _i32, _vp, _sz,
+                                                       _vp]),
+    "mb200_gptj_sched_backward_range_attn": (_i32, [_GPTJ, _vp, _VPP, _VPP, _i64, _f32, _i32, _i32, _i32, _i32, _i32, _vp,
+                                                    _sz, _vp]),
+    "mb200_gptj_sched_backward_range_attn_recompute": (_i32, [_GPTJ, _vp, _VPP, _VPP, _i64, _f32, _i32, _i32, _i32, _i32,
+                                                              _i32, _vp, _sz, _vp]),
     "mb200_gptj_sched_infer_workspace_bytes": (_sz, [_GPTJ, _i32, _i32, _i32]),
     "mb200_gptj_sched_infer": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz,
                                       _vp]),
     "mb200_gptj_sched_infer_hidden": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32,
                                              _vp, _sz, _vp]),
+    "mb200_gptj_sched_infer_attn": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _i64, _VPP, _i64, _vp, _vp, _i32, _i32, _i32,
+                                           _i32, _vp, _sz, _vp]),
     "mb200_gptj_sched_decode_step": (_i32, [_GPTJ, _vp, _vp, _i64, _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
     "mb200_decode_embed": (_i32, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "mb200_decode_advance": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _vp]),
@@ -266,9 +275,12 @@ SIGNATURES = {
     "mb200_dot": (_i32, [_vp, _vp, _i64, _vp, _i32, _vp]),
     "mb200_attn_fwd_tile": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
     "mb200_attn_bwd_tile": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_attn_bwd_tile_dp": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32,
+                                      _i32, _vp]),
     "mb200_attn_fwd_flash": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _vp,
                                     _i64, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mb200_attn_decode": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mb200_attn_decode_probs": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mb200_kv_append": (_i32, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
 }
 

@@ -19,6 +19,8 @@
 //   dP = dO V^T ; dS = P*(dP - rowsum(dP*P))/sqrt(hd) ; dV = P^T dO (P, dO as MN-major operands: same smem bytes)
 //   dQ = dS K ; dK = dS^T Q, both with the inverse rotary rotation applied on the way out (they are gradients of the
 //   rotated q,k), written straight into the fused dqkv buffer.
+//   The EXT_DP instantiation adds a gradient that reaches P from outside the block (a loss reading the returned
+//   attention probabilities) to dP before the row sum: the same algebra, dP = dO V^T + dP_ext.
 #include <stdlib.h>
 
 #include "gemm_common.cuh"
@@ -40,6 +42,9 @@ struct AttnParams {
   bf16* dqkv;
   long long ld_dqkv;
   const float2* rope_tab;  // [S][rot/2] (cos, sin), positions 0..S-1
+  // backward input of attn_bwd_tile_kernel<HD, true>: the gradient on P from outside the block, [B,H,S,ld_dpe]
+  const bf16* dPe;
+  long long ld_dpe;
 };
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -219,7 +224,7 @@ attn_fwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 // ---------------------------------------------------------------------------------------------
 // backward
 // ---------------------------------------------------------------------------------------------
-template <int HD>
+template <int HD, bool EXT_DP>
 __global__ void __launch_bounds__(kAttThreads, 1)
 attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
@@ -265,9 +270,41 @@ attn_bwd_tile_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   }
   const uint32_t R3_s = smem_u32(R3), R4_s = smem_u32(R4);
   {
+    // dP_ext, read straight into the fragment's layout from global memory and issued before the wgmma so the loads
+    // overlap it. Every element is read once by one thread, so a TMA tile (32 KB, which would still fit next to the
+    // 193 KB of hd = 256) would buy no reuse. Elements at rows or columns >= S (the caller's row padding) read as zero:
+    // P is zero there, but 0 * NaN would not be.
+    uint32_t ext[EXT_DP ? 32 : 1];
+    if (EXT_DP) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int q = f.r0 + 8 * hh;
+        const bf16* erow = p.dPe + (((long long)b * p.H + h) * p.S + q) * p.ld_dpe;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + f.c0;
+          uint32_t v = 0u;
+          if (q < p.S && c < p.S) {
+            v = __ldg(reinterpret_cast<const unsigned int*>(erow + c));
+            if (c + 1 >= p.S) v &= 0xffffu;  // low half = column c
+          }
+          ext[16 * hh + j] = v;
+        }
+      }
+    }
     mbar_wait(bar_a, 0);
     float dp[64];
     wg_mma<128, false, false>(dp, f.wg, smem_u32(R1), smem_u32(R2), nhb);  // dP[q,k] = dO V^T
+    if (EXT_DP) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 e = bf16x2_to_f32(ext[16 * hh + j]);
+          dp[4 * j + 2 * hh] += e.x;
+          dp[4 * j + 2 * hh + 1] += e.y;
+        }
+    }
     // ---- dS = P * (dP - rowsum(dP * P)) / sqrt(hd); P as loaded by TMA (zeros beyond S) ----
     mbar_wait(bar_p, 0);
 #pragma unroll
@@ -573,10 +610,13 @@ int attn_fwd_tile(const bf16* qkv, long long ld_qkv, bf16* P, long long ldP, bf1
   return 0;
 }
 
+// dPe (NULL, or the bf16 [B,H,S,ld_dpe] gradient on P) selects the instantiation that adds it to dP
 int attn_bwd_tile(const bf16* qkv, long long ld_qkv, const bf16* dO, long long ld_do, const bf16* P, long long ldP,
-                  bf16* dqkv, long long ld_dqkv, const float* rope_tab, int rot, int B, int S, int H, int hd,
-                  cudaStream_t st) {
+                  const bf16* dPe, long long ld_dpe, bf16* dqkv, long long ld_dqkv, const float* rope_tab, int rot, int B,
+                  int S, int H, int hd, cudaStream_t st) {
   MB_REQUIRE(attn_tile_supported(S, hd) && ldP % 8 == 0, MB200_E_SHAPE, "attn_bwd_tile: unsupported S=%d hd=%d", S, hd);
+  MB_REQUIRE(dPe == nullptr || (ld_dpe >= S && ld_dpe % 8 == 0 && (reinterpret_cast<uintptr_t>(dPe) & 3) == 0),
+             MB200_E_ALIGN, "attn_bwd_tile_dp: ld_dpe=%lld must be >= S and %%8, dP_ext 4-byte aligned", ld_dpe);
   CUtensorMap tq, tk, tv, tdo, tp;
   const long long d = (long long)H * hd;
   int rc;
@@ -597,22 +637,34 @@ int attn_bwd_tile(const bf16* qkv, long long ld_qkv, const bf16* dO, long long l
   p.dqkv = dqkv;
   p.ld_dqkv = ld_dqkv;
   p.rope_tab = reinterpret_cast<const float2*>(rope_tab);
+  p.dPe = dPe;
+  p.ld_dpe = ld_dpe;
   const int smem = (2 * (hd / 64) + 4) * kTile + 1024 + 128;
-#define MB_BWD(HD)                                                                                                   \
+#define MB_BWD(HD, EXT)                                                                                               \
   {                                                                                                                  \
     static bool set = false;                                                                                         \
     if (!set) {                                                                                                      \
-      MB_CUDA(cudaFuncSetAttribute(attn_bwd_tile_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)); \
+      MB_CUDA(cudaFuncSetAttribute(attn_bwd_tile_kernel<HD, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
+                                   smem_max));                                                                       \
       set = true;                                                                                                    \
     }                                                                                                                \
-    MB_CUDA(launch_pdl(attn_bwd_tile_kernel<HD>, dim3(B * H), dim3(kAttThreads), (size_t)smem, st, tq, tk, tv, tdo,  \
-                       tp, p));                                                                                      \
+    MB_CUDA(launch_pdl(attn_bwd_tile_kernel<HD, EXT>, dim3(B * H), dim3(kAttThreads), (size_t)smem, st, tq, tk, tv,  \
+                       tdo, tp, p));                                                                                 \
   }
-  switch (hd) {
-    case 64: MB_BWD(64) break;
-    case 128: MB_BWD(128) break;
-    case 192: MB_BWD(192) break;
-    default: MB_BWD(256) break;
+  if (dPe == nullptr) {
+    switch (hd) {
+      case 64: MB_BWD(64, false) break;
+      case 128: MB_BWD(128, false) break;
+      case 192: MB_BWD(192, false) break;
+      default: MB_BWD(256, false) break;
+    }
+  } else {
+    switch (hd) {
+      case 64: MB_BWD(64, true) break;
+      case 128: MB_BWD(128, true) break;
+      case 192: MB_BWD(192, true) break;
+      default: MB_BWD(256, true) break;
+    }
   }
 #undef MB_BWD
   count_launch();
@@ -695,7 +747,19 @@ extern "C" int mb200_attn_bwd_tile(const void* qkv, int64_t ld_qkv, const void* 
   int rc = mb200::check_arch();
   if (rc) return rc;
   return mb200::attn_bwd_tile((const mb200::bf16*)qkv, ld_qkv, (const mb200::bf16*)dO, ld_do, (const mb200::bf16*)P, ldP,
-                              (mb200::bf16*)dqkv, ld_dqkv, rope_tab, rot, B, S, H, hd, (cudaStream_t)stream);
+                              nullptr, 0, (mb200::bf16*)dqkv, ld_dqkv, rope_tab, rot, B, S, H, hd, (cudaStream_t)stream);
+}
+
+extern "C" int mb200_attn_bwd_tile_dp(const void* qkv, int64_t ld_qkv, const void* dO, int64_t ld_do, const void* P,
+                                      int64_t ldP, const void* dP_ext, int64_t ld_dpe, void* dqkv, int64_t ld_dqkv,
+                                      const float* rope_tab, int32_t rot, int32_t B, int32_t S, int32_t H, int32_t hd,
+                                      void* stream) {
+  int rc = mb200::check_arch();
+  if (rc) return rc;
+  MB_REQUIRE(dP_ext != nullptr, MB200_E_ARG, "attn_bwd_tile_dp: dP_ext is NULL");
+  return mb200::attn_bwd_tile((const mb200::bf16*)qkv, ld_qkv, (const mb200::bf16*)dO, ld_do, (const mb200::bf16*)P, ldP,
+                              (const mb200::bf16*)dP_ext, ld_dpe, (mb200::bf16*)dqkv, ld_dqkv, rope_tab, rot, B, S, H, hd,
+                              (cudaStream_t)stream);
 }
 
 extern "C" int mb200_attn_fwd_flash(const void* q, int64_t ldq, int64_t q_bsh, int64_t q_bsb, const void* k, int64_t ldk,

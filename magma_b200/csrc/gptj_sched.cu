@@ -28,6 +28,12 @@
 
 #include <stdlib.h>
 
+// The two kernels only output_attentions uses are weak references: the CPU build of this file (oracle/build_emul.py)
+// links an emulation that may not carry them and must still load. A pass that needs one that is absent fails with
+// MB200_E_ARG; the CUDA library always defines both.
+#pragma weak mb200_attn_bwd_tile_dp
+#pragma weak mb200_attn_decode_probs
+
 namespace mb200 {
 namespace {
 
@@ -326,18 +332,27 @@ int layer_fwd(const mb200_gptj_model_ex* m, Plan& P, int l, bf16s* xout, void* s
   return 0;
 }
 
+// attn (NULL, or n_layer pointers, each NULL or bf16 [B,H,S,ld_attn]): output_attentions, each block's probabilities
+// copied out of P.acts[l].P as soon as the block has run (on the recompute path the next block overwrites them). The
+// saved P and the gradients on it share its layout, so ld_attn must be the plan's ldP = S rounded up to 8.
 int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels, bf16s* logits, long long ldv,
-            float* loss, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute) {
+            float* loss, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute,
+            bf16s* const* attn = nullptr, long long ld_attn = 0) {
   Plan P;
   MBS_TRY(make_plan(P, m, B, S, ws, recompute));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_forward: workspace too small (%zu < %zu)",
               ws_bytes, P.bytes);
+  MBS_REQUIRE(!attn || ld_attn == P.ldP, MB200_E_ALIGN, "gptj_sched_forward_attn: ld_attn=%lld must be %d (S rounded up to 8)",
+              ld_attn, P.ldP);
   const int M = P.M, d = P.d;
   ScratchScope scratch(P.gemm_ws, P.gemm_ws_bytes);
   MBS_TRY(mb200_rope_table(P.rope_tab, S, m->rotary_dim, 0, st));
   MBS_TRY(rt_copy(P.acts[0].x_in, x, (size_t)M * d * sizeof(bf16s), st));
-  for (int l = 0; l < m->n_layer; ++l)
+  for (int l = 0; l < m->n_layer; ++l) {
     MBS_TRY(layer_fwd(m, P, l, l + 1 < m->n_layer ? P.acts[l + 1].x_in : P.x_final, st));
+    if (attn && attn[l])
+      MBS_TRY(rt_copy(attn[l], P.acts[l].P, (size_t)B * P.H * S * P.ldP * sizeof(bf16s), st));
+  }
   // ln_f + LM head (+ shifted cross-entropy; the logits' gradient is written now, scaled in backward)
   MBS_TRY(mb200_layernorm_fwd(P.x_final, d, m->lnf_g, m->lnf_b, P.xf_ln, d, P.lnf_mean, P.lnf_rstd, M, d, m->ln_eps, st));
   bf16s* lg = logits ? logits : P.dlogits;
@@ -366,11 +381,17 @@ int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels,
 // Entry l < n_layer is layer l's input, so its gradient joins the residual-stream gradient once layer l's backward has
 // produced it (entry 0 thus reaches dx); the ln_f entry joins the LM head's dgrad in that GEMM's epilogue. Each entry is
 // added by the one call whose range holds its layer, so a chunked backward adds it once.
+// dattn (NULL, or n_layer pointers, each NULL or bf16 [B,H,S,ld_attn] with ld_attn = ldP): gradients of the attention
+// probabilities forward() returned. Layer l's joins dP = dO V^T before rowsum(dP * P) — in the tile kernel's fragment
+// (mb200_attn_bwd_tile_dp), or as the dP GEMM's residual on the materialised path.
 int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, float loss_scale, int layer_hi,
-             int layer_lo, int acc, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute) {
+             int layer_lo, int acc, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute,
+             const bf16s* const* dattn = nullptr, long long ld_attn = 0) {
   Plan P;
   MBS_TRY(make_plan(P, m, B, S, ws, recompute));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_backward: workspace too small");
+  MBS_REQUIRE(!dattn || ld_attn == P.ldP, MB200_E_ALIGN,
+              "gptj_sched_backward_range_attn: ld_attn=%lld must be %d (S rounded up to 8)", ld_attn, P.ldP);
   MBS_REQUIRE(0 <= layer_lo && layer_lo <= layer_hi && layer_hi <= m->n_layer, MB200_E_ARG,
               "gptj_sched_backward: bad layer range [%d,%d)", layer_lo, layer_hi);
   const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd;
@@ -425,12 +446,17 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, 
       dh_acc = P.dhp;
     }
     MBS_TRY(gemm(st, M, d, d, mat(da, d), wmat(L.w_out, d, 1), P.dattn_o, d, 0));  // d(attn_o) = da Wo
-    if (tile_ok(S, hd)) {
+    const bf16s* dPe = dattn ? dattn[l] : nullptr;
+    if (tile_ok(S, hd) && dPe) {
+      MBS_REQUIRE(mb200_attn_bwd_tile_dp, MB200_E_ARG, "gptj_sched: mb200_attn_bwd_tile_dp is not in this build");
+      MBS_TRY(mb200_attn_bwd_tile_dp(a.qkv, 3 * d, P.dattn_o, d, a.P, P.ldP, dPe, ld_attn, P.dqkv, 3 * d, P.rope_tab,
+                                     m->rotary_dim, B, S, H, hd, st));
+    } else if (tile_ok(S, hd)) {
       MBS_TRY(mb200_attn_bwd_tile(a.qkv, 3 * d, P.dattn_o, d, a.P, P.ldP, P.dqkv, 3 * d, P.rope_tab, m->rotary_dim, B, S, H,
                                   hd, st));
     } else {  // dQ, dK w.r.t. the rotated q, k: inverse rotation in the epilogue
       MBS_TRY(attn_bwd_gemm(st, a.qkv, a.P, P.dattn_o, P.dqkv, P.scores, P.dS, P.ldP, S, H, B, hd,
-                            rope_epi(P.rope_tab, -1, S, hd, m->rotary_dim, hd)));
+                            rope_epi(P.rope_tab, -1, S, hd, m->rotary_dim, hd), dPe));
     }
     {
       Epi e;
@@ -510,9 +536,13 @@ int make_infer_plan(InferPlan& P, const mb200_gptj_model_ex* m, int B, int S, in
 // hidden_all != NULL: n_layer + 1 hidden states of the S positions of this call, entry l at hidden_all + l * ld_hidden:
 // x, the outputs of blocks 0 .. n_layer-2 (each block writes its output there directly) and ln_f of the last block's
 // output over all S rows, also when last_only projects the last row alone.
+// attn != NULL: n_layer pointers, each NULL or bf16 [B,H,S,ld_attn] (ld_attn >= Sk = pos0 + S and % 8), which receive
+// the probabilities each block multiplies V with: the fused kernels and the softmax write them there in place of
+// their own buffer, a decode step through mb200_attn_decode_probs.
 int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, long long ldv, int last_only, bf16s* hidden,
                   bf16s* kcache, bf16s* vcache, int Smax, int pos0, int B, int S, void* ws, size_t ws_bytes, void* st,
-                  const int32_t* pos_dev = nullptr, bf16s* hidden_all = nullptr, long long ld_hidden = 0) {
+                  const int32_t* pos_dev = nullptr, bf16s* hidden_all = nullptr, long long ld_hidden = 0,
+                  bf16s* const* attn = nullptr, long long ld_attn = 0) {
   InferPlan P;
   MBS_TRY(make_infer_plan(P, m, B, S, kcache ? Smax : S, ws));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_infer: workspace too small (%zu < %zu)",
@@ -532,6 +562,8 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
   MBS_REQUIRE(!hidden_all || (ld_hidden >= (long long)M * d && ld_hidden % 8 == 0), MB200_E_ALIGN,
               "gptj_sched_infer_hidden: ld_hidden=%lld must be >= B*S*d and %%8", ld_hidden);
   const int Sk = kcache ? pos0 + S : S;
+  MBS_REQUIRE(!attn || (!pos_dev && ld_attn >= Sk && ld_attn % 8 == 0), MB200_E_ALIGN,
+              "gptj_sched_infer_attn: ld_attn=%lld must be >= %d and %%8", ld_attn, Sk);
   const size_t cache_layer = (size_t)B * H * Smax * hd;
   ScratchScope scratch(P.splitk, P.splitk_bytes);
   if (pos_dev) MBS_TRY(mb200_rope_table_dev(P.rope_tab, S, m->rotary_dim, pos_dev, st));
@@ -547,8 +579,12 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
                  rope_epi(P.rope_tab, 1, S, hd, m->rotary_dim, 2 * d)));
     bf16s* kc = kcache ? kcache + (size_t)l * cache_layer : nullptr;
     bf16s* vc = vcache ? vcache + (size_t)l * cache_layer : nullptr;
+    bf16s* Pl = attn ? attn[l] : nullptr;  // this block's probabilities, when asked for
     if (kcache && S == 1 && pos_dev) {
       MBS_TRY(mb200_attn_decode_dev(P.qkv, 3 * d, kc, vc, P.attn_o, d, B, H, hd, Smax, pos_dev, st));
+    } else if (kcache && S == 1 && Pl) {
+      MBS_REQUIRE(mb200_attn_decode_probs, MB200_E_ARG, "gptj_sched: mb200_attn_decode_probs is not in this build");
+      MBS_TRY(mb200_attn_decode_probs(P.qkv, 3 * d, kc, vc, P.attn_o, d, Pl, ld_attn, B, H, hd, Smax, pos0, st));
     } else if (kcache && S == 1) {
       MBS_TRY(mb200_attn_decode(P.qkv, 3 * d, kc, vc, P.attn_o, d, B, H, hd, Smax, pos0, st));
     } else if (flash_ok(hd)) {  // prompts of any length and prefill continuations: fused forward over qkv or the cache
@@ -556,11 +592,11 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
       if (kcache) {
         MBS_TRY(mb200_kv_append(P.qkv, 3 * d, kc, vc, B, S, H, hd, Smax, pos0, st));
         const long long cb0 = (long long)Smax * hd, cb1 = (long long)H * Smax * hd;
-        MBS_TRY(mb200_attn_fwd_flash(P.qkv, 3 * d, qb0, qb1, kc, hd, cb0, cb1, vc, hd, cb0, cb1, P.attn_o, d, nullptr, 0,
-                                     nullptr, B, S, Sk, H, hd, 1, st));
+        MBS_TRY(mb200_attn_fwd_flash(P.qkv, 3 * d, qb0, qb1, kc, hd, cb0, cb1, vc, hd, cb0, cb1, P.attn_o, d, Pl,
+                                     Pl ? ld_attn : 0, nullptr, B, S, Sk, H, hd, 1, st));
       } else {
         MBS_TRY(mb200_attn_fwd_flash(P.qkv, 3 * d, qb0, qb1, P.qkv + d, 3 * d, qb0, qb1, P.qkv + 2 * d, 3 * d, qb0, qb1,
-                                     P.attn_o, d, nullptr, 0, nullptr, B, S, S, H, hd, 1, st));
+                                     P.attn_o, d, Pl, Pl ? ld_attn : 0, nullptr, B, S, S, H, hd, 1, st));
       }
     } else {
       Mat Q = mat(P.qkv, 3 * d, 0, hd, (long long)S * 3 * d), Kk, Vv;
@@ -572,7 +608,8 @@ int forward_infer(const mb200_gptj_model_ex* m, const bf16s* x, bf16s* logits, l
         Kk = mat(P.qkv + d, 3 * d, 0, hd, (long long)S * 3 * d);
         Vv = mat(P.qkv + 2 * d, 3 * d, 1, hd, (long long)S * 3 * d);
       }
-      MBS_TRY(attn_fwd_gemm(st, Q, Kk, Vv, S, Sk, H, B, hd, P.scores, P.P, P.ldS, P.attn_o, d, 1, Sk - S));
+      MBS_TRY(attn_fwd_gemm(st, Q, Kk, Vv, S, Sk, H, B, hd, P.scores, Pl ? Pl : P.P, P.ldS, P.attn_o, d, 1, Sk - S,
+                            Pl ? (int)ld_attn : 0));
     }
     if (m->attn_adapter == MB200_ADAPTER_NONE) {
       Epi e;
@@ -664,6 +701,18 @@ extern "C" int mb200_gptj_sched_infer_hidden(const mb200_gptj_model_ex* m, const
   return mb200::forward_infer(m, (const mb200::bf16s*)x, (mb200::bf16s*)logits, ldv, last_only, nullptr,
                               (mb200::bf16s*)kcache, (mb200::bf16s*)vcache, S_kv_max, pos0, B, S, ws, ws_bytes, stream,
                               nullptr, (mb200::bf16s*)hidden_all, ld_hidden);
+}
+
+extern "C" int mb200_gptj_sched_infer_attn(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv,
+                                           int32_t last_only, void* hidden_all, int64_t ld_hidden, void* const* attn,
+                                           int64_t ld_attn, void* kcache, void* vcache, int32_t S_kv_max, int32_t pos0,
+                                           int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  MBS_REQUIRE(attn != nullptr, MB200_E_ARG, "gptj_sched_infer_attn: attn is NULL");
+  return mb200::forward_infer(m, (const mb200::bf16s*)x, (mb200::bf16s*)logits, ldv, last_only, nullptr,
+                              (mb200::bf16s*)kcache, (mb200::bf16s*)vcache, S_kv_max, pos0, B, S, ws, ws_bytes, stream,
+                              nullptr, (mb200::bf16s*)hidden_all, ld_hidden, (mb200::bf16s* const*)attn, ld_attn);
 }
 
 extern "C" int mb200_gptj_sched_decode_step(const mb200_gptj_model_ex* m, const void* x, void* logits, int64_t ldv,
@@ -764,4 +813,46 @@ extern "C" int mb200_gptj_sched_backward_range_hidden_recompute(const mb200_gptj
   if (rc) return rc;
   return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
                          accumulate, B, S, ws, ws_bytes, stream, true);
+}
+
+extern "C" int mb200_gptj_sched_forward_attn(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels,
+                                             void* logits, int64_t ldv, float* loss, void* const* attn, int64_t ld_attn,
+                                             int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  MBS_REQUIRE(attn != nullptr, MB200_E_ARG, "gptj_sched_forward_attn: attn is NULL");
+  return mb200::forward(m, (const mb200::bf16s*)x, labels, (mb200::bf16s*)logits, ldv, loss, B, S, ws, ws_bytes, stream,
+                        false, (mb200::bf16s* const*)attn, ld_attn);
+}
+
+extern "C" int mb200_gptj_sched_forward_attn_recompute(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels,
+                                                       void* logits, int64_t ldv, float* loss, void* const* attn,
+                                                       int64_t ld_attn, int32_t B, int32_t S, void* ws, size_t ws_bytes,
+                                                       void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  MBS_REQUIRE(attn != nullptr, MB200_E_ARG, "gptj_sched_forward_attn: attn is NULL");
+  return mb200::forward(m, (const mb200::bf16s*)x, labels, (mb200::bf16s*)logits, ldv, loss, B, S, ws, ws_bytes, stream,
+                        true, (mb200::bf16s* const*)attn, ld_attn);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_attn(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                    void* const* dattn, int64_t ld_attn, float loss_scale,
+                                                    int32_t layer_hi, int32_t layer_lo, int32_t accumulate, int32_t B,
+                                                    int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
+                         accumulate, B, S, ws, ws_bytes, stream, false, (const mb200::bf16s* const*)dattn, ld_attn);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_attn_recompute(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                              void* const* dattn, int64_t ld_attn, float loss_scale,
+                                                              int32_t layer_hi, int32_t layer_lo, int32_t accumulate,
+                                                              int32_t B, int32_t S, void* ws, size_t ws_bytes,
+                                                              void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
+                         accumulate, B, S, ws, ws_bytes, stream, true, (const mb200::bf16s* const*)dattn, ld_attn);
 }

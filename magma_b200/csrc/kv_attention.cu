@@ -36,11 +36,14 @@ __global__ void kv_append_kernel(const bf16* __restrict__ qkv, long long ld, bf1
 // (`attn_weights.to(value.dtype)`, hf:gptj/modeling_gptj.py:146). HBM-bound: K and V are each read once, with
 // 512-byte coalesced rows.
 // ---------------------------------------------------------------------------------------------
+// The PROBS instantiation also writes the probabilities it multiplies V with, bf16(p_j), to row b*H + h of probs (row
+// stride ld_probs), zeros from column pos + 1 on: output_attentions of a decode step.
 static constexpr int kDecThreads = 256;
+template <bool PROBS>
 __global__ void __launch_bounds__(kDecThreads)
 attn_decode_kernel(const bf16* __restrict__ qkv, long long ld_qkv, bf16* __restrict__ kc, bf16* __restrict__ vc,
                    bf16* __restrict__ out, long long ld_out, int H, int hd, int Smax, int pos_host,
-                   const int* __restrict__ pos_dev) {
+                   const int* __restrict__ pos_dev, bf16* __restrict__ probs, long long ld_probs) {
   extern __shared__ float sc[];  // [pos+1] scores, then [32] reduction scratch
   // the cache position: a kernel argument, or — device-resident decode loop, one replayed CUDA graph per token — read
   // from device memory (shared memory is then sized for Smax by the launch)
@@ -99,6 +102,10 @@ attn_decode_kernel(const bf16* __restrict__ qkv, long long ld_qkv, bf16* __restr
   sum = 0.f;
   for (int w = 0; w < kDecThreads / 32; ++w) sum += red[w];
   const float inv = 1.f / sum;
+  if (PROBS) {
+    bf16* prow = probs + (long long)blockIdx.x * ld_probs;
+    for (int j = threadIdx.x; j < ld_probs; j += kDecThreads) prow[j] = __float2bfloat16(j < nk ? sc[j] * inv : 0.f);
+  }
   // out[c] = sum_j bf16(p_j) * v[j][c]
   for (int c = threadIdx.x; c < hd; c += kDecThreads) {
     float acc = 0.f;
@@ -118,7 +125,8 @@ static int decode_smem(long long n_keys, size_t* smem) {
   MB_REQUIRE(*smem <= 200 * 1024, MB200_E_SHAPE, "attn_decode: %lld keys need %zu bytes of shared memory", n_keys, *smem);
   static bool set = false;
   if (!set) {
-    MB_CUDA(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    MB_CUDA(cudaFuncSetAttribute(attn_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    MB_CUDA(cudaFuncSetAttribute(attn_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     set = true;
   }
   return 0;
@@ -137,9 +145,28 @@ extern "C" int mb200_attn_decode(const void* qkv, int64_t ld_qkv, void* kcache, 
              S_kv_max);
   size_t smem;
   if ((rc = decode_smem((long long)pos + 1, &smem))) return rc;
-  attn_decode_kernel<<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>((const bf16*)qkv, ld_qkv, (bf16*)kcache,
-                                                                         (bf16*)vcache, (bf16*)out, ld_out, H, hd,
-                                                                         S_kv_max, pos, nullptr);
+  attn_decode_kernel<false><<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>(
+      (const bf16*)qkv, ld_qkv, (bf16*)kcache, (bf16*)vcache, (bf16*)out, ld_out, H, hd, S_kv_max, pos, nullptr, nullptr, 0);
+  count_launch();
+  MB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// the same step, also writing its probabilities (output_attentions of a host-driven decode step)
+extern "C" int mb200_attn_decode_probs(const void* qkv, int64_t ld_qkv, void* kcache, void* vcache, void* out,
+                                       int64_t ld_out, void* probs, int64_t ld_probs, int32_t B, int32_t H, int32_t hd,
+                                       int32_t S_kv_max, int32_t pos, void* stream) {
+  int rc = check_arch();
+  if (rc) return rc;
+  MB_REQUIRE(hd % 8 == 0 && pos >= 0 && pos < S_kv_max, MB200_E_SHAPE, "attn_decode_probs: bad hd=%d pos=%d Smax=%d", hd,
+             pos, S_kv_max);
+  MB_REQUIRE(probs != nullptr && ld_probs > pos, MB200_E_ARG, "attn_decode_probs: ld_probs=%lld must be > pos=%d",
+             (long long)ld_probs, pos);
+  size_t smem;
+  if ((rc = decode_smem((long long)pos + 1, &smem))) return rc;
+  attn_decode_kernel<true><<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>(
+      (const bf16*)qkv, ld_qkv, (bf16*)kcache, (bf16*)vcache, (bf16*)out, ld_out, H, hd, S_kv_max, pos, nullptr,
+      (bf16*)probs, ld_probs);
   count_launch();
   MB_CUDA(cudaGetLastError());
   return 0;
@@ -155,9 +182,8 @@ extern "C" int mb200_attn_decode_dev(const void* qkv, int64_t ld_qkv, void* kcac
              S_kv_max);
   size_t smem;
   if ((rc = decode_smem(S_kv_max, &smem))) return rc;
-  attn_decode_kernel<<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>((const bf16*)qkv, ld_qkv, (bf16*)kcache,
-                                                                         (bf16*)vcache, (bf16*)out, ld_out, H, hd,
-                                                                         S_kv_max, 0, pos_dev);
+  attn_decode_kernel<false><<<B * H, kDecThreads, smem, (cudaStream_t)stream>>>(
+      (const bf16*)qkv, ld_qkv, (bf16*)kcache, (bf16*)vcache, (bf16*)out, ld_out, H, hd, S_kv_max, 0, pos_dev, nullptr, 0);
   count_launch();
   MB_CUDA(cudaGetLastError());
   return 0;

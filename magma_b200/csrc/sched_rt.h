@@ -165,24 +165,31 @@ inline bool flash_ok(int hd) {
 // Materialised attention forward over B x H heads: scores = Q K^T (fp32), P = softmax(scores / sqrt(hd) + mask),
 // O = P V. Q, K, V carry their per-head (bs0) and per-batch (bs1) strides; scores and P are [B,H,Sq,ldP]; O is
 // [B,Sq,H*hd] with row stride ldo. causal masks key j > i + koff for query i (koff = Sk - Sq over a KV cache).
+// ldPo (0: ldP) is P's own row stride, when P is a caller's buffer rather than the scores' twin.
 inline int attn_fwd_gemm(void* st, Mat Q, Mat K, Mat V, int Sq, int Sk, int H, int B, int hd, float* scores, bf16s* P,
-                         int ldP, bf16s* O, long long ldo, int causal, int koff) {
+                         int ldP, bf16s* O, long long ldo, int causal, int koff, int ldPo = 0) {
   const long long pb0 = (long long)Sq * ldP, pb1 = (long long)H * Sq * ldP;
+  if (ldPo == 0) ldPo = ldP;
+  const long long ob0 = (long long)Sq * ldPo, ob1 = (long long)H * Sq * ldPo;
   MBS_TRY(gemm(st, Sq, Sk, hd, Q, K, scores, ldP, 1, Epi(), H, B, pb0, pb1));
-  MBS_TRY(mb200_softmax_fwd(scores, ldP, pb0, P, ldP, pb0, B * H, Sq, Sk, 1.0f / sqrtf((float)hd), causal, koff, st));
-  return gemm(st, Sq, hd, Sk, mat(P, ldP, 0, pb0, pb1), V, O, ldo, 0, Epi(), H, B, hd, (long long)Sq * ldo);
+  MBS_TRY(mb200_softmax_fwd(scores, ldP, pb0, P, ldPo, ob0, B * H, Sq, Sk, 1.0f / sqrtf((float)hd), causal, koff, st));
+  return gemm(st, Sq, hd, Sk, mat(P, ldPo, 0, ob0, ob1), V, O, ldo, 0, Epi(), H, B, hd, (long long)Sq * ldo);
 }
 
 // Materialised attention backward on the fused qkv layout: qkv and dqkv are [B,S,3*H*hd] (q | k | v), dO is [B,S,H*hd],
 // P the saved [B,H,S,ldP] probabilities. dP (fp32) and dS are [B,H,S,ldP] scratch. eqk is the epilogue of dQ and dK
-// (e.g. the inverse rotary embedding of q and k).
+// (e.g. the inverse rotary embedding of q and k). dPe (optional, bf16 [B,H,S,ldP]): a gradient on P from outside the
+// block, added to dP in its GEMM's epilogue.
 inline int attn_bwd_gemm(void* st, const bf16s* qkv, const bf16s* P, const bf16s* dO, bf16s* dqkv, float* dP, bf16s* dS,
-                         int ldP, int S, int H, int B, int hd, const Epi& eqk) {
+                         int ldP, int S, int H, int B, int hd, const Epi& eqk, const bf16s* dPe = nullptr) {
   const int d = H * hd;
   const long long qb0 = hd, qb1 = (long long)S * 3 * d;
   const long long pb0 = (long long)S * ldP, pb1 = (long long)H * S * ldP;
-  // dP = dO V^T ; dV = P^T dO
-  MBS_TRY(gemm(st, S, S, hd, mat(dO, d, 0, hd, (long long)S * d), mat(qkv + 2 * d, 3 * d, 0, qb0, qb1), dP, ldP, 1, Epi(),
+  // dP = dO V^T (+ dPe) ; dV = P^T dO
+  Epi edp;
+  edp.res1 = dPe;
+  edp.ld_res = dPe ? ldP : 0;
+  MBS_TRY(gemm(st, S, S, hd, mat(dO, d, 0, hd, (long long)S * d), mat(qkv + 2 * d, 3 * d, 0, qb0, qb1), dP, ldP, 1, edp,
                H, B, pb0, pb1));
   MBS_TRY(gemm(st, S, hd, S, mat(P, ldP, 1, pb0, pb1), mat(dO, d, 1, hd, (long long)S * d), dqkv + 2 * d, 3 * d, 0, Epi(),
                H, B, qb0, qb1));

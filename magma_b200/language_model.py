@@ -4,8 +4,8 @@
 `.config.{max_position_embeddings,hidden_size,pad_token_id}`, `.resize_token_embeddings(n)`, `.transformer.wte`
 (callable on int64 ids), `.transformer.h[l].{mlp,attn}` (get/settable — the seam `Magma.add_adapters` rewires,
 magma/magma.py:128-169), `named_parameters()` with "adapter" in adapter names, and
-`__call__(inputs_embeds=|input_ids=, labels=, use_cache=, past_key_values=, output_hidden_states=)` returning an
-object with `.loss`, `.logits`, `.past_key_values`, `.hidden_states`.
+`__call__(inputs_embeds=|input_ids=, labels=, use_cache=, past_key_values=, output_hidden_states=, output_attentions=)`
+returning an object with `.loss`, `.logits`, `.past_key_values`, `.hidden_states` (and `.attentions` when asked for).
 
 All frozen weights are bf16 tensors on the GPU; parameter names follow HF GPT-J (`attn.q_proj.weight`, `mlp.fc_in.*`,
 `ln_1`, `ln_f`, `lm_head`) — the executable stand-in for the reference's fork. The whole
@@ -216,28 +216,31 @@ def _backward_scale(model, dloss):
 class _LMTrainFn(torch.autograd.Function):
     """loss = LM(inputs_embeds, labels) with the backward pass of the C++ runtime (LM frozen: dgrad through every
     GEMM, wgrad only for adapters, written straight into the parameter arena's fp32 gradient buffer). With
-    want_hidden the n_layer + 1 hidden states follow (loss, logits) as outputs, and their gradients flow back through
-    the same backward pass."""
+    want_hidden the n_layer + 1 hidden states follow (loss, logits) as outputs, then with want_attn the n_layer
+    attention probabilities ([B, H, S, S rounded up to 8]); the gradients of both flow back through the same backward
+    pass."""
 
     @staticmethod
-    def forward(ctx, model, x, labels, anchor, want_hidden=False):
-        loss, logits, hidden = model._run_forward(x, labels, training=True, want_hidden=want_hidden)
+    def forward(ctx, model, x, labels, anchor, want_hidden=False, want_attn=False):
+        loss, logits, hidden, attn = model._run_forward(x, labels, training=True, want_hidden=want_hidden,
+                                                        want_attn=want_attn)
         ctx.model = model
         ctx.generation = model._generation
         ctx.shape = x.shape
         ctx.x_dtype = x.dtype
+        ctx.n_hidden = len(hidden or ())
         ctx.mark_non_differentiable(logits)
-        if want_hidden:
-            ctx.set_materialize_grads(False)  # an unused hidden state has no gradient to add
-        return (loss, logits, *(hidden or ()))
+        if want_hidden or want_attn:
+            ctx.set_materialize_grads(False)  # an unused hidden state or attention map has no gradient to add
+        return (loss, logits, *(hidden or ()), *(attn or ()))
 
     @staticmethod
-    def backward(ctx, dloss, _dlogits, *dhidden):
+    def backward(ctx, dloss, _dlogits, *douts):
         model = ctx.model
         if ctx.generation != model._generation:
             raise MB200Error("backward called after another training forward overwrote the saved activations")
-        dx = model._run_backward(ctx.shape, _backward_scale(model, dloss), dhidden)
-        return None, dx.to(ctx.x_dtype), None, None, None
+        dx = model._run_backward(ctx.shape, _backward_scale(model, dloss), douts[: ctx.n_hidden], douts[ctx.n_hidden :])
+        return None, dx.to(ctx.x_dtype), None, None, None, None
 
 
 class B200GPTJForCausalLM(nn.Module):
@@ -396,21 +399,25 @@ class B200GPTJForCausalLM(nn.Module):
         return (self.lm_head.weight.shape[0] + 63) // 64 * 64
 
     # ---- passes --------------------------------------------------------------------------------
-    def _run_forward(self, x, labels, training, cache=None, last_only=False, want_hidden=False, want_logits=True):
-        """(loss, logits, hidden states): the hidden states are output_hidden_states' tuple of n_layer + 1 [B, S, d]
-        tensors when want_hidden, else None."""
+    def _run_forward(self, x, labels, training, cache=None, last_only=False, want_hidden=False, want_logits=True,
+                     want_attn=False):
+        """(loss, logits, hidden states, attentions): the hidden states are output_hidden_states' tuple of n_layer + 1
+        [B, S, d] tensors when want_hidden, else None; the attentions n_layer [B, H, S, ld] bf16 probability buffers
+        when want_attn, else None (ld = S_kv rounded up to 8; columns from S_kv on are not part of the result)."""
         B, S, d = x.shape
         x = x.to(torch.bfloat16).contiguous()
         if self._arena is not None or self.adapter_parameters():
             self._ensure_arena().sync_shadow()
-        return self._run_pass(x, labels, training, cache, last_only, want_hidden, want_logits)
+        return self._run_pass(x, labels, training, cache, last_only, want_hidden, want_logits, want_attn)
 
-    def _run_pass(self, x, labels, training, cache, last_only, want_hidden, want_logits):
+    def _run_pass(self, x, labels, training, cache, last_only, want_hidden, want_logits, want_attn=False):
         """csrc/gptj_sched.cu: the training pass (activations saved for backward) when a loss is asked for, else the
-        inference pass — full sequence, KV-cache prefill / decode step, last-position logits, every hidden state."""
+        inference pass — full sequence, KV-cache prefill / decode step, last-position logits, every hidden state,
+        every block's attention probabilities."""
         B, S, d = x.shape
         m = self._cmodel_ex()[0]
         V, ldv = self.lm_head.weight.shape[0], self.ldv
+        n, H = len(self.transformer.h), self.config.num_heads
         if labels is not None or training:
             if cache is not None or last_only:
                 raise MB200Error("a loss together with a KV cache / last-position logits is not supported")
@@ -421,9 +428,18 @@ class B200GPTJForCausalLM(nn.Module):
                 labels = labels.to(device=x.device, dtype=torch.int64).contiguous()
             self._generation += 1  # this pass records its activations in the workspace
             self._generation_recompute = recompute
-            fwd = lib().mb200_gptj_sched_forward_recompute if recompute else lib().mb200_gptj_sched_forward
-            check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ldv, ops._ptr(loss), B, S,
-                      ops._ptr(ws), ws.numel(), ops._stream()))
+            attn = None
+            if want_attn:  # written by the forward as each block runs, in the layout of the saved probabilities
+                ld_attn = (S + 7) // 8 * 8
+                attn = tuple(torch.empty(B, H, S, ld_attn, dtype=torch.bfloat16, device=x.device) for _ in range(n))
+                fwd = (lib().mb200_gptj_sched_forward_attn_recompute if recompute
+                       else lib().mb200_gptj_sched_forward_attn)
+                check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ldv, ops._ptr(loss),
+                          _ptr_array(attn), ld_attn, B, S, ops._ptr(ws), ws.numel(), ops._stream()))
+            else:
+                fwd = lib().mb200_gptj_sched_forward_recompute if recompute else lib().mb200_gptj_sched_forward
+                check(fwd(ctypes.byref(m), ops._ptr(x), ops._ptr(labels), ops._ptr(logits), ldv, ops._ptr(loss), B, S,
+                          ops._ptr(ws), ws.numel(), ops._stream()))
             hidden = None
             if want_hidden:  # copied out of the workspace, which the next forward overwrites
                 hidden = tuple(torch.empty(B, S, d, dtype=torch.bfloat16, device=x.device)
@@ -432,7 +448,7 @@ class B200GPTJForCausalLM(nn.Module):
                         else lib().mb200_gptj_sched_hidden_states)
                 check(copy(ctypes.byref(m), _ptr_array(hidden), B, S, ops._ptr(ws), ws.numel(), ops._stream()))
             lg = logits.view(B, S, ldv)[..., :V] if logits is not None else None
-            return (loss.squeeze(0) if loss is not None else None), lg, hidden
+            return (loss.squeeze(0) if loss is not None else None), lg, hidden, attn
         S_kv = cache.S_max if cache is not None else S
         # ONE grow-only inference workspace: a serving process sees many (B, prompt length, cache length) combinations,
         # and the C side only needs `nbytes` of scratch for the pass at hand (nothing survives between calls)
@@ -446,25 +462,37 @@ class B200GPTJForCausalLM(nn.Module):
         rows = B if last_only else B * S
         logits = torch.empty(rows, ldv, dtype=torch.bfloat16, device=x.device) if want_logits else None
         kv = (ops._ptr(cache.k), ops._ptr(cache.v), S_kv, cache.pos) if cache is not None else (None, None, 0, 0)
-        hidden = None
+        hidden = attn = None
         if want_hidden:  # one buffer, entry l at l * B*S*d: each block writes its output into its entry
             hidden = torch.empty(len(self.transformer.h) + 1, B, S, d, dtype=torch.bfloat16, device=x.device)
+        if want_attn:  # one buffer, entry l the [B, H, S, ld_attn] probabilities block l multiplies V with
+            S_kv = S + (cache.pos if cache is not None else 0)
+            ld_attn = (S_kv + 7) // 8 * 8
+            attn = torch.empty(n, B, H, S, ld_attn, dtype=torch.bfloat16, device=x.device)
+            check(lib().mb200_gptj_sched_infer_attn(
+                ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, ops._ptr(hidden),
+                hidden.stride(0) if hidden is not None else 0, _ptr_array(attn.unbind(0)), ld_attn, *kv, B, S,
+                ops._ptr(ws), ws.numel(), ops._stream()))
+            attn = attn.unbind(0)
+        elif want_hidden:
             check(lib().mb200_gptj_sched_infer_hidden(
                 ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, ops._ptr(hidden), hidden.stride(0), *kv,
                 B, S, ops._ptr(ws), ws.numel(), ops._stream()))
-            hidden = hidden.unbind(0)
         else:
             check(lib().mb200_gptj_sched_infer(
                 ctypes.byref(m), ops._ptr(x), ops._ptr(logits), ldv, last_only, None, *kv, B, S, ops._ptr(ws),
                 ws.numel(), ops._stream()))
         if cache is not None:
             cache.pos += S
+        if hidden is not None:
+            hidden = hidden.unbind(0)
         lg = logits.view(B, 1 if last_only else S, ldv)[..., :V] if logits is not None else None
-        return None, lg, hidden
+        return None, lg, hidden, attn
 
-    def _run_backward(self, shape, loss_scale, dhidden=()):
-        """dhidden: the gradients of the hidden states the forward returned (each None or [B, S, d]); all None or
-        empty runs the backward of the loss alone."""
+    def _run_backward(self, shape, loss_scale, dhidden=(), dattn=()):
+        """dhidden: the gradients of the hidden states the forward returned (each None or [B, S, d]); dattn: those of
+        its attention buffers (each None or [B, H, S, S rounded up to 8]); all None or empty runs the backward of the
+        loss alone."""
         B, S, d = shape
         arena = self._arena
         dx = torch.empty(B, S, d, dtype=torch.bfloat16, device=self._device)
@@ -472,8 +500,17 @@ class B200GPTJForCausalLM(nn.Module):
         if recompute != self._generation_recompute:
             raise MB200Error("backward called on a workspace of the other activation path (stored / recomputed) than "
                              "its forward's")
-        if any(g is not None for g in dhidden):
-            dh = [None if g is None else g.to(device=self._device, dtype=torch.bfloat16).contiguous() for g in dhidden]
+
+        def prep(gs):
+            return [None if g is None else g.to(device=self._device, dtype=torch.bfloat16).contiguous() for g in gs]
+
+        if any(g is not None for g in dattn):  # hidden-state and attention gradients in one pass
+            dh, da = prep(dhidden), prep(dattn)
+            extra = (_ptr_array(dh) if any(g is not None for g in dh) else None, _ptr_array(da), (S + 7) // 8 * 8)
+            bwd = (lib().mb200_gptj_sched_backward_range_attn_recompute if recompute
+                   else lib().mb200_gptj_sched_backward_range_attn)
+        elif any(g is not None for g in dhidden):
+            dh = prep(dhidden)
             extra = (_ptr_array(dh),)
             bwd = (lib().mb200_gptj_sched_backward_range_hidden_recompute if recompute
                    else lib().mb200_gptj_sched_backward_range_hidden)
@@ -491,7 +528,15 @@ class B200GPTJForCausalLM(nn.Module):
         return dx
 
     def forward(self, input_ids=None, inputs_embeds=None, labels=None, use_cache=False, past_key_values=None,
-                output_hidden_states=False, max_cache_len=None, **_unused):
+                output_hidden_states=False, output_attentions=False, max_cache_len=None, **_unused):
+        """GPTJForCausalLM.forward. output_attentions=True adds `.attentions`: one bf16 [B, H, S, S_kv] tensor per
+        block (S_kv = S, or pos0 + S over a KV cache), the probabilities the block multiplied V with, as
+        `attn_weights.to(value.dtype)` of hf:gptj/modeling_gptj.py:145-146 returns them; entries above the causal
+        diagonal are 0. They are views of buffers whose rows are S_kv rounded up to 8 long. In training they are outputs
+        of the autograd function, and the gradient of a loss that reads them joins the one backward pass. Not covered:
+        the gradient of the loss with respect to the attentions themselves (HF's retain_grad on an intermediate), and an
+        output_attentions argument of Magma.forward, which the reference does not have. generate() never asks for
+        them."""
         if (input_ids is None) == (inputs_embeds is None):
             raise ValueError("pass exactly one of input_ids / inputs_embeds")
         if inputs_embeds is None:
@@ -501,21 +546,28 @@ class B200GPTJForCausalLM(nn.Module):
         has_trainable = any(p.requires_grad for _, p in self.adapter_parameters()) or inputs_embeds.requires_grad
         if labels is not None and torch.is_grad_enabled() and has_trainable and not use_cache:
             anchor = next((p for _, p in self.adapter_parameters() if p.requires_grad), None)
-            res = _LMTrainFn.apply(self, inputs_embeds, labels, anchor, output_hidden_states)
+            res = _LMTrainFn.apply(self, inputs_embeds, labels, anchor, output_hidden_states, output_attentions)
             out.loss, out.logits = res[0], res[1]
+            nh = len(self.transformer.h) + 1 if output_hidden_states else 0
             if output_hidden_states:
-                out.hidden_states = tuple(res[2:])
+                out.hidden_states = tuple(res[2 : 2 + nh])
+            if output_attentions:
+                out.attentions = tuple(a[..., :S] for a in res[2 + nh :])
             return out
         cache = past_key_values
         if use_cache and cache is None:
             S_max = max_cache_len or self.config.max_position_embeddings
             cfg = self.config
             cache = KVCache(cfg.num_layers, B, cfg.num_heads, S_max, cfg.hidden_size // cfg.num_heads, self._device)
+        S_kv = S + (cache.pos if use_cache else 0)
         with torch.no_grad():
-            loss, logits, hidden = self._run_forward(inputs_embeds, labels, training=False,
-                                                     cache=cache if use_cache else None, last_only=False,
-                                                     want_hidden=output_hidden_states)
+            loss, logits, hidden, attn = self._run_forward(inputs_embeds, labels, training=False,
+                                                           cache=cache if use_cache else None, last_only=False,
+                                                           want_hidden=output_hidden_states,
+                                                           want_attn=output_attentions)
         out.loss, out.logits, out.hidden_states = loss, logits, hidden
+        if output_attentions:
+            out.attentions = tuple(a[..., :S_kv] for a in attn)
         out.past_key_values = cache if use_cache else None
         return out
 
@@ -543,7 +595,7 @@ class B200GPTJForCausalLM(nn.Module):
     @torch.no_grad()
     def decode_logits(self, inputs_embeds, cache):
         """Last-position logits only (what magma/sampling.py:92 consumes): the LM head runs on B rows, not B*S."""
-        _, lg, _ = self._run_forward(inputs_embeds, None, training=False, cache=cache, last_only=True)
+        _, lg, _, _ = self._run_forward(inputs_embeds, None, training=False, cache=cache, last_only=True)
         return lg[:, 0, :]
 
 

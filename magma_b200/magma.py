@@ -36,7 +36,7 @@ class _EmbedLMFn(torch.autograd.Function):
     def forward(ctx, magma, prefix, captions, labels, anchor, want_hidden=False):
         lm = magma.lm
         x = ops.embed_assemble(captions, lm.transformer.wte.weight, prefix.to(torch.bfloat16).contiguous())
-        loss, logits, hidden = lm._run_forward(x, labels, training=True, want_hidden=want_hidden)
+        loss, logits, hidden, _ = lm._run_forward(x, labels, training=True, want_hidden=want_hidden)
         ctx.magma, ctx.generation = magma, lm._generation
         ctx.shape, ctx.L, ctx.pdtype = x.shape, prefix.shape[1], prefix.dtype
         ctx.mark_non_differentiable(logits)
