@@ -244,6 +244,12 @@ int mb200_sample(const void* logits, int32_t dtype, int64_t ld, int32_t rows, in
                  int32_t top_k, float top_p, uint64_t seed, uint64_t offset, int64_t* tokens, uint8_t* keep_mask,
                  void* stream);
 int mb200_add(const void* a, const void* b, const void* c, void* y, int64_t n, void* stream);
+/* The gradient the LM head's backward reads when a loss reads the logits: out[r, j] = alpha * dce[r, j] + g[r, j] for
+ * r < M, j < V, in fp32 with one rounding to bf16. dce and out are bf16 [M, ldv] (ldv % 8 == 0, 16-byte aligned); g is
+ * bf16 with unit column stride and row stride ld_g >= V, 2-byte aligned (rows read with the widest load their
+ * alignment allows). Columns from V on are not written. alpha == 0 never reads dce (it may be NULL). */
+int mb200_logits_grad_combine(const void* dce, int64_t ldv, const void* g, int64_t ld_g, void* out, int32_t M, int32_t V,
+                              float alpha, void* stream);
 /* Data-parallel gradient exchange over peer memory (stands where DeepSpeed's gradient all-reduce stood, train.py:103-111).
  * bufs[r], r < world: rank r's fp32 exchange buffer as mapped into THIS process (peer memory for r != own rank; 16-byte
  * aligned, same layout on every rank). Elements [offset, offset + n) — the calling rank's shard — are read from all
@@ -472,6 +478,24 @@ int mb200_gptj_sched_backward_range_attn_recompute(const mb200_gptj_model_ex* m,
                                                    void* const* dattn, int64_t ld_attn, float loss_scale,
                                                    int32_t layer_hi, int32_t layer_lo, int32_t accumulate, int32_t B,
                                                    int32_t S, void* ws, size_t ws_bytes, void* stream);
+/* The backward of a loss that reads the logits, and / or hidden states and attention probabilities, in one pass:
+ * dhidden, dattn and ld_attn as in mb200_gptj_sched_backward_range_attn. dlogits (NULL, or bf16 [B*S, V] with unit
+ * column stride and row stride ld_dlogits >= V, any 2-byte alignment) is the gradient of the logits the forward
+ * returned. The call whose range holds the LM head (layer_hi == n_layer) writes loss_scale * (the cross-entropy
+ * gradient the forward wrote) + dlogits into dlogits_comb (bf16 [B*S, ldv], ldv = vocab rounded up to 64, 16-byte
+ * aligned; mb200_logits_grad_combine) and runs the LM head's dgrad on it, so the workspace is not written and a second
+ * backward over the same forward gives the same result. Without dlogits and with loss_scale == 0 the LM head adds
+ * nothing and the cross-entropy gradient is not read: the backward of a forward without labels. Otherwise, without
+ * dlogits, the result equals mb200_gptj_sched_backward_range_attn(_recompute). */
+int mb200_gptj_sched_backward_range_logits(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden, void* const* dattn,
+                                           int64_t ld_attn, const void* dlogits, int64_t ld_dlogits, void* dlogits_comb,
+                                           float loss_scale, int32_t layer_hi, int32_t layer_lo, int32_t accumulate,
+                                           int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream);
+int mb200_gptj_sched_backward_range_logits_recompute(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                     void* const* dattn, int64_t ld_attn, const void* dlogits,
+                                                     int64_t ld_dlogits, void* dlogits_comb, float loss_scale,
+                                                     int32_t layer_hi, int32_t layer_lo, int32_t accumulate, int32_t B,
+                                                     int32_t S, void* ws, size_t ws_bytes, void* stream);
 /* Inference pass (no saved activations) — use_cache=True of magma/sampling.py:81-90: kcache / vcache bf16
  * [n_layer][B][H][S_kv_max][hd] or NULL; the K / V of this call are written at positions [pos0, pos0 + S) and attention
  * runs over [0, pos0 + S) (prefill S > 1 through mb200_attn_fwd_flash, decode S == 1 through mb200_attn_decode).

@@ -225,6 +225,7 @@ SIGNATURES = {
     "mb200_argmax": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp]),
     "mb200_sample": (_i32, [_vp, _i32, _i64, _i32, _i32, _f32, _i32, _f32, _u64, _u64, _vp, _vp, _vp]),
     "mb200_add": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp]),
+    "mb200_logits_grad_combine": (_i32, [_vp, _i64, _vp, _i64, _vp, _i32, _i32, _f32, _vp]),
     "mb200_peer_reduce_bcast": (_i32, [ctypes.POINTER(_vp), _i32, _i64, _i64, _i32, _vp]),
     "mb200_sumsq": (_i32, [_vp, _i64, _vp, _vp]),
     "mb200_adamw_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _f32, _vp, _f32, _i32,
@@ -258,6 +259,10 @@ SIGNATURES = {
                                                     _sz, _vp]),
     "mb200_gptj_sched_backward_range_attn_recompute": (_i32, [_GPTJ, _vp, _VPP, _VPP, _i64, _f32, _i32, _i32, _i32, _i32,
                                                               _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_backward_range_logits": (_i32, [_GPTJ, _vp, _VPP, _VPP, _i64, _vp, _i64, _vp, _f32, _i32, _i32,
+                                                      _i32, _i32, _i32, _vp, _sz, _vp]),
+    "mb200_gptj_sched_backward_range_logits_recompute": (_i32, [_GPTJ, _vp, _VPP, _VPP, _i64, _vp, _i64, _vp, _f32, _i32,
+                                                                _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
     "mb200_gptj_sched_infer_workspace_bytes": (_sz, [_GPTJ, _i32, _i32, _i32]),
     "mb200_gptj_sched_infer": (_i32, [_GPTJ, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz,
                                       _vp]),

@@ -419,6 +419,22 @@ extern "C" int mb200_add(const void* a, const void* b, const void* c, void* y, i
   return 0;
 }
 
+extern "C" int mb200_logits_grad_combine(const void* dce, int64_t ldv, const void* g, int64_t ld_g, void* out, int32_t M,
+                                         int32_t V, float alpha, void* stream) {
+  MB_ENTER();
+  MB_REQUIRE(M > 0 && V > 0 && V <= ldv && V <= ld_g, MB200_E_SHAPE,
+             "logits_grad_combine: need M=%d > 0 and 0 < V=%d <= ldv=%lld, ld_g=%lld", M, V, (long long)ldv,
+             (long long)ld_g);
+  MB_REQUIRE(g && out && (dce || alpha == 0.f), MB200_E_ARG, "logits_grad_combine: g, out (and dce unless alpha == 0) are NULL");
+  MB_REQUIRE(ldv % 8 == 0 && aligned_to(16, dce, out) && aligned_to(2, g), MB200_E_ALIGN,
+             "logits_grad_combine: ldv must be a multiple of 8, dce and out 16-byte aligned, g 2-byte aligned");
+  const int col_blocks = (V / 8 + kLgThreads * kLgChunks - 1) / (kLgThreads * kLgChunks);
+  launch(logits_grad_combine_kernel, dim3((unsigned)M, col_blocks > 0 ? col_blocks : 1), kLgThreads, 0, ST(stream), (const bf16*)dce, (long long)ldv, (const bf16*)g,
+         (long long)ld_g, (bf16*)out, (int)V, alpha);
+  MB_LAUNCH_CHECK();
+  return 0;
+}
+
 extern "C" int mb200_sumsq(const float* x, int64_t n, float* out, void* stream) {
   MB_ENTER();
   int grid = grid_for(n, 256);

@@ -601,6 +601,64 @@ __global__ void add_kernel(const bf16* __restrict__ a, const bf16* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------------
+// The gradient that enters the LM head's dgrad when a loss reads the logits: out[r, j] = alpha * dce[r, j] + g[r, j]
+// for j < V, one fp32 fma and one rounding. dce (the cross-entropy gradient) and out are [M, ldv] with 16-byte aligned
+// rows. g is autograd's gradient on the logits: unit column stride, any row stride, so a row may start on any 2-byte
+// boundary (ld_g = 50258 gives rows 4-byte aligned only); each row reads g with the widest load its alignment allows.
+// alpha == 0 never reads dce, which then may hold anything (no cross-entropy gradient was written).
+// grid = (M rows, column blocks of kLgChunks * kLgThreads 8-column chunks); the last column block also does the V % 8
+// tail of its row.
+// ---------------------------------------------------------------------------------------------
+static constexpr int kLgThreads = 256;
+static constexpr int kLgChunks = 4;
+
+__device__ __forceinline__ void load8_aligned_to(const bf16* p, int align, float (&f)[8]) {
+  if (align == 16) {
+    unpack8(*reinterpret_cast<const uint4*>(p), f);
+  } else if (align == 4) {
+    const uint32_t* q = reinterpret_cast<const uint32_t*>(p);
+    const uint4 u = make_uint4(q[0], q[1], q[2], q[3]);
+    unpack8(u, f);
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) f[e] = __bfloat162float(p[e]);
+  }
+}
+
+__global__ void __launch_bounds__(kLgThreads)
+logits_grad_combine_kernel(const bf16* __restrict__ dce, long long ldv, const bf16* __restrict__ g, long long ld_g,
+                           bf16* __restrict__ out, int V, float alpha) {
+  const long long r = blockIdx.x;
+  const bf16* gr = g + r * ld_g;
+  const bf16* dr = dce + r * ldv;
+  bf16* orow = out + r * ldv;
+  const uintptr_t a = reinterpret_cast<uintptr_t>(gr);
+  const int align = (a & 15) == 0 ? 16 : (a & 3) == 0 ? 4 : 2;  // the same for every chunk of the row
+  const int nvec = V >> 3;
+  const int c0 = (int)blockIdx.y * kLgThreads * kLgChunks + (int)threadIdx.x;
+#pragma unroll
+  for (int k = 0; k < kLgChunks; ++k) {
+    const int c = c0 + k * kLgThreads;
+    if (c < nvec) {
+      float f[8];
+      load8_aligned_to(gr + 8 * (long long)c, align, f);
+      if (alpha != 0.f) {
+        float d[8];
+        unpack8(reinterpret_cast<const uint4*>(dr)[c], d);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] = fmaf(alpha, d[e], f[e]);
+      }
+      reinterpret_cast<uint4*>(orow)[c] = pack8(f);
+    }
+  }
+  if (blockIdx.y == gridDim.y - 1)
+    for (int j = nvec * 8 + (int)threadIdx.x; j < V; j += kLgThreads) {
+      const float gj = __bfloat162float(gr[j]);
+      orow[j] = __float2bfloat16(alpha != 0.f ? fmaf(alpha, __bfloat162float(dr[j]), gj) : gj);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Gradient exchange over NVLink peer memory (data parallelism; replaces the NCCL all-reduce of DeepSpeed's engine,
 // train.py:103-111). Every rank owns one shard of the slice: it reads that shard from ALL ranks' exchange buffers
 // (peer-mapped pointers: plain loads over NVLink / NVSwitch), adds them in rank order, and stores the sum back into ALL

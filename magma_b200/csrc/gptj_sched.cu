@@ -33,6 +33,8 @@
 // MB200_E_ARG; the CUDA library always defines both.
 #pragma weak mb200_attn_bwd_tile_dp
 #pragma weak mb200_attn_decode_probs
+// likewise the kernel that joins a loss's gradient on the logits to the cross-entropy gradient
+#pragma weak mb200_logits_grad_combine
 
 namespace mb200 {
 namespace {
@@ -384,9 +386,15 @@ int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels,
 // dattn (NULL, or n_layer pointers, each NULL or bf16 [B,H,S,ld_attn] with ld_attn = ldP): gradients of the attention
 // probabilities forward() returned. Layer l's joins dP = dO V^T before rowsum(dP * P) — in the tile kernel's fragment
 // (mb200_attn_bwd_tile_dp), or as the dP GEMM's residual on the materialised path.
+// logits_grad (the backward_range_logits entries): dlg (NULL, or bf16 [M, V] rows of stride ld_dlg) is the gradient of
+// a loss on the logits the forward returned. It joins loss_scale * P.dlogits in the caller's dcomb ([M, ldv]), which
+// the LM head's dgrad then reads with alpha 1, so P.dlogits is never written and a second backward gives the same
+// result. Without dlg and with loss_scale == 0 (a forward without labels, whose P.dlogits was never written) the LM
+// head adds nothing and P.dlogits is not read.
 int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, float loss_scale, int layer_hi,
              int layer_lo, int acc, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute,
-             const bf16s* const* dattn = nullptr, long long ld_attn = 0) {
+             const bf16s* const* dattn = nullptr, long long ld_attn = 0, bool logits_grad = false,
+             const bf16s* dlg = nullptr, long long ld_dlg = 0, bf16s* dcomb = nullptr) {
   Plan P;
   MBS_TRY(make_plan(P, m, B, S, ws, recompute));
   MBS_REQUIRE(ws != nullptr && ws_bytes >= P.bytes, MB200_E_ARG, "gptj_sched_backward: workspace too small");
@@ -394,19 +402,37 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, 
               "gptj_sched_backward_range_attn: ld_attn=%lld must be %d (S rounded up to 8)", ld_attn, P.ldP);
   MBS_REQUIRE(0 <= layer_lo && layer_lo <= layer_hi && layer_hi <= m->n_layer, MB200_E_ARG,
               "gptj_sched_backward: bad layer range [%d,%d)", layer_lo, layer_hi);
+  MBS_REQUIRE(!dlg || (dcomb && ld_dlg >= m->vocab), MB200_E_ARG,
+              "gptj_sched_backward_range_logits: dlogits needs ld_dlogits=%lld >= vocab=%d and a dlogits_comb buffer",
+              ld_dlg, m->vocab);
   const int M = P.M, d = P.d, dff = P.dff, H = P.H, hd = P.hd;
   ScratchScope scratch(P.gemm_ws, P.gemm_ws_bytes);
   // gradient w.r.t. the residual stream entering layer l lives in g[(l) & 1]
   bf16s* gb[2] = {P.g0, P.g1};
   if (layer_hi == m->n_layer) {  // dxf = loss_scale * dlogits Wlm ; g = LN_f backward
-    Epi e;
-    e.alpha = loss_scale;
-    if (dhid && dhid[m->n_layer]) {
-      e.res1 = dhid[m->n_layer];
-      e.ld_res = d;
+    const bf16s* dhf = dhid ? dhid[m->n_layer] : nullptr;
+    const bf16s* dxf = P.dh;
+    if (logits_grad && !dlg && loss_scale == 0.f) {  // nothing reaches the LM head
+      if (dhf) dxf = dhf;
+      else MBS_TRY(rt_zero(P.dh, (size_t)M * d * sizeof(bf16s), st));
+    } else {
+      Epi e;
+      e.alpha = loss_scale;
+      if (dhf) {
+        e.res1 = dhf;
+        e.ld_res = d;
+      }
+      const bf16s* dl = P.dlogits;
+      if (dlg) {  // dcomb = loss_scale * dlogits + dlg, read with alpha 1
+        MBS_REQUIRE(mb200_logits_grad_combine, MB200_E_ARG, "gptj_sched: mb200_logits_grad_combine is not in this build");
+        MBS_TRY(mb200_logits_grad_combine(loss_scale != 0.f ? P.dlogits : nullptr, P.ldv, dlg, ld_dlg, dcomb, M, m->vocab,
+                                          loss_scale, st));
+        dl = dcomb;
+        e.alpha = 1.f;
+      }
+      MBS_TRY(gemm(st, M, d, m->vocab, mat(dl, P.ldv), wmat(m->w_lm, d, 1), P.dh, d, 0, e));
     }
-    MBS_TRY(gemm(st, M, d, m->vocab, mat(P.dlogits, P.ldv), wmat(m->w_lm, d, 1), P.dh, d, 0, e));
-    MBS_TRY(mb200_layernorm_bwd(P.dh, d, P.x_final, d, m->lnf_g, P.lnf_mean, P.lnf_rstd, nullptr, 0, gb[m->n_layer & 1], d,
+    MBS_TRY(mb200_layernorm_bwd(dxf, d, P.x_final, d, m->lnf_g, P.lnf_mean, P.lnf_rstd, nullptr, 0, gb[m->n_layer & 1], d,
                                 M, d, st));
   }
   for (int l = layer_hi - 1; l >= layer_lo; --l) {
@@ -855,4 +881,29 @@ extern "C" int mb200_gptj_sched_backward_range_attn_recompute(const mb200_gptj_m
   if (rc) return rc;
   return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
                          accumulate, B, S, ws, ws_bytes, stream, true, (const mb200::bf16s* const*)dattn, ld_attn);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_logits(const mb200_gptj_model_ex* m, void* dx, void* const* dhidden,
+                                                      void* const* dattn, int64_t ld_attn, const void* dlogits,
+                                                      int64_t ld_dlogits, void* dlogits_comb, float loss_scale,
+                                                      int32_t layer_hi, int32_t layer_lo, int32_t accumulate, int32_t B,
+                                                      int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
+                         accumulate, B, S, ws, ws_bytes, stream, false, (const mb200::bf16s* const*)dattn, ld_attn, true,
+                         (const mb200::bf16s*)dlogits, ld_dlogits, (mb200::bf16s*)dlogits_comb);
+}
+
+extern "C" int mb200_gptj_sched_backward_range_logits_recompute(const mb200_gptj_model_ex* m, void* dx,
+                                                                void* const* dhidden, void* const* dattn, int64_t ld_attn,
+                                                                const void* dlogits, int64_t ld_dlogits,
+                                                                void* dlogits_comb, float loss_scale, int32_t layer_hi,
+                                                                int32_t layer_lo, int32_t accumulate, int32_t B,
+                                                                int32_t S, void* ws, size_t ws_bytes, void* stream) {
+  int rc = mb200::rt_check_arch();
+  if (rc) return rc;
+  return mb200::backward(m, (mb200::bf16s*)dx, (const mb200::bf16s* const*)dhidden, loss_scale, layer_hi, layer_lo,
+                         accumulate, B, S, ws, ws_bytes, stream, true, (const mb200::bf16s* const*)dattn, ld_attn, true,
+                         (const mb200::bf16s*)dlogits, ld_dlogits, (mb200::bf16s*)dlogits_comb);
 }

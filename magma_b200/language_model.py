@@ -206,19 +206,23 @@ def _free_bytes(device):
 
 
 def _backward_scale(model, dloss):
-    """The loss gradient the LM head's backward scales by: B200Engine.backward's hint, else dloss (a host sync), or 0
-    when only hidden states feed the loss."""
+    """The loss gradient the LM head's backward scales the cross-entropy gradient by: 0 when the loss does not read
+    `.loss` (also under B200Engine.backward: its hint must not add a CE term the loss does not have), else
+    B200Engine.backward's hint, else dloss (a host sync). Gradients a loss sends through the logits, hidden states or
+    attentions are not scaled by it."""
+    if dloss is None:
+        return 0.0
     if model._loss_scale_hint is not None:
         return model._loss_scale_hint
-    return 0.0 if dloss is None else float(dloss)
+    return float(dloss)
 
 
 class _LMTrainFn(torch.autograd.Function):
-    """loss = LM(inputs_embeds, labels) with the backward pass of the C++ runtime (LM frozen: dgrad through every
-    GEMM, wgrad only for adapters, written straight into the parameter arena's fp32 gradient buffer). With
-    want_hidden the n_layer + 1 hidden states follow (loss, logits) as outputs, then with want_attn the n_layer
-    attention probabilities ([B, H, S, S rounded up to 8]); the gradients of both flow back through the same backward
-    pass."""
+    """(loss, logits) = LM(inputs_embeds, labels) with the backward pass of the C++ runtime (LM frozen: dgrad through
+    every GEMM, wgrad only for adapters, written straight into the parameter arena's fp32 gradient buffer). loss is None
+    without labels. With want_hidden the n_layer + 1 hidden states follow (loss, logits) as outputs, then with want_attn
+    the n_layer attention probabilities ([B, H, S, S rounded up to 8]); the gradients of the logits, the hidden states
+    and the attentions flow back through the same backward pass."""
 
     @staticmethod
     def forward(ctx, model, x, labels, anchor, want_hidden=False, want_attn=False):
@@ -229,17 +233,17 @@ class _LMTrainFn(torch.autograd.Function):
         ctx.shape = x.shape
         ctx.x_dtype = x.dtype
         ctx.n_hidden = len(hidden or ())
-        ctx.mark_non_differentiable(logits)
-        if want_hidden or want_attn:
-            ctx.set_materialize_grads(False)  # an unused hidden state or attention map has no gradient to add
+        ctx.has_labels = labels is not None
+        ctx.set_materialize_grads(False)  # an output the loss does not read has no gradient to add
         return (loss, logits, *(hidden or ()), *(attn or ()))
 
     @staticmethod
-    def backward(ctx, dloss, _dlogits, *douts):
+    def backward(ctx, dloss, dlogits, *douts):
         model = ctx.model
         if ctx.generation != model._generation:
             raise MB200Error("backward called after another training forward overwrote the saved activations")
-        dx = model._run_backward(ctx.shape, _backward_scale(model, dloss), douts[: ctx.n_hidden], douts[ctx.n_hidden :])
+        scale = _backward_scale(model, dloss) if ctx.has_labels else None
+        dx = model._run_backward(ctx.shape, scale, douts[: ctx.n_hidden], douts[ctx.n_hidden :], dlogits)
         return None, dx.to(ctx.x_dtype), None, None, None, None
 
 
@@ -489,10 +493,11 @@ class B200GPTJForCausalLM(nn.Module):
         lg = logits.view(B, 1 if last_only else S, ldv)[..., :V] if logits is not None else None
         return None, lg, hidden, attn
 
-    def _run_backward(self, shape, loss_scale, dhidden=(), dattn=()):
-        """dhidden: the gradients of the hidden states the forward returned (each None or [B, S, d]); dattn: those of
-        its attention buffers (each None or [B, H, S, S rounded up to 8]); all None or empty runs the backward of the
-        loss alone."""
+    def _run_backward(self, shape, loss_scale, dhidden=(), dattn=(), dlogits=None):
+        """loss_scale: the factor of the cross-entropy gradient, None when the forward had no labels; dhidden: the
+        gradients of the hidden states the forward returned (each None or [B, S, d]); dattn: those of its attention
+        buffers (each None or [B, H, S, S rounded up to 8]); dlogits: that of its logits (None or [B, S, V]), used as
+        autograd delivers it. All None or empty runs the backward of the loss alone."""
         B, S, d = shape
         arena = self._arena
         dx = torch.empty(B, S, d, dtype=torch.bfloat16, device=self._device)
@@ -504,7 +509,26 @@ class B200GPTJForCausalLM(nn.Module):
         def prep(gs):
             return [None if g is None else g.to(device=self._device, dtype=torch.bfloat16).contiguous() for g in gs]
 
-        if any(g is not None for g in dattn):  # hidden-state and attention gradients in one pass
+        if dlogits is not None or loss_scale is None:  # the logits' gradient joins the CE term at the LM head
+            dh, da = prep(dhidden), prep(dattn)
+            g, comb, ld_g = None, None, 0
+            if dlogits is not None:
+                V = dlogits.shape[-1]
+                # rows [B*S, V] of stride ld_g >= V: what autograd hands over, unless the loss's backward built a
+                # broadcast or a layout no [B*S, V] view has; those are copied into fresh rows. The stride is read off
+                # the 2-D view, because torch does not define the stride of a size-1 dim (S == 1).
+                g = dlogits.to(device=self._device, dtype=torch.bfloat16).reshape(B * S, V)
+                if g.stride(1) != 1 or (B * S > 1 and g.stride(0) < V):
+                    g = torch.empty(B * S, V, dtype=torch.bfloat16, device=self._device).copy_(g)
+                ld_g = g.stride(0) if B * S > 1 else V
+                comb = torch.empty(B * S, self.ldv, dtype=torch.bfloat16, device=self._device)
+            extra = (_ptr_array(dh) if any(t is not None for t in dh) else None,
+                     _ptr_array(da) if any(t is not None for t in da) else None, (S + 7) // 8 * 8,
+                     ops._ptr(g), ld_g, ops._ptr(comb))
+            loss_scale = loss_scale or 0.0
+            bwd = (lib().mb200_gptj_sched_backward_range_logits_recompute if recompute
+                   else lib().mb200_gptj_sched_backward_range_logits)
+        elif any(g is not None for g in dattn):  # hidden-state and attention gradients in one pass
             dh, da = prep(dhidden), prep(dattn)
             extra = (_ptr_array(dh) if any(g is not None for g in dh) else None, _ptr_array(da), (S + 7) // 8 * 8)
             bwd = (lib().mb200_gptj_sched_backward_range_attn_recompute if recompute
@@ -529,7 +553,15 @@ class B200GPTJForCausalLM(nn.Module):
 
     def forward(self, input_ids=None, inputs_embeds=None, labels=None, use_cache=False, past_key_values=None,
                 output_hidden_states=False, output_attentions=False, max_cache_len=None, **_unused):
-        """GPTJForCausalLM.forward. output_attentions=True adds `.attentions`: one bf16 [B, H, S, S_kv] tensor per
+        """GPTJForCausalLM.forward. Under grad, with trainable adapters or an input that requires grad and without
+        use_cache, it runs the training pass, with or without labels: `.logits` then has a grad_fn, and the gradient of
+        any loss on it joins the cross-entropy gradient at the LM head in the one backward pass (it reaches the
+        adapters and inputs_embeds). That gradient is used as autograd delivers it: B200Engine's 1/grad_accum scaling
+        applies to the cross-entropy term only, as it does for the hidden-state and attention gradients, and a loss
+        that does not read `.loss` gets no cross-entropy term, under B200Engine as well. The backward
+        of a loss on the logits takes one more bf16 [B*S, vocab rounded up to 64] buffer, the size of the logits.
+
+        output_attentions=True adds `.attentions`: one bf16 [B, H, S, S_kv] tensor per
         block (S_kv = S, or pos0 + S over a KV cache), the probabilities the block multiplied V with, as
         `attn_weights.to(value.dtype)` of hf:gptj/modeling_gptj.py:145-146 returns them; entries above the causal
         diagonal are 0. They are views of buffers whose rows are S_kv rounded up to 8 long. In training they are outputs
@@ -544,7 +576,7 @@ class B200GPTJForCausalLM(nn.Module):
         B, S, _ = inputs_embeds.shape
         out = LMOutput(loss=None, logits=None, past_key_values=None, hidden_states=None)
         has_trainable = any(p.requires_grad for _, p in self.adapter_parameters()) or inputs_embeds.requires_grad
-        if labels is not None and torch.is_grad_enabled() and has_trainable and not use_cache:
+        if torch.is_grad_enabled() and has_trainable and not use_cache:
             anchor = next((p for _, p in self.adapter_parameters() if p.requires_grad), None)
             res = _LMTrainFn.apply(self, inputs_embeds, labels, anchor, output_hidden_states, output_attentions)
             out.loss, out.logits = res[0], res[1]

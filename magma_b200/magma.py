@@ -29,8 +29,9 @@ from .utils import build_labels, get_tokenizer, print_main
 
 class _EmbedLMFn(torch.autograd.Function):
     """loss = LM(cat(prefix, wte[captions][:, :S-L]), labels): assembles the input in one gather kernel, runs the
-    fused forward, and routes d(input)[:, :L] back to the image prefix. With want_hidden the LM's n_layer + 1 hidden
-    states follow (loss, logits), and their gradients join the same backward pass (entry 0's prefix rows included)."""
+    fused forward, and routes d(input)[:, :L] back to the image prefix. The logits are differentiable, and with
+    want_hidden the LM's n_layer + 1 hidden states follow (loss, logits); the gradients of both join the same backward
+    pass (entry 0's prefix rows included)."""
 
     @staticmethod
     def forward(ctx, magma, prefix, captions, labels, anchor, want_hidden=False):
@@ -39,20 +40,18 @@ class _EmbedLMFn(torch.autograd.Function):
         loss, logits, hidden, _ = lm._run_forward(x, labels, training=True, want_hidden=want_hidden)
         ctx.magma, ctx.generation = magma, lm._generation
         ctx.shape, ctx.L, ctx.pdtype = x.shape, prefix.shape[1], prefix.dtype
-        ctx.mark_non_differentiable(logits)
-        if want_hidden:
-            ctx.set_materialize_grads(False)  # an unused hidden state has no gradient to add
+        ctx.set_materialize_grads(False)  # an output the loss does not read has no gradient to add
         return (loss, logits, *(hidden or ()))
 
     @staticmethod
-    def backward(ctx, dloss, _dlogits, *dhidden):
+    def backward(ctx, dloss, dlogits, *dhidden):
         lm = ctx.magma.lm
         if ctx.generation != lm._generation:
             raise RuntimeError("backward called after another training forward overwrote the saved activations")
         arena = ctx.magma._arena
         if arena is not None:
             arena._accumulate_current = arena.grads_live()
-        dx = lm._run_backward(ctx.shape, _backward_scale(lm, dloss), dhidden)
+        dx = lm._run_backward(ctx.shape, _backward_scale(lm, dloss), dhidden, (), dlogits)
         if arena is not None:
             arena.publish_grads()
         dprefix = dx[:, : ctx.L, :].contiguous().to(ctx.pdtype)

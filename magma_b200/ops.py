@@ -457,6 +457,16 @@ def add(a, b, c=None, out=None):
     return y
 
 
+def logits_grad_combine(dce, g, out, alpha):
+    """mb200_logits_grad_combine: out[:, :V] = alpha * dce[:, :V] + g for bf16 rows; dce and out share the row stride,
+    g [M, V] may have any."""
+    M, V = g.shape
+    assert dce.stride(0) == out.stride(0) and g.stride(1) == 1
+    check(lib().mb200_logits_grad_combine(_ptr(dce), out.stride(0), _ptr(g), g.stride(0), _ptr(out), M, V, alpha,
+                                          _stream()))
+    return out
+
+
 def peer_reduce_bcast(buffer_ptrs, offset, n, max_blocks=0):
     """mb200_peer_reduce_bcast: `buffer_ptrs` = device addresses of every rank's exchange buffer as mapped here."""
     arr = (ctypes.c_void_p * len(buffer_ptrs))(*[int(p) for p in buffer_ptrs])
