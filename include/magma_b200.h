@@ -179,6 +179,12 @@ int mb200_embed_assemble(const int64_t* captions, int64_t ldc, const void* wte, 
 /* word_embedding(ids) (magma/magma.py:205; sampling.py:88-90 input_ids path). */
 int mb200_embed_gather(const int64_t* ids, const void* wte, void* out, int32_t n, int32_t d, int32_t vocab,
                        void* stream);
+/* Backward of the two gathers above: dwte[ids[b, j]] += dy[b, j] for b < B, j < T. ids int64 [B][ld_ids]; row (b, j) of
+ * dy (bf16, 16-byte aligned rows) at dy + b * dy_bs + j * lddy; dwte fp32 [vocab, d], overwritten (accumulate == 0) or
+ * added to. An id outside [0, vocab) counts as 0, as the gathers read row 0 for it. The rows of one id are summed in
+ * position order (b * T + j) without atomics, so the result is the same bit for bit from run to run. */
+int mb200_embed_grad(const int64_t* ids, int64_t ld_ids, const void* dy, int64_t lddy, int64_t dy_bs, int32_t B, int32_t T,
+                     float* dwte, int32_t vocab, int32_t d, int32_t accumulate, void* stream);
 /* ForCausalLMLoss (hf:loss/loss_utils.py:28-67): shifted CE over bf16 logits [B*S][ldv], mean over the valid targets.
  * A target is valid when it lies in [0, V); every other label (-100, any other negative value, V..ldv-1 and beyond)
  * is ignored: its row gets zero loss and zero gradient and does not count in n_valid.
@@ -376,6 +382,24 @@ typedef struct {
   mb200_adapter_ex attn_ad;
 } mb200_gptj_layer_ex;
 
+/* fp32 gradients of GPT-J's own weights (freeze_lm: false, or any subset of them), each with its parameter's shape. A
+ * NULL entry is a frozen parameter; the training backward writes (accumulate == 0) or adds into every other one. */
+typedef struct {
+  float *ln1_g, *ln1_b;
+  float* w_qkv; /* [3d, d]: q, k and v train together */
+  float* w_out;
+  float *w_fc_in, *b_fc_in;
+  float *w_fc_out, *b_fc_out;
+} mb200_gptj_layer_grads;
+
+/* The word embedding's gradient is not here: the pass never sees the token ids. The caller scatters the input
+ * gradient dx into it with mb200_embed_grad. */
+typedef struct {
+  const mb200_gptj_layer_grads* layers; /* host array [n_layer], or NULL when no block parameter trains */
+  float *lnf_g, *lnf_b;
+  float *w_lm, *b_lm; /* a trainable LM head needs the dlogits_comb buffer of the _logits backward entry points */
+} mb200_gptj_lm_grads;
+
 typedef struct {
   int32_t n_layer, d, n_head, rotary_dim;
   int32_t vocab;
@@ -392,6 +416,7 @@ typedef struct {
   const void* lnf_b;
   const void* w_lm;
   const void* b_lm;
+  const mb200_gptj_lm_grads* lm_grads; /* NULL: the LM is frozen (dgrad through every GEMM, wgrad for adapters only) */
 } mb200_gptj_model_ex;
 
 /* bytes of caller-provided workspace for a [B,S] training pass (per-layer activations are kept: 122 MB per GPT-J-6B
@@ -404,9 +429,9 @@ size_t mb200_gptj_sched_workspace_bytes(const mb200_gptj_model_ex* m, int32_t B,
  * for the backward pass. */
 int mb200_gptj_sched_forward(const mb200_gptj_model_ex* m, const void* x, const int64_t* labels, void* logits,
                              int64_t ldv, float* loss, int32_t B, int32_t S, void* ws, size_t ws_bytes, void* stream);
-/* Backward of the pass recorded in `ws` (loss.backward() of magma/train_loop.py:18 with the LM frozen: dgrad through
- * every GEMM, wgrad only for adapters). dx: bf16 [B,S,d] gradient w.r.t. x (or NULL). accumulate != 0 adds into the
- * fp32 gradient buffers (gradient accumulation), else overwrites. */
+/* Backward of the pass recorded in `ws` (loss.backward() of magma/train_loop.py:18: dgrad through every GEMM, wgrad for
+ * the adapters and for every LM weight m->lm_grads names). dx: bf16 [B,S,d] gradient w.r.t. x (or NULL). accumulate != 0
+ * adds into the fp32 gradient buffers (gradient accumulation), else overwrites. */
 int mb200_gptj_sched_backward(const mb200_gptj_model_ex* m, void* dx, float loss_scale, int32_t accumulate, int32_t B,
                               int32_t S, void* ws, size_t ws_bytes, void* stream);
 

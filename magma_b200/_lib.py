@@ -143,6 +143,18 @@ class GptjLayerExC(ctypes.Structure):
     ] + [("mlp_ad", AdapterExC), ("attn_ad", AdapterExC)]
 
 
+class GptjLayerGradsC(ctypes.Structure):
+    """mb200_gptj_layer_grads: fp32 gradients of one block's own weights (NULL = frozen)."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ("ln1_g", "ln1_b", "w_qkv", "w_out", "w_fc_in", "b_fc_in", "w_fc_out",
+                                               "b_fc_out")]
+
+
+class GptjLmGradsC(ctypes.Structure):
+    """mb200_gptj_lm_grads."""
+    _fields_ = [("layers", ctypes.POINTER(GptjLayerGradsC))] + [
+        (n, ctypes.c_void_p) for n in ("lnf_g", "lnf_b", "w_lm", "b_lm")]
+
+
 class GptjModelExC(ctypes.Structure):
     """mb200_gptj_model_ex (include/magma_b200.h)."""
     _fields_ = [
@@ -163,6 +175,7 @@ class GptjModelExC(ctypes.Structure):
         ("lnf_b", ctypes.c_void_p),
         ("w_lm", ctypes.c_void_p),
         ("b_lm", ctypes.c_void_p),
+        ("lm_grads", ctypes.POINTER(GptjLmGradsC)),
     ]
 
 
@@ -207,6 +220,7 @@ SIGNATURES = {
     "mb200_build_labels": (_i32, [_vp, _i64, _vp, _i32, _i32, _i32, _i64, _vp]),
     "mb200_embed_assemble": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp]),
     "mb200_embed_gather": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "mb200_embed_grad": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _i32, _vp, _i32, _i32, _i32, _vp]),
     "mb200_cross_entropy": (_i32, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _vp]),
     "mb200_colsum": (_i32, [_vp, _i64, _i32, _i32, _vp, _i32, _vp]),
     "mb200_dropout_fwd": (_i32, [_vp, _vp, _vp, _i64, _f32, _u64, _vp]),

@@ -1,4 +1,5 @@
-"""Flat parameter arena for the trainable set (adapters + ImagePrefix proj/LN, ~0.24 B params).
+"""Flat parameter arena for the trainable set (adapters + ImagePrefix proj/LN, ~0.24 B params, plus whichever GPT-J
+weights train).
 
 All trainable parameters are views into ONE fp32 master buffer, with a parallel bf16 compute copy (what the kernels
 read) and a parallel fp32 gradient buffer (what wgrad kernels write). One flat buffer means: the data-parallel
@@ -7,14 +8,37 @@ reduce-scatter/all-gather, train.py:103-111), and the optimizer step is one fuse
 import torch
 
 from . import dp, ops
+from ._lib import MB200Error
+
+# what one trainable parameter costs: fp32 master, gradient and two Adam moments, and the bf16 copy the kernels read
+BYTES_PER_PARAM = 18
+
+
+def check_fits(numels, released, free):
+    """Raise MB200Error when an arena of parameters with these sizes, Adam moments included, does not fit: `free` is
+    what the device can still allocate, `released` the bytes of the parameters' current copies, which the arena
+    replaces."""
+    need = dp.arena_layout(numels)[1] * BYTES_PER_PARAM
+    if need > free + released:
+        raise MB200Error(f"the {sum(numels)} trainable parameters need {need} bytes ({need / 2**30:.1f} GiB: "
+                         f"{BYTES_PER_PARAM} bytes each for the fp32 master, gradient and two Adam moments and the bf16 "
+                         f"copy), but only {int(free + released)} bytes ({(free + released) / 2**30:.1f} GiB) can be "
+                         "allocated: train fewer parameters")
 
 
 class ParamArena:
-    def __init__(self, named_params, device):
+    def __init__(self, named_params, device, previous=None):
         """named_params: list of (name, nn.Parameter) in the order gradients become ready in backward
-        (last layer first), so early slices can be all-reduced while the rest of backward runs."""
+        (last layer first), so early slices can be all-reduced while the rest of backward runs. previous: the arena this
+        one replaces (its memory is released once the caller drops it), or None."""
+        from .language_model import _free_bytes
+
         self.names = [n for n, _ in named_params]
         self.params = [p for _, p in named_params]
+        released = previous.nbytes() if previous is not None else 0
+        released += sum(p.numel() * p.element_size() for p in self.params
+                        if p.device.type == "cuda" and not (previous is not None and previous.holds(p)))
+        check_fits([p.numel() for p in self.params], released, _free_bytes(torch.device(device)))
         self.offsets, off = dp.arena_layout([p.numel() for p in self.params])
         self.numel = off
         self.master = torch.zeros(off, dtype=torch.float32, device=device)
@@ -38,6 +62,14 @@ class ParamArena:
         self.exp_avg_sq = None
         self.gnorm_sq = torch.zeros(1, dtype=torch.float32, device=device)
         self.step_count = 0
+
+    def nbytes(self):
+        """Device bytes the arena holds: master, bf16 copy, gradient and the Adam moments once allocated."""
+        ts = (self.master, self.shadow, self.grad, self.exp_avg, self.exp_avg_sq)
+        return sum(t.numel() * t.element_size() for t in ts if t is not None and t.device.type == "cuda")
+
+    def holds(self, p):
+        return any(q is p for q in self.params)
 
     def _version(self):
         return sum(p._version for p in self.params)

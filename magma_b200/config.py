@@ -58,7 +58,7 @@ class MultimodalConfig:
     pretrained_img_encoder: bool = False  # no weight source offline; accepted for schema parity
     seq_len: int = None  # present but never read by the reference; magma_b200 uses it to set Magma.seq_len
     # freezing
-    freeze_lm: bool = True  # must stay true: the LM is frozen on this path
+    freeze_lm: bool = True  # false trains every LM parameter too (18 bytes each: ~109 GB for GPT-J-6B)
     freeze_img_encoder: bool = True  # false trains the encoder (ViT: vit_sched.cu; conv trunks: train-mode BN)
     image_embed_dropout_prob: float = 0.0  # nn.Dropout on the prefix (image_prefix.py:104)
     use_image_embed_layernorm: bool = False  # LayerNorm on the prefix (image_prefix.py:106-107)

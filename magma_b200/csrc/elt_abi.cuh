@@ -295,6 +295,26 @@ extern "C" int mb200_embed_gather(const int64_t* ids, const void* wte, void* out
   return 0;
 }
 
+extern "C" int mb200_embed_grad(const int64_t* ids, int64_t ld_ids, const void* dy, int64_t lddy, int64_t dy_bs,
+                                int32_t B, int32_t T, float* dwte, int32_t vocab, int32_t d, int32_t accumulate,
+                                void* stream) {
+  MB_ENTER();
+  MB_REQUIRE(B >= 0 && T >= 0 && (long long)B * T <= 0x7fffffffLL && vocab > 0 && d > 0 && d % 8 == 0 && ld_ids >= T &&
+                 lddy % 8 == 0 && dy_bs % 8 == 0,
+             MB200_E_SHAPE, "embed_grad: bad B=%d T=%d vocab=%d d=%d or strides (ld_ids >= T, lddy and dy_bs %% 8)", B, T,
+             vocab, d);
+  MB_REQUIRE(ids && dwte && (dy || B * T == 0) && aligned_to(16, dy, dwte), MB200_E_ALIGN,
+             "embed_grad: ids, dy, dwte must be non-NULL and dy, dwte 16-byte aligned");
+  if (!accumulate) MB_CUDA(cudaMemsetAsync(dwte, 0, (size_t)vocab * d * sizeof(float), ST(stream)));
+  const int n = B * T;
+  if (n == 0) return 0;
+  launch(embed_grad_kernel, dim3((unsigned)n, (unsigned)((d / 8 + kEgThreads - 1) / kEgThreads)), kEgThreads, 0,
+         ST(stream), (const long long*)ids, (long long)ld_ids, (const bf16*)dy, (long long)lddy, (long long)dy_bs, (int)T,
+         n, dwte, (int)vocab, (int)d);
+  MB_LAUNCH_CHECK();
+  return 0;
+}
+
 extern "C" int mb200_cross_entropy(const void* logits, int64_t ldv, const int64_t* labels, int32_t B, int32_t S,
                                    int32_t V, float* row_loss, int32_t* n_valid, float* loss, void* dlogits,
                                    float grad_scale, void* stream) {

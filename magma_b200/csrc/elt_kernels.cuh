@@ -285,6 +285,54 @@ __global__ void embed_gather_kernel(const long long* __restrict__ ids, const bf1
   for (int c = threadIdx.x; c < (d >> 3); c += blockDim.x) dst[c] = __ldg(src + c);
 }
 
+// Backward of the gathers: dwte[id(p)] += the dy rows of the positions p = b * T + j with that id. Block (p, column
+// strip) runs only when p is the first position of its id; it then walks positions p.. in order, 256 at a time, finds
+// the ones with its id by warp ballot and adds their rows, so each id's sum has one fixed order and one writer. 8
+// columns per thread.
+constexpr int kEgThreads = 256;
+__device__ __forceinline__ long long eg_id(const long long* ids, long long ld, int T, int p, int vocab) {
+  const long long t = ids[(long long)(p / T) * ld + p % T];
+  return (t < 0 || t >= vocab) ? 0 : t;  // the gathers' rule
+}
+__global__ void __launch_bounds__(kEgThreads)
+embed_grad_kernel(const long long* __restrict__ ids, long long ld_ids, const bf16* __restrict__ dy, long long lddy,
+                  long long dy_bs, int T, int n, float* __restrict__ dwte, int vocab, int d) {
+  __shared__ unsigned hits[kEgThreads / 32];
+  const int p = blockIdx.x;
+  const long long id = eg_id(ids, ld_ids, T, p, vocab);
+  int first = 1;  // no earlier position has this id
+  for (int q = threadIdx.x; q < p; q += kEgThreads) first &= eg_id(ids, ld_ids, T, q, vocab) != id;
+  if (!__syncthreads_and(first)) return;
+  const int c0 = (blockIdx.y * kEgThreads + threadIdx.x) * 8;
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int q0 = p; q0 < n; q0 += kEgThreads) {
+    const int q = q0 + (int)threadIdx.x;
+    const unsigned b = __ballot_sync(0xffffffffu, q < n && eg_id(ids, ld_ids, T, q, vocab) == id);
+    if ((threadIdx.x & 31) == 0) hits[threadIdx.x >> 5] = b;
+    __syncthreads();
+    if (c0 < d) {
+      for (int w = 0; w < kEgThreads / 32; ++w) {
+        for (unsigned m = hits[w]; m; m &= m - 1) {
+          const int r = q0 + w * 32 + __ffs(m) - 1;
+          const uint4 v = __ldg(reinterpret_cast<const uint4*>(dy + (long long)(r / T) * dy_bs + (long long)(r % T) * lddy + c0));
+          const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float2 f = __bfloat1622float2(h[k]);
+            acc[2 * k] += f.x;
+            acc[2 * k + 1] += f.y;
+          }
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (c0 >= d) return;
+  float* out = dwte + id * (long long)d + c0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) out[k] += acc[k];
+}
+
 // ---------------------------------------------------------------------------------------------
 // Shifted cross-entropy over bf16 logits [M = B*S][ldv] (ForCausalLMLoss, loss_utils.py:28-67):
 // target of row (b, s) is labels[b, s+1]; the last position and every target outside [0, V) (-100 among them) are

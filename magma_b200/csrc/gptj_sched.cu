@@ -17,8 +17,8 @@
 // Attention: the fused single-tile kernels when the sequence fits one tile (S <= 128: BASELINE config 2), the fused
 // multi-tile forward (mb200_attn_fwd_flash) for longer sequences / prefill over a KV cache — in training it also writes
 // the probabilities, and the backward then runs as strided batched GEMMs on the fused qkv buffer + softmax_bwd — and
-// batched GEMMs + softmax kernels for head dims the fused kernels do not take. The LM is frozen: dgrad through every
-// GEMM, wgrad only for adapters.
+// batched GEMMs + softmax kernels for head dims the fused kernels do not take. The backward runs dgrad through every
+// GEMM, and wgrad for the adapters and for the LM weights m->lm_grads names (none when it is NULL: the LM is frozen).
 //
 // No kernels and no CUDA calls here (sched_rt.h, which also holds the GEMM helpers and the materialised attention this
 // file shares with vit_sched.cu): tests/test_sched_emul_cpu.py compiles this file as plain C++ against
@@ -58,6 +58,7 @@ struct LayerActs {
   bf16s* P;        // [B,H,S,ldP]
   bf16s* attn_o;   // [M,d] merged heads, before out_proj
   bf16s* pre;      // [M,dff] fc_in pre-activation
+  bf16s* hact;     // [M,dff] gelu(pre): the plan's shared P.hact, or the layer's own when its fc_out trains (stored path)
   bf16s* mlp_out;  // [M,d] fc_out output (input of a "normal" MLP adapter)
   bf16s* a_out;    // [M,d] out_proj output (input of a "normal" attention adapter)
   AdapterActs am, aa;
@@ -75,6 +76,7 @@ struct Plan {
   bf16s *g0, *g1, *gs, *dt, *dzn, *dm, *dhact, *dh_mlp, *dattn_o, *dqkv, *dS, *dh, *da, *dhp;
   void* gemm_ws;  // scratch lent to the GEMM core: split-K slices
   size_t gemm_ws_bytes;
+  float* ln_scratch;  // [2d] the half of a LayerNorm's parameter gradient whose parameter is frozen
   size_t bytes;
 };
 
@@ -104,6 +106,9 @@ inline Epi rope_epi(const float* tab, int mode, int S, int hd, int rot, int ncol
 
 inline bool has_ln(const mb200_adapter_ex& a) { return a.ln_g != nullptr; }
 inline bool has_scale(const mb200_adapter_ex& a) { return a.scale != nullptr; }
+inline const mb200_gptj_layer_grads* layer_grads(const mb200_gptj_model_ex* m, int l) {
+  return m->lm_grads && m->lm_grads->layers ? &m->lm_grads->layers[l] : nullptr;
+}
 
 void carve_adapter(Carver& c, AdapterActs& a, const mb200_adapter_ex& ad, int kind, size_t M, size_t d, int r,
                    int act = 0, bool training = true) {
@@ -210,6 +215,13 @@ int make_plan(Plan& P, const mb200_gptj_model_ex* m, int B, int S, void* ws, boo
   P.dhp = c.take<bf16s>(M * d);
   P.gemm_ws_bytes = M > 128 ? kGemmScratchBytes : 0;
   P.gemm_ws = P.gemm_ws_bytes ? c.take<uint8_t>(P.gemm_ws_bytes) : nullptr;
+  // what trainable LM weights add, after everything a frozen LM's plan holds: fc_out's wgrad reads gelu(pre), which
+  // the next layer's forward overwrites in P.hact on the stored path
+  P.ln_scratch = m->lm_grads ? c.take<float>(2 * d) : nullptr;
+  for (int l = 0; l < m->n_layer; ++l) {
+    const mb200_gptj_layer_grads* G = layer_grads(m, l);
+    P.acts[l].hact = G && G->w_fc_out && !recompute ? c.take<bf16s>(M * dff) : P.hact;
+  }
   P.bytes = align_up(c.off, 256);
   return 0;
 }
@@ -272,6 +284,14 @@ int adapter_bwd(void* st, const mb200_adapter_ex& ad, const AdapterActs& a, cons
   return mb200_layernorm_bwd(P.dzn, d, z, d, ad.ln_g, a.mean, a.rstd, res, d, dz_out, d, M, d, st);
 }
 
+// gradients of a LayerNorm's weight and bias when either trains (the kernel writes both: a frozen half goes to scratch)
+int ln_param_grad(void* st, const Plan& P, const bf16s* dy, const bf16s* x, const float* mean, const float* rstd,
+                  float* g_gamma, float* g_beta, int acc) {
+  if (!g_gamma && !g_beta) return 0;
+  return mb200_layernorm_param_grad_rows(dy, P.d, x, P.d, mean, rstd, g_gamma ? g_gamma : P.ln_scratch,
+                                         g_beta ? g_beta : P.ln_scratch + P.d, P.M, P.d, acc, st);
+}
+
 // one block of the training forward: from P.acts[l].x_in to xout, keeping the activations the backward reads in
 // P.acts[l]. The forward pass and the recompute backward both issue it, so a recomputed layer is the stored one bit for bit.
 int layer_fwd(const mb200_gptj_model_ex* m, Plan& P, int l, bf16s* xout, void* st) {
@@ -314,21 +334,21 @@ int layer_fwd(const mb200_gptj_model_ex* m, Plan& P, int l, bf16s* xout, void* s
     e.bias = L.b_fc_in;
     e.act = MB200_ACT_GELU_NEW;
     e.aux_out = a.pre;
-    MBS_TRY(gemm(st, M, dff, d, mat(a.h, d), wmat(L.w_fc_in, d), P.hact, dff, 0, e));
+    MBS_TRY(gemm(st, M, dff, d, mat(a.h, d), wmat(L.w_fc_in, d), a.hact, dff, 0, e));
   }
   Epi eo;
   eo.bias = L.b_fc_out;
   if (m->mlp_adapter == MB200_ADAPTER_NONE) {
     eo.res1 = P.ax;
     eo.ld_res = d;
-    MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), xout, d, 0, eo));
+    MBS_TRY(gemm(st, M, d, dff, mat(a.hact, dff), wmat(L.w_fc_out, dff), xout, d, 0, eo));
   } else if (m->mlp_adapter == MB200_ADAPTER_NORMAL) {  // Sequential(mlp, Adapter): A(mlp(h)) + mlp(h)
-    MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
+    MBS_TRY(gemm(st, M, d, dff, mat(a.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
     MBS_TRY(adapter_fwd(st, L.mlp_ad, a.am, M, d, m->mlp_adapter_r, m->ln_eps, a.mlp_out, xout, a.mlp_out, P.ax, m->adapter_act));
   } else {  // ParallelAdapter: mlp(h) + s * A(h)
     eo.res1 = P.ax;
     eo.ld_res = d;
-    MBS_TRY(gemm(st, M, d, dff, mat(P.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
+    MBS_TRY(gemm(st, M, d, dff, mat(a.hact, dff), wmat(L.w_fc_out, dff), a.mlp_out, d, 0, eo));
     MBS_TRY(adapter_fwd(st, L.mlp_ad, a.am, M, d, m->mlp_adapter_r, m->ln_eps, a.h, xout, a.mlp_out, nullptr, m->adapter_act));
   }
   return 0;
@@ -391,6 +411,9 @@ int forward(const mb200_gptj_model_ex* m, const bf16s* x, const int64_t* labels,
 // the LM head's dgrad then reads with alpha 1, so P.dlogits is never written and a second backward gives the same
 // result. Without dlg and with loss_scale == 0 (a forward without labels, whose P.dlogits was never written) the LM
 // head adds nothing and P.dlogits is not read.
+// m->lm_grads: the weight gradients of the LM's own parameters join those of the adapters, from the gradients the dgrad
+// GEMMs read and the activations the forward kept (each block's on the recompute path once it is rebuilt). A trainable
+// LM head needs dcomb: its gradient, loss_scale * P.dlogits (+ dlg), is formed there once and read by all three GEMMs.
 int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, float loss_scale, int layer_hi,
              int layer_lo, int acc, int B, int S, void* ws, size_t ws_bytes, void* st, bool recompute,
              const bf16s* const* dattn = nullptr, long long ld_attn = 0, bool logits_grad = false,
@@ -410,11 +433,17 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, 
   // gradient w.r.t. the residual stream entering layer l lives in g[(l) & 1]
   bf16s* gb[2] = {P.g0, P.g1};
   if (layer_hi == m->n_layer) {  // dxf = loss_scale * dlogits Wlm ; g = LN_f backward
+    const mb200_gptj_lm_grads* G = m->lm_grads;
+    const bool head_trains = G && (G->w_lm || G->b_lm);
     const bf16s* dhf = dhid ? dhid[m->n_layer] : nullptr;
     const bf16s* dxf = P.dh;
     if (logits_grad && !dlg && loss_scale == 0.f) {  // nothing reaches the LM head
       if (dhf) dxf = dhf;
       else MBS_TRY(rt_zero(P.dh, (size_t)M * d * sizeof(bf16s), st));
+      if (head_trains && !acc) {
+        if (G->w_lm) MBS_TRY(rt_zero(G->w_lm, (size_t)m->vocab * d * sizeof(float), st));
+        if (G->b_lm) MBS_TRY(rt_zero(G->b_lm, (size_t)m->vocab * sizeof(float), st));
+      }
     } else {
       Epi e;
       e.alpha = loss_scale;
@@ -429,11 +458,21 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, 
                                           loss_scale, st));
         dl = dcomb;
         e.alpha = 1.f;
+      } else if (head_trains) {  // dcomb = loss_scale * dlogits, formed as (loss_scale - 1) * dlogits + dlogits
+        MBS_REQUIRE(dcomb, MB200_E_ARG,
+                    "gptj_sched_backward: a trainable LM head needs the dlogits_comb buffer of the _logits entry points");
+        MBS_REQUIRE(mb200_logits_grad_combine, MB200_E_ARG, "gptj_sched: mb200_logits_grad_combine is not in this build");
+        MBS_TRY(mb200_logits_grad_combine(P.dlogits, P.ldv, P.dlogits, P.ldv, dcomb, M, m->vocab, loss_scale - 1.f, st));
+        dl = dcomb;
+        e.alpha = 1.f;
       }
       MBS_TRY(gemm(st, M, d, m->vocab, mat(dl, P.ldv), wmat(m->w_lm, d, 1), P.dh, d, 0, e));
+      if (head_trains && G->w_lm) MBS_TRY(wgrad(st, m->vocab, d, M, dl, P.ldv, P.xf_ln, d, G->w_lm, d, acc));  // dl^T xf
+      if (head_trains && G->b_lm) MBS_TRY(mb200_colsum(dl, P.ldv, M, m->vocab, G->b_lm, acc, st));
     }
     MBS_TRY(mb200_layernorm_bwd(dxf, d, P.x_final, d, m->lnf_g, P.lnf_mean, P.lnf_rstd, nullptr, 0, gb[m->n_layer & 1], d,
                                 M, d, st));
+    if (G) MBS_TRY(ln_param_grad(st, P, dxf, P.x_final, P.lnf_mean, P.lnf_rstd, G->lnf_g, G->lnf_b, acc));
   }
   for (int l = layer_hi - 1; l >= layer_lo; --l) {
     if (recompute) MBS_TRY(layer_fwd(m, P, l, P.dh, st));
@@ -492,6 +531,15 @@ int backward(const mb200_gptj_model_ex* m, bf16s* dx, const bf16s* const* dhid, 
     }
     MBS_TRY(mb200_layernorm_bwd(P.dh, d, a.x_in, d, L.ln1_g, a.mean, a.rstd, g, d, gout, d, M, d, st));
     if (dhid && dhid[l]) MBS_TRY(mb200_add(gout, dhid[l], nullptr, gout, (int64_t)M * d, st));
+    if (const mb200_gptj_layer_grads* G = layer_grads(m, l)) {  // the block's own weights: dW = dy^T x of each linear
+      if (G->w_qkv) MBS_TRY(wgrad(st, 3 * d, d, M, P.dqkv, 3 * d, a.h, d, G->w_qkv, d, acc));
+      if (G->w_out) MBS_TRY(wgrad(st, d, d, M, da, d, a.attn_o, d, G->w_out, d, acc));
+      if (G->w_fc_in) MBS_TRY(wgrad(st, dff, d, M, P.dhact, dff, a.h, d, G->w_fc_in, d, acc));
+      if (G->b_fc_in) MBS_TRY(mb200_colsum(P.dhact, dff, M, dff, G->b_fc_in, acc, st));
+      if (G->w_fc_out) MBS_TRY(wgrad(st, d, dff, M, dm, d, a.hact, dff, G->w_fc_out, dff, acc));
+      if (G->b_fc_out) MBS_TRY(mb200_colsum(dm, d, M, d, G->b_fc_out, acc, st));
+      MBS_TRY(ln_param_grad(st, P, P.dh, a.x_in, a.mean, a.rstd, G->ln1_g, G->ln1_b, acc));
+    }
   }
   return 0;
 }

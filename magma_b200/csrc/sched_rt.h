@@ -65,8 +65,9 @@ struct Mat {
 inline Mat mat(const void* p, long long ld, int mn = 0, long long bs0 = 0, long long bs1 = 0) {
   return Mat{p, ld, bs0, bs1, mn, 0};
 }
-// a frozen weight matrix (never written by a kernel of the stream): the GEMM may fetch its first tiles ahead of the
-// programmatic dependency on the previous kernel (mb200_operand.static_data)
+// a weight matrix no kernel of the pass writes: the GEMM may fetch its first tiles ahead of the programmatic dependency
+// on the previous kernel (mb200_operand.static_data). A trainable GPT-J weight qualifies too: only the optimizer step
+// writes it, between passes, and every pass starts with a copy or a plain launch that waits for all earlier work.
 inline Mat wmat(const void* p, long long ld, int mn = 0) { return Mat{p, ld, 0, 0, mn, 1}; }
 struct Epi {
   float alpha = 1.f;

@@ -4,6 +4,7 @@ The reference's only parallelism is DP under DeepSpeed ZeRO-2 (train.py:103-111)
 holds the full (frozen) model and a flat fp32 gradient arena for the ~0.24 B trainable parameters; the arena is
 laid out in the order gradients become ready in backward (last GPT-J layer first, image prefix last) and is
 all-reduced slice by slice as backward proceeds."""
+import re
 from typing import List, Sequence, Tuple
 
 import torch
@@ -21,11 +22,20 @@ def arena_layout(numels: Sequence[int]) -> Tuple[List[int], int]:
     return offs, off
 
 
+_BLOCK = re.compile(r"(?:^|\.)transformer\.h\.(\d+)\.")
+_HEAD = re.compile(r"(?:^|\.)(?:lm_head|transformer\.ln_f)\.")
+
+
 def backward_order_key(name: str):
-    """Sort key: GPT-J layers descending (their gradients are produced first), then everything else."""
-    if ".transformer.h." in name:
-        return (0, -int(name.split(".transformer.h.")[1].split(".")[0]))
-    return (1, 0)
+    """Sort key in the order the backward produces gradients: the LM head and ln_f, GPT-J layers descending, then
+    everything else (the word embedding and the image prefix, from the input gradient). Names may carry a prefix
+    (`lm.` in Magma)."""
+    if _HEAD.search(name):
+        return (0, 0)
+    m = _BLOCK.search(name)
+    if m:
+        return (1, -int(m.group(1)))
+    return (2, 0)
 
 
 def layer_chunks(n_layer: int, n_buckets: int) -> List[Tuple[int, int]]:

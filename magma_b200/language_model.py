@@ -7,7 +7,8 @@ magma/magma.py:128-169), `named_parameters()` with "adapter" in adapter names, a
 `__call__(inputs_embeds=|input_ids=, labels=, use_cache=, past_key_values=, output_hidden_states=, output_attentions=)`
 returning an object with `.loss`, `.logits`, `.past_key_values`, `.hidden_states` (and `.attentions` when asked for).
 
-All frozen weights are bf16 tensors on the GPU; parameter names follow HF GPT-J (`attn.q_proj.weight`, `mlp.fc_in.*`,
+Frozen weights are bf16 tensors on the GPU; a weight set to train (requires_grad, then `finalize()`) moves into the
+fp32 parameter arena, and the kernels read the arena's bf16 copy of it. Parameter names follow HF GPT-J (`attn.q_proj.weight`, `mlp.fc_in.*`,
 `ln_1`, `ln_f`, `lm_head`) — the executable stand-in for the reference's fork. The whole
 28-block forward and backward run inside libmagma_b200.so (csrc/gptj_sched.cu); this file only owns tensors and plumbing.
 """
@@ -20,7 +21,8 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from ._lib import (AdapterExC, GptjLayerExC, GptjModelExC, MB200Error, check,
+from . import dp
+from ._lib import (AdapterExC, GptjLayerExC, GptjLayerGradsC, GptjLmGradsC, GptjModelExC, MB200Error, check,
                    lib)
 from .adapters import Adapter, AdapterWrapper, ParallelAdapter, ParallelAdapterWrapper
 from .arena import ParamArena
@@ -106,9 +108,17 @@ class WordEmbedding(nn.Module):
     def __init__(self, V, d, device):
         super().__init__()
         self.weight = _frozen(V, d, device=device)
+        self._arena = None  # the parameter arena while the weight trains
+
+    def compute_weight(self):
+        """The bf16 [V, d] table the kernels read: the weight, or the arena's bf16 copy of it while it trains."""
+        if self._arena is None:
+            return self.weight
+        self._arena.sync_shadow()
+        return self._arena.shadow_of(self.weight)
 
     def forward(self, ids):
-        return ops.embed_gather(ids.to(self.weight.device), self.weight)
+        return ops.embed_gather(ids.to(self.weight.device), self.compute_weight())
 
 
 class GPTJAttention(nn.Module):
@@ -124,9 +134,10 @@ class GPTJAttention(nn.Module):
     def fused_qkv(self):
         """[3d, d] = cat(q, k, v) weights in one buffer (re-fused if a .to()/load split the views)."""
         d = self.q_proj.weight.shape[0]
-        base, esz = self._fused.data_ptr(), 2
+        base, esz = (self._fused.data_ptr(), 2) if self._fused is not None else (0, 2)
         ptrs = [p.weight.data_ptr() for p in (self.q_proj, self.k_proj, self.v_proj)]
-        if ptrs != [base, base + d * d * esz, base + 2 * d * d * esz] or self._fused.device != self.q_proj.weight.device:
+        if (self._fused is None or ptrs != [base, base + d * d * esz, base + 2 * d * d * esz]
+                or self._fused.device != self.q_proj.weight.device):
             dev = self.q_proj.weight.device
             fused = torch.cat([p.weight.data.to(torch.bfloat16) for p in (self.q_proj, self.k_proj, self.v_proj)], 0).to(dev)
             self._fused = fused
@@ -205,6 +216,25 @@ def _free_bytes(device):
     return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
 
 
+def _block_index(name):
+    m = dp._BLOCK.search(name)
+    return int(m.group(1)) if m else None
+
+
+def lm_train_check(named_params):
+    """Raise when the trainable choice among GPT-J's own parameters (named as `named_parameters()` gives them, with or
+    without a prefix) cannot run: q_proj, k_proj and v_proj of a block are one fused [3d, d] weight and train together."""
+    qkv = {}
+    for n, p in named_params:
+        for part in ("q_proj", "k_proj", "v_proj"):
+            if f".{part}.weight" in n:
+                qkv.setdefault(_block_index(n), set()).add(bool(p.requires_grad))
+    mixed = sorted(l for l, v in qkv.items() if len(v) > 1)
+    if mixed:
+        raise MB200Error(f"q_proj, k_proj and v_proj of block {mixed[0]} must train together or not at all: they are one "
+                         "fused [3d, d] weight (attn.fused_qkv)")
+
+
 def _backward_scale(model, dloss):
     """The loss gradient the LM head's backward scales the cross-entropy gradient by: 0 when the loss does not read
     `.loss` (also under B200Engine.backward: its hint must not add a CE term the loss does not have), else
@@ -225,10 +255,11 @@ class _LMTrainFn(torch.autograd.Function):
     and the attentions flow back through the same backward pass."""
 
     @staticmethod
-    def forward(ctx, model, x, labels, anchor, want_hidden=False, want_attn=False):
+    def forward(ctx, model, x, labels, anchor, want_hidden=False, want_attn=False, ids=None):
         loss, logits, hidden, attn = model._run_forward(x, labels, training=True, want_hidden=want_hidden,
                                                         want_attn=want_attn)
         ctx.model = model
+        ctx.ids = ids  # input_ids whose embedding rows receive dx, when the word embedding trains
         ctx.generation = model._generation
         ctx.shape = x.shape
         ctx.x_dtype = x.dtype
@@ -243,8 +274,9 @@ class _LMTrainFn(torch.autograd.Function):
         if ctx.generation != model._generation:
             raise MB200Error("backward called after another training forward overwrote the saved activations")
         scale = _backward_scale(model, dloss) if ctx.has_labels else None
-        dx = model._run_backward(ctx.shape, scale, douts[: ctx.n_hidden], douts[ctx.n_hidden :], dlogits)
-        return None, dx.to(ctx.x_dtype), None, None, None, None
+        dx = model._run_backward(ctx.shape, scale, douts[: ctx.n_hidden], douts[ctx.n_hidden :], dlogits,
+                                 embed=None if ctx.ids is None else (ctx.ids, 0))
+        return None, dx.to(ctx.x_dtype), None, None, None, None, None
 
 
 class B200GPTJForCausalLM(nn.Module):
@@ -298,18 +330,69 @@ class B200GPTJForCausalLM(nn.Module):
     def adapter_parameters(self):
         return [(n, p) for n, p in self.named_parameters() if "adapter" in n]
 
+    def lm_parameters(self):
+        """GPT-J's own parameters (everything but the adapters), as (name, parameter)."""
+        return [(n, p) for n, p in self.named_parameters() if "adapter" not in n]
+
     def attach_arena(self, arena: ParamArena):
         self._arena = arena
         self._own_arena = False
         self._cmodel_ex_cache = None
+        self._arena_attached()
 
-    def _ensure_arena(self):
+    def _in_arena(self, p):
+        return self._arena is not None and any(q is p for q in self._arena.params)
+
+    def _arena_attached(self):
+        """The embedding reads its table from the arena while it trains; the bf16 fused q/k/v copy of a block whose
+        projections train is freed (the kernels read the arena's)."""
+        for _, p in self.lm_parameters():
+            if self._in_arena(p):
+                p._mb200_arena_fp32 = True  # its data is now an fp32 view of the arena's master copy
+        wte = self.transformer.wte
+        wte._arena = self._arena if self._in_arena(wte.weight) else None
+        for blk in self.transformer.h:
+            attn = _split_attn(blk.attn)[1]
+            if self._in_arena(attn.q_proj.weight):
+                attn._fused = None
+
+    def prepare_lm_parameters(self):
+        """Check the trainable choice among the LM's own parameters and return frozen ones an earlier arena held in
+        fp32 to the bf16 the kernels read (their bf16 copies were freed when they moved into it). Other parameters are
+        left as they are: a frozen one in another dtype is refused by the next pass."""
+        lm_train_check(self.lm_parameters())
+        for _, p in self.lm_parameters():
+            if not p.requires_grad and getattr(p, "_mb200_arena_fp32", False):
+                p.data = p.data.to(torch.bfloat16)
+                p._mb200_arena_fp32 = False
+
+    def finalize(self):
+        """(Re)build this model's own parameter arena after changing which parameters train (requires_grad): the
+        adapters and every trainable LM parameter, fp32 master copies the optimizer updates. Raises before allocating
+        when the arena and its Adam moments do not fit in the memory the device can still allocate."""
+        previous = self._arena if self._own_arena else None
+        self.invalidate()
+        self.drop_training_workspace()
+        self._ensure_arena(previous)
+        return self
+
+    def drop_training_workspace(self):
+        """Free the training workspace: its layout depends on which LM weights train. A backward of a forward run before
+        this raises."""
+        for k in [k for k in self._ws if isinstance(k, tuple) and k[0] == "ex"]:
+            del self._ws[k]
+        self._generation += 1
+
+    def _ensure_arena(self, previous=None):
         if self._arena is None:
-            params = self.adapter_parameters()
-            # backward visits layers last-to-first: order the arena the same way for all-reduce overlap
-            params.sort(key=lambda np_: -int(np_[0].split(".h.")[1].split(".")[0]) if ".h." in np_[0] else 0)
-            self._arena = ParamArena(params, self._device) if params else None
+            self.prepare_lm_parameters()
+            params = self.adapter_parameters() + [(n, p) for n, p in self.lm_parameters() if p.requires_grad]
+            # the order the backward produces gradients in (LM head, layers last-to-first, embedding), for all-reduce
+            # overlap
+            params.sort(key=lambda np_: dp.backward_order_key(np_[0]))
+            self._arena = ParamArena(params, self._device, previous) if params else None
             self._own_arena = True
+            self._arena_attached()
         return self._arena
 
     # ---- C model struct ---------------------------------------------------------------------
@@ -332,24 +415,51 @@ class B200GPTJForCausalLM(nn.Module):
                 c.g_scale = ar.grad_of(sc).data_ptr()
         return c
 
+    def _lm_weight(self, p, grad_of_trainable):
+        """(pointer the kernels read, fp32 gradient pointer or None) of an LM parameter: the weight itself while it is
+        frozen, the arena's bf16 copy and gradient slice while it trains."""
+        if not p.requires_grad:
+            return p.data_ptr(), None
+        if not self._in_arena(p):
+            raise MB200Error("an LM parameter requires grad but is not in the parameter arena: call finalize() after "
+                             "changing requires_grad")
+        grad_of_trainable.append(p)
+        return self._arena.shadow_of(p).data_ptr(), self._arena.grad_of(p).data_ptr()
+
     def _cmodel_ex(self):
-        """mb200_gptj_model_ex: frozen-weight pointers and the adapter tables (every adapter form of the reference)."""
+        """mb200_gptj_model_ex: weight pointers, the adapter tables (every adapter form of the reference) and the
+        gradient table of the trainable LM weights (NULL when the LM is frozen)."""
         self._ensure_arena()
         if self._cmodel_ex_cache is not None:
             return self._cmodel_ex_cache
+        lm_train_check(self.lm_parameters())
         cfg = self.config
-        n = len(self.transformer.h)
+        n, d = len(self.transformer.h), cfg.hidden_size
         layers = (GptjLayerExC * n)()
+        lgrads = (GptjLayerGradsC * n)()
+        trains, block_trains = [], []
         kinds, rm, ra = set(), 0, 0
         for l, blk in enumerate(self.transformer.h):
             mk, mlp, mad = _split_mlp(blk.mlp)
             ak, attn, aad = _split_attn(blk.attn)
             kinds.add((mk, ak))
-            L = layers[l]
-            L.ln1_g, L.ln1_b = blk.ln_1.weight.data_ptr(), blk.ln_1.bias.data_ptr()
-            L.w_qkv, L.w_out = attn.fused_qkv().data_ptr(), attn.out_proj.weight.data_ptr()
-            L.w_fc_in, L.b_fc_in = mlp.fc_in.weight.data_ptr(), mlp.fc_in.bias.data_ptr()
-            L.w_fc_out, L.b_fc_out = mlp.fc_out.weight.data_ptr(), mlp.fc_out.bias.data_ptr()
+            L, G = layers[l], lgrads[l]
+            for lf, gf, p in (("ln1_g", "ln1_g", blk.ln_1.weight), ("ln1_b", "ln1_b", blk.ln_1.bias),
+                              ("w_out", "w_out", attn.out_proj.weight), ("w_fc_in", "w_fc_in", mlp.fc_in.weight),
+                              ("b_fc_in", "b_fc_in", mlp.fc_in.bias), ("w_fc_out", "w_fc_out", mlp.fc_out.weight),
+                              ("b_fc_out", "b_fc_out", mlp.fc_out.bias)):
+                ptr, gptr = self._lm_weight(p, block_trains)
+                setattr(L, lf, ptr)
+                setattr(G, gf, gptr)
+            q = attn.q_proj.weight
+            if q.requires_grad:  # q, k, v back to back in the arena: one [3d, d] weight and one gradient
+                ptrs = [self._lm_weight(p.weight, block_trains) for p in (attn.q_proj, attn.k_proj, attn.v_proj)]
+                if [w for w, _ in ptrs] != [ptrs[0][0] + i * d * d * 2 for i in range(3)] or \
+                        [g for _, g in ptrs] != [ptrs[0][1] + i * d * d * 4 for i in range(3)]:
+                    raise MB200Error(f"q/k/v of block {l} are not back to back in the parameter arena")
+                L.w_qkv, G.w_qkv = ptrs[0]
+            else:
+                L.w_qkv = attn.fused_qkv().data_ptr()
             L.mlp_ad, L.attn_ad = self._adapter_struct_ex(mad), self._adapter_struct_ex(aad)
             rm = mad.bottleneck if mad is not None else rm
             ra = aad.bottleneck if aad is not None else ra
@@ -360,8 +470,8 @@ class B200GPTJForCausalLM(nn.Module):
                 for ad in (_split_mlp(blk.mlp)[2], _split_attn(blk.attn)[2]) if ad is not None}
         if len(acts) > 1:
             raise MB200Error("all adapters must use the same activation")
-        for name, p in self.named_parameters():
-            if "adapter" not in name and (p.dtype != torch.bfloat16 or p.device.type != self._device.type):
+        for name, p in self.lm_parameters():
+            if not p.requires_grad and (p.dtype != torch.bfloat16 or p.device.type != self._device.type):
                 raise MB200Error(f"frozen LM parameter {name} must be bf16 on {self._device} (got {p.dtype}, {p.device})")
         m = GptjModelExC()
         m.n_layer, m.d, m.n_head, m.rotary_dim = n, cfg.hidden_size, cfg.num_heads, cfg.rotary_dim
@@ -370,10 +480,24 @@ class B200GPTJForCausalLM(nn.Module):
         m.ln_eps = cfg.layer_norm_epsilon
         m.adapter_act = acts.pop() if acts else 0
         m.layers = ctypes.cast(layers, ctypes.POINTER(GptjLayerExC))
-        m.lnf_g, m.lnf_b = self.transformer.ln_f.weight.data_ptr(), self.transformer.ln_f.bias.data_ptr()
-        m.w_lm, m.b_lm = self.lm_head.weight.data_ptr(), self.lm_head.bias.data_ptr()
-        self._cmodel_ex_cache = (m, layers)
+        top = GptjLmGradsC()
+        for f, p in (("lnf_g", self.transformer.ln_f.weight), ("lnf_b", self.transformer.ln_f.bias),
+                     ("w_lm", self.lm_head.weight), ("b_lm", self.lm_head.bias)):
+            ptr, gptr = self._lm_weight(p, trains)
+            setattr(m, f, ptr)
+            setattr(top, f, gptr)
+        if block_trains:
+            top.layers = ctypes.cast(lgrads, ctypes.POINTER(GptjLayerGradsC))
+        if trains or block_trains:
+            m.lm_grads = ctypes.pointer(top)
+        self._cmodel_ex_cache = (m, layers, lgrads, top)
         return self._cmodel_ex_cache
+
+    def _head_trains(self):
+        return self.lm_head.weight.requires_grad or self.lm_head.bias.requires_grad
+
+    def _wte_trains(self):
+        return self.transformer.wte._arena is not None
 
     def _workspace_ex(self, B, S):
         """(training workspace for [B, S], whether its pass recomputes block activations). The path is chosen once,
@@ -493,11 +617,13 @@ class B200GPTJForCausalLM(nn.Module):
         lg = logits.view(B, 1 if last_only else S, ldv)[..., :V] if logits is not None else None
         return None, lg, hidden, attn
 
-    def _run_backward(self, shape, loss_scale, dhidden=(), dattn=(), dlogits=None):
+    def _run_backward(self, shape, loss_scale, dhidden=(), dattn=(), dlogits=None, embed=None):
         """loss_scale: the factor of the cross-entropy gradient, None when the forward had no labels; dhidden: the
         gradients of the hidden states the forward returned (each None or [B, S, d]); dattn: those of its attention
         buffers (each None or [B, H, S, S rounded up to 8]); dlogits: that of its logits (None or [B, S, V]), used as
-        autograd delivers it. All None or empty runs the backward of the loss alone."""
+        autograd delivers it. All None or empty runs the backward of the loss alone. embed: (ids [B, T], L) when the
+        word embedding trains and input rows L .. L+T-1 are its rows ids: dx of those rows is added to its gradient
+        before the last layer chunk's callback."""
         B, S, d = shape
         arena = self._arena
         dx = torch.empty(B, S, d, dtype=torch.bfloat16, device=self._device)
@@ -509,7 +635,8 @@ class B200GPTJForCausalLM(nn.Module):
         def prep(gs):
             return [None if g is None else g.to(device=self._device, dtype=torch.bfloat16).contiguous() for g in gs]
 
-        if dlogits is not None or loss_scale is None:  # the logits' gradient joins the CE term at the LM head
+        if dlogits is not None or loss_scale is None or self._head_trains():
+            # the logits' gradient joins the CE term at the LM head; a trainable head reads the combined buffer too
             dh, da = prep(dhidden), prep(dattn)
             g, comb, ld_g = None, None, 0
             if dlogits is not None:
@@ -521,6 +648,7 @@ class B200GPTJForCausalLM(nn.Module):
                 if g.stride(1) != 1 or (B * S > 1 and g.stride(0) < V):
                     g = torch.empty(B * S, V, dtype=torch.bfloat16, device=self._device).copy_(g)
                 ld_g = g.stride(0) if B * S > 1 else V
+            if dlogits is not None or self._head_trains():
                 comb = torch.empty(B * S, self.ldv, dtype=torch.bfloat16, device=self._device)
             extra = (_ptr_array(dh) if any(t is not None for t in dh) else None,
                      _ptr_array(da) if any(t is not None for t in da) else None, (S + 7) // 8 * 8,
@@ -545,6 +673,10 @@ class B200GPTJForCausalLM(nn.Module):
         for hi, lo in (self._bwd_chunks or [(len(self.transformer.h), 0)]):
             check(bwd(ctypes.byref(self._cmodel_ex()[0]), ops._ptr(dx) if lo == 0 else None, *extra, loss_scale, hi, lo,
                       accumulate, B, S, ops._ptr(ws), ws.numel(), ops._stream()))
+            if lo == 0 and embed is not None and self._wte_trains():
+                ids, L = embed
+                ids = ids.to(device=self._device, dtype=torch.int64)
+                ops.embed_grad(ids, dx[:, L : L + ids.shape[1]], arena.grad_of(self.transformer.wte.weight), accumulate)
             if self._after_chunk is not None:
                 self._after_chunk(hi, lo)
         if arena is not None and self._own_arena:
@@ -553,8 +685,8 @@ class B200GPTJForCausalLM(nn.Module):
 
     def forward(self, input_ids=None, inputs_embeds=None, labels=None, use_cache=False, past_key_values=None,
                 output_hidden_states=False, output_attentions=False, max_cache_len=None, **_unused):
-        """GPTJForCausalLM.forward. Under grad, with trainable adapters or an input that requires grad and without
-        use_cache, it runs the training pass, with or without labels: `.logits` then has a grad_fn, and the gradient of
+        """GPTJForCausalLM.forward. Under grad, with trainable adapters or LM parameters (see finalize) or an input that
+        requires grad and without use_cache, it runs the training pass, with or without labels: `.logits` then has a grad_fn, and the gradient of
         any loss on it joins the cross-entropy gradient at the LM head in the one backward pass (it reaches the
         adapters and inputs_embeds). That gradient is used as autograd delivers it: B200Engine's 1/grad_accum scaling
         applies to the cross-entropy term only, as it does for the hidden-state and attention gradients, and a loss
@@ -571,14 +703,17 @@ class B200GPTJForCausalLM(nn.Module):
         them."""
         if (input_ids is None) == (inputs_embeds is None):
             raise ValueError("pass exactly one of input_ids / inputs_embeds")
+        ids = None
+        self._ensure_arena()
         if inputs_embeds is None:
             inputs_embeds = self.transformer.wte(input_ids)
+            ids = input_ids if self._wte_trains() else None  # their rows receive dx
         B, S, _ = inputs_embeds.shape
         out = LMOutput(loss=None, logits=None, past_key_values=None, hidden_states=None)
-        has_trainable = any(p.requires_grad for _, p in self.adapter_parameters()) or inputs_embeds.requires_grad
-        if torch.is_grad_enabled() and has_trainable and not use_cache:
-            anchor = next((p for _, p in self.adapter_parameters() if p.requires_grad), None)
-            res = _LMTrainFn.apply(self, inputs_embeds, labels, anchor, output_hidden_states, output_attentions)
+        trainable = [p for p in self.parameters() if p.requires_grad]
+        if torch.is_grad_enabled() and (trainable or inputs_embeds.requires_grad) and not use_cache:
+            anchor = trainable[0] if trainable else None
+            res = _LMTrainFn.apply(self, inputs_embeds, labels, anchor, output_hidden_states, output_attentions, ids)
             out.loss, out.logits = res[0], res[1]
             nh = len(self.transformer.h) + 1 if output_hidden_states else 0
             if output_hidden_states:

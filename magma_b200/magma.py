@@ -3,12 +3,14 @@
 
 Differences from the reference, all deliberate:
   * the LM is really frozen when `freeze_lm` is set (the reference only sets requires_grad=True on adapters and
-    never False on anything, magma/magma.py:93-96);
+    never False on anything, magma/magma.py:93-96); with `freeze_lm: false` every LM parameter trains, as in the
+    reference, and any subset can be chosen with requires_grad followed by `finalize()`;
   * `seq_len` defaults to the LM's max_position_embeddings (2048) like the reference but honours `config.seq_len`
     and stays a plain attribute (`model.seq_len = 128`);
   * the word embedding is gathered straight into the fused [B,S,d] input buffer (the reference embeds the full
     padded caption and slices, magma.py:258-267) — same values;
-  * trainable parameters (adapters, image_prefix.proj/ln) live in one flat fp32 arena with a bf16 compute copy.
+  * trainable parameters (adapters, image_prefix.proj/ln, trainable LM weights) live in one flat fp32 arena with a
+    bf16 compute copy.
 """
 from copy import deepcopy
 from pathlib import Path
@@ -36,9 +38,10 @@ class _EmbedLMFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, magma, prefix, captions, labels, anchor, want_hidden=False):
         lm = magma.lm
-        x = ops.embed_assemble(captions, lm.transformer.wte.weight, prefix.to(torch.bfloat16).contiguous())
+        x = ops.embed_assemble(captions, lm.transformer.wte.compute_weight(), prefix.to(torch.bfloat16).contiguous())
         loss, logits, hidden, _ = lm._run_forward(x, labels, training=True, want_hidden=want_hidden)
         ctx.magma, ctx.generation = magma, lm._generation
+        ctx.captions = captions  # row L + j of x is the embedding of captions[:, j]
         ctx.shape, ctx.L, ctx.pdtype = x.shape, prefix.shape[1], prefix.dtype
         ctx.set_materialize_grads(False)  # an output the loss does not read has no gradient to add
         return (loss, logits, *(hidden or ()))
@@ -51,7 +54,9 @@ class _EmbedLMFn(torch.autograd.Function):
         arena = ctx.magma._arena
         if arena is not None:
             arena._accumulate_current = arena.grads_live()
-        dx = lm._run_backward(ctx.shape, _backward_scale(lm, dloss), dhidden, (), dlogits)
+        L = ctx.L
+        dx = lm._run_backward(ctx.shape, _backward_scale(lm, dloss), dhidden, (), dlogits,
+                              embed=(ctx.captions[:, : ctx.shape[1] - L], L))
         if arena is not None:
             arena.publish_grads()
         dprefix = dx[:, : ctx.L, :].contiguous().to(ctx.pdtype)
@@ -104,11 +109,8 @@ class Magma(nn.Module):
                 self.add_adapters(location="attention", adapter_type=attn_config.pop("adapter_type"), **attn_config)
 
         # freezing (intended semantics of magma.py:92-100)
-        if config.freeze_lm:
-            for name, param in self.lm.named_parameters():
-                param.requires_grad = bool(config.adapter_config) and "adapter" in name
-        else:
-            raise NotImplementedError("freeze_lm: false (full LM fine-tuning) is outside the re-backed hot path")
+        for name, param in self.lm.named_parameters():
+            param.requires_grad = not config.freeze_lm or (bool(config.adapter_config) and "adapter" in name)
         # magma.py:98-100 freezes the encoder only when asked to (MAGMA_v1.yml trains it). The ViT family has a backward
         # pass (csrc/vit_sched.cu); the conv trunks do not (eval-mode BatchNorm folded into their weights).
         enc_trains = (not config.freeze_img_encoder) and getattr(self.image_prefix.enc, "supports_training", False)
@@ -128,16 +130,17 @@ class Magma(nn.Module):
 
     # ------------------------------------------------------------------------------------------
     def finalize(self):
-        """(Re)build the trainable-parameter arena: adapters in reverse layer order (the order their gradients
-        become ready), then the image prefix. Call again after adding/removing trainable parameters."""
+        """(Re)build the trainable-parameter arena in the order gradients become ready: the LM head and ln_f, the
+        blocks' adapters and weights in reverse layer order, then the word embedding and the image prefix. Call again
+        after adding/removing trainable parameters (requires_grad). Raises before allocating when the arena and its Adam
+        moments do not fit in the memory the device can still allocate."""
+        self.lm.prepare_lm_parameters()
         named = [(n, p) for n, p in self.named_parameters() if p.requires_grad]
 
         named.sort(key=lambda item: dp.backward_order_key(item[0]))
-        for _, p in named:
-            if p.dtype != torch.float32:
-                p.data = p.data.float()
-        self._arena = ParamArena(named, self.device) if named else None
+        self._arena = ParamArena(named, self.device, previous=self._arena) if named else None
         self.lm.invalidate()
+        self.lm.drop_training_workspace()
         self.lm.attach_arena(self._arena)
         self.image_prefix.attach_arena(self._arena)
         return self
@@ -248,7 +251,7 @@ class Magma(nn.Module):
             return LMOutput(loss=res[0], logits=res[1], past_key_values=None,
                             hidden_states=tuple(res[2:]) if output_hidden_states else None)
         with torch.no_grad():
-            x = ops.embed_assemble(captions, self.lm.transformer.wte.weight,
+            x = ops.embed_assemble(captions, self.lm.transformer.wte.compute_weight(),
                                    input_embeddings.to(torch.bfloat16).contiguous())
         return self.lm(inputs_embeds=x, labels=labels, output_hidden_states=output_hidden_states)
 

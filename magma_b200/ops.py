@@ -266,6 +266,19 @@ def embed_gather(ids, wte, out=None):
     return out
 
 
+def embed_grad(ids, dy, dwte, accumulate=False):
+    """dwte (fp32 [V, d]) = or += the scatter-add of dy's rows over ids: ids int64 [B, T], dy
+    bf16 [B, T, d] with unit inner stride and any row / batch strides (e.g. dx[:, L:])."""
+    ids = ids.contiguous()
+    B, T = ids.shape
+    V, d = dwte.shape
+    if dy.shape != (B, T, d) or dy.stride(2) != 1:
+        raise ValueError(f"embed_grad: ids {tuple(ids.shape)} / dy {tuple(dy.shape)} / dwte {tuple(dwte.shape)}")
+    check(lib().mb200_embed_grad(_ptr(ids), ids.stride(0), _ptr(dy), dy.stride(1), dy.stride(0), B, T, _ptr(dwte), V, d,
+                                 int(accumulate), _stream()))
+    return dwte
+
+
 def cross_entropy(logits, labels, V, write_grad=False, grad_scale=1.0, dlogits=None, row_loss=None):
     """logits bf16 [B,S,ldv]; returns (loss fp32 [1], dlogits or None). `dlogits` (same strides as logits; may be
     logits itself) receives the gradient instead of a new buffer; `row_loss` (fp32 [B*S]) the per-row losses."""

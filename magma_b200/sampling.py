@@ -99,9 +99,10 @@ def generate(model, embeddings, max_steps: int = 100, temperature: float = 0.7, 
                 nxt_buf = torch.empty(b, dtype=torch.int64, device=dev)
                 V = lm.lm_head.weight.shape[0]
                 eos_i = -1 if eos_token is None else int(eos_token)
+                wte = lm.transformer.wte.compute_weight()  # the bf16 table, also while the embedding trains
 
                 def dev_step():
-                    ops.decode_embed(out, pos_dev, lm.transformer.wte.weight, x_buf)
+                    ops.decode_embed(out, pos_dev, wte, x_buf)
                     lm.decode_step_dev(x_buf, cache, pos_dev, lg_buf)
                     if temperature == 0.0:
                         ops.argmax(lg_buf, V, out=nxt_buf)

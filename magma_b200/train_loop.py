@@ -148,8 +148,13 @@ class B200Engine:
         lm._bwd_chunks = self.chunks
         boundary = self._is_boundary()
         if boundary and self.world > 1:
-            def after(hi, lo):
-                s = arena.slice_for([f"lm.transformer.h.{l}." for l in range(lo, hi)])
+            n_layer = len(lm.transformer.h)
+
+            def after(hi, lo):  # the first chunk also finished the LM head and ln_f, the last one the word embedding
+                prefixes = [f"lm.transformer.h.{l}." for l in range(lo, hi)]
+                prefixes += ["lm.lm_head.", "lm.transformer.ln_f."] if hi == n_layer else []
+                prefixes += ["lm.transformer.wte."] if lo == 0 else []
+                s = arena.slice_for(prefixes)
                 self._allreduce_slice(*s)
             lm._after_chunk = after
         else:

@@ -172,6 +172,7 @@ POINTERS = {
     "attn_decode": ("qkv", "kc", "vc", "out"),
     "patchify": ("img", "patches"),
     "vit_assemble": ("x", "pe", "cls", "pos"),
+    "logits_grad_combine": ("dce", "g", "out"),
 }
 
 
